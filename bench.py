@@ -1,8 +1,9 @@
 #!/usr/bin/env python3
 """
-bench.py -- reads/sec of the adapter-trimming hot path on B200 (BASELINE.json metric).
+bench.py -- reads/sec of the adapter-trimming hot path on H100 (BASELINE.json metric).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--config C]     this repo's CUDA path
+                    [--dump-outputs DIR]                                  + the last step's outputs as .npy
     python bench.py --impl reference ...                                  the reference's CPU path
 
 --config 2 (default, the configuration BASELINE.json's metric is quoted on): 100 M x 150 bp single-end synthetic
@@ -21,10 +22,17 @@ One "step" = one pass of the hot path over the whole per-GPU batch.
   roofline.achieved : algorithmic bytes (190 B/read: 150 sequence + 8 offset + 32 result; 340 with qualities)
            x reads per pass / mean device time of ALL kernels of the trimming pass, measured with CUDA events on the
            launching stream inside the library -- i.e. the whole hot path, not just its largest kernel.
+           roofline.peak is the measured HBM bandwidth in MEASURED_PEAKS.json ("hbm_gbs") when that file is present
+           next to bench.py, else the data-sheet HBM3 bandwidth of the H100 SXM (3.35 TB/s); peak_source says which.
   parity_checked : every 1000th read of the batch is re-computed with the oracle after the timed region and
            compared with the device's record (bit-exact); a mismatch fails the run.
   cpu_baseline : the reference's own compiled hot path (oracle/_ref) on the host cores, bounded sample, rank 0 at
            N=1 only.
+
+--dump-outputs DIR: after the timed steps, rank 0 writes what the last step returned to its caller as float64
+.npy files (match records, quality-trim intervals, statistics vector) for a fixed, seeded sample of the reads, at
+most 64 MB in all.  The reads come from seeded generators, so two builds given the same arguments on the same GPU
+model see the same inputs and can be compared output for output.
 """
 import argparse
 import json
@@ -42,9 +50,10 @@ ERROR_RATE = 0.1
 READ_LEN = 150
 # SURVEY.md section 8(d): sequence + offset + record (+ qualities when quality trimming is fused)
 ALGO_BYTES = {2: READ_LEN + 8 + 32, 3: READ_LEN + 8 + 32, 4: 2 * READ_LEN + 8 + 32, 5: READ_LEN + 8 + 32}
-# ncu --set full, dram__bytes_read.sum + dram__bytes_write.sum of all kernels of one pass divided by the reads
-# (profiles/README.md); measured once per round, not in the timed run.  None: not captured for that configuration.
-NCU_DRAM_BYTES_PER_READ = {2: 259, 3: None, 4: None, 5: 189}     # profiles/r2_launches_config{2_16M,5_25M}.csv
+# NVIDIA's data sheet for the H100 SXM: 3.35 TB/s of HBM3 bandwidth (a peak, not a measured rate); the fallback
+# when no measured peak is present
+HBM_PEAK_GBS = 3350.0
+DUMP_BYTES = 48 << 20                    # --dump-outputs: the sampled records stay well under 64 MB
 DEFAULT_READS = {2: 100_000_000, 3: 100_000_000, 4: 50_000_000, 5: 25_000_000}   # config 4: pairs
 CONFIG_TEXT = {
     2: "one 3' adapter AGATCGGAAGAGC, e=0.1",
@@ -384,6 +393,32 @@ def parity_check(config, mates, results, stride=1000):
     return checked, mismatches
 
 
+def dump_outputs(out_dir, mates, results, all_stats):
+    """
+    The last step's outputs as a caller of DeviceBatch.run_with_statistics receives them, for a fixed seeded sample of
+    the reads (sorted read numbers in read_index.npy): per mate the match records [k, slots, 8] (MATCH_DTYPE field
+    order) and, with quality trimming, the kept intervals [k, 2]; the statistics vector of the step.  float64 holds
+    every int32 field and every count exactly.
+    """
+    import numpy as np
+    import torch
+
+    n = results[0].n_reads
+    per_read = sum(8 * 8 * m["batch"].adapter_set.slots + (16 if m["qt"] is not None else 0) for m in mates)
+    k = min(n, DUMP_BYTES // per_read)
+    pick = np.sort(np.random.default_rng(12345).choice(n, size=k, replace=False))
+    idx = torch.from_numpy(pick).to(results[0].matches.device)
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "read_index.npy"), pick.astype(np.float64))
+    for i, (m, res) in enumerate(zip(mates, results)):
+        slots = m["batch"].adapter_set.slots
+        rec = res.matches.view(n, slots, 8)[idx].cpu().numpy().astype(np.float64)
+        np.save(os.path.join(out_dir, f"r{i + 1}_matches.npy"), rec)
+        if res.qtrim is not None:
+            np.save(os.path.join(out_dir, f"r{i + 1}_qtrim.npy"), res.qtrim[idx].cpu().numpy().astype(np.float64))
+    np.save(os.path.join(out_dir, "statistics.npy"), all_stats.cpu().numpy().astype(np.float64))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -398,6 +433,8 @@ def main():
                     help="weak: --reads per GPU (default); strong: --reads in total, split evenly over the GPUs")
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-cpu", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs (a fixed sample of the reads) to DIR/<name>.npy")
     args = ap.parse_args()
     cfg = args.config
     if not args.reads:
@@ -534,6 +571,8 @@ def main():
     if world > 1:
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
     elapsed_ms = float(t.item())
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, mates, results, all_stats)
     with_adapters = [int(m["stats"][2].item()) for m in mates]
     total_reads_stat = int(sum(int(m["stats"][0].item()) for m in mates))
     reads_per_step = n * reads_per_unit
@@ -615,9 +654,7 @@ def main():
         host_ctx.host_profile(reset=True)
         l0 = host_ctx.launch_count()
         t0 = time.perf_counter()
-        # all --steps, and at least 3e8 reads in the timed region: a step of a small configuration (25 M reads) lasts
-        # 50 ms, which one scheduling hiccup of a host thread would double
-        e2e_steps = max(1, args.steps, -(-300_000_000 // max(1, reads_per_step)))
+        e2e_steps = max(1, args.steps)
         for _ in range(e2e_steps):
             e2e_step()
         barrier()
@@ -670,10 +707,9 @@ def main():
             peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         except Exception:
             pass
-        peak = float(peaks.get("hbm_gbs", 6650.0))
+        peak = float(peaks.get("hbm_gbs", HBM_PEAK_GBS))
         algo = ALGO_BYTES[cfg]
         achieved = algo * reads_per_step / (kern_per_step / 1000.0) / 1e9 if kern_per_step > 0 else None
-        dram = NCU_DRAM_BYTES_PER_READ.get(cfg)
         line = {
             "metric": metric, "value": value, "unit": "reads/s",
             "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
@@ -688,12 +724,9 @@ def main():
             "parity_checked": checked, "parity_mismatches": mismatches,
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s",
                          "frac": (achieved / peak) if achieved else None,
-                         # ncu --set full, dram__bytes_read.sum + dram__bytes_write.sum of the pipeline's kernels
-                         # (profiles/README.md), scaled to the reads of one pass: bytes per launch
-                         "traffic": dram * reads_per_step if dram else None,
-                         "traffic_unit": "bytes per pass (ncu DRAM bytes per read x reads)",
-                         "peak_source": "MEASURED_PEAKS.json hbm_gbs" if peaks else "fallback 6650 GB/s",
-                         "kernel": "all kernels of one trimming pass (per-kernel shares in profiles/)",
+                         "peak_source": ("MEASURED_PEAKS.json hbm_gbs" if "hbm_gbs" in peaks
+                                         else "H100 SXM data sheet, HBM3 3.35 TB/s"),
+                         "kernel": "all kernels of one trimming pass",
                          "kernel_ms_per_launch": kern_per_step,
                          "stage_ms_per_launch": ({k: v / args.steps for k, v in stage_ms.items()} if stage_ms else None),
                          "algorithmic_bytes_per_read": algo},

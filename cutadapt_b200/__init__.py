@@ -1,5 +1,5 @@
 """
-cutadapt_b200 -- B200-native adapter-trimming core with cutadapt's adapter/aligner API.
+cutadapt_b200 -- H100-native adapter-trimming core with cutadapt's adapter/aligner API.
 
 The package mirrors the *hot path* of marcelm/cutadapt and nothing else:
 
@@ -14,7 +14,7 @@ The package mirrors the *hot path* of marcelm/cutadapt and nothing else:
     cutadapt_b200.pipeline        batched per-chunk dispatch    (ref: pipeline.py + modifiers.py
                                                                  AdapterCutter/QualityTrimmer)
 
-All per-read work runs in hand-written sm_100a CUDA kernels behind the C ABI declared in
+All per-read work runs in hand-written sm_90a CUDA kernels behind the C ABI declared in
 include/cutadapt_b200.h (cutadapt_b200/libcutadapt_b200.so, loaded with ctypes).  There is no
 CPU fallback: without the built library and a CUDA device the first call raises.
 """

@@ -305,7 +305,7 @@ extern "C" int cg_ctx_synchronize(cg_ctx *c)
 extern "C" int64_t cg_ctx_launch_count(cg_ctx *c) { return c ? c->launches : 0; }
 
 // Device time of the three stages of the split pipeline (first stage, plan, DP rounds) since the last reset, in ms;
-// only recorded while CUTADAPT_B200_STAGE_TIMES is set in the environment (profiles/, tools).
+// only recorded while CUTADAPT_B200_STAGE_TIMES is set in the environment (tools).
 extern "C" int cg_ctx_stage_times(cg_ctx *c, double *out3, int reset)
 {
     if (!c || !out3) return fail(CG_EINVAL, "cg_ctx_stage_times: NULL argument");

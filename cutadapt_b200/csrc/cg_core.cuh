@@ -851,7 +851,7 @@ CG_HD uint32_t plane_load(PlaneState<W> &st, const uint8_t *base, int off0)
 // one chain step: acc = plane (first character of a chain) or (acc << 1) & plane
 #ifndef CG_CHAIN_IMAD
 #define CG_CHAIN_IMAD 0             // words of the accumulator whose shift runs on the multiply pipe (bit b = word b);
-                                    // measured on B200: 0xFF is 2 % SLOWER than funnel shifts (IMAD.WIDE issues at half
+                                    // measured: 0xFF was SLOWER than funnel shifts (IMAD.WIDE issues at half
                                     // rate), so the default keeps the shifts on the ALU pipe
 #endif
 template <int W>
@@ -1696,8 +1696,8 @@ CG_HD bool loc_state_result(const LocState &st, int *out6)
 // this call covers the read's last run).
 #ifndef CG_RUN_BAND
 #define CG_RUN_BAND 0       // 1: the DP runs skip the rows outside the band (run_band_d).  Exact (tests/hostsim is built
-                            // with it: test_banded_dp_runs_on_crowded_reads) but measured SLOWER on B200: DP rounds of
-                            // config 2 1.52 -> 1.56 ms, of config 4 (33-row adapters) 16.6 -> 18.7 ms -- the four-row
+                            // with it: test_banded_dp_runs_on_crowded_reads) but measured SLOWER: DP rounds of
+                            // configs 2 and 4 (33-row adapters) -- the four-row
                             // chunks above the band are few once the Ukkonen bound has cut the column, and the extra
                             // live values push the 48-row kernel into spills
 #endif

@@ -826,7 +826,7 @@ cudaError_t cg_launch_fastq_gather(const uint8_t *d_buf, const CgFastqRecord *d_
 {
     if (n_records <= 0) return cudaSuccess;
     long long grid = (n_records + 7) / 8;
-    if (grid > 148 * 16) grid = 148 * 16;
+    grid = cg_grid_cap(grid, 16);
     fq_gather_kernel<<<(unsigned)grid, 256, 0, st>>>(d_buf, d_rec, d_offsets, n_records, d_seq, d_qual, rc);
     return cudaGetLastError();
 }
@@ -846,7 +846,7 @@ cudaError_t cg_launch_fastq_revcomp_commit(uint8_t *d_buf, CgFastqRecord *d_rec,
 {
     if (n_records <= 0) return cudaSuccess;
     long long grid = (n_records + 7) / 8;
-    if (grid > 148 * 16) grid = 148 * 16;
+    grid = cg_grid_cap(grid, 16);
     fq_revcomp_commit_kernel<<<(unsigned)grid, 256, 0, st>>>(d_buf, d_rec, d_seq_len, d_origin, n_records, d_matches,
                                                              d_matches_rc, per_read, d_is_rc, d_counters);
     return cudaGetLastError();
@@ -898,7 +898,7 @@ cudaError_t cg_launch_fastq_write(const uint8_t *d_buf, const CgFastqRecord *d_r
 {
     if (n_records <= 0) return cudaSuccess;
     long long grid = (n_records + 7) / 8;
-    if (grid > 148 * 16) grid = 148 * 16;
+    grid = cg_grid_cap(grid, 16);
     fq_write_kernel<<<(unsigned)grid, 256, 0, st>>>(d_buf, d_rec, d_interval, d_out_off, d_out_len, n_records, d_out, action,
                                                     d_keep_interval, d_mask, rc_suffix);
     return cudaGetLastError();
@@ -955,7 +955,7 @@ cudaError_t cg_launch_fastq_info(int phase, const uint8_t *d_buf, const CgFastqR
         fq_info_count_kernel<<<(unsigned)((n_records + 127) / 128), 128, 0, st>>>(a, n_records, d_row_bytes);
     } else {
         long long grid = (n_records + 7) / 8;
-        if (grid > 148 * 16) grid = 148 * 16;
+        grid = cg_grid_cap(grid, 16);
         fq_info_write_kernel<<<(unsigned)grid, 256, 0, st>>>(a, n_records, d_row_off, d_out);
     }
     return cudaGetLastError();

@@ -1,4 +1,4 @@
-// cg_kernels.cu -- sm_100a kernels of the adapter-trimming hot path.
+// cg_kernels.cu -- sm_90a (H100) kernels of the adapter-trimming hot path.
 //
 // cg_trim_fast_kernel   the fused pass: quality trim -> k-mer prefilter -> banded DP ->
 //                       best-adapter selection, one lane per read, persistent CTAs.
@@ -13,6 +13,8 @@
 //                       reads straight from HBM, DP columns in an HBM scratch.
 // plus the stand-alone batched KmerFinder / quality_trim_index kernels and the statistics
 // reduction.
+#include <atomic>
+
 #include "cg_kernels.cuh"
 #include "cg_device.cuh"
 #include "cg_pscan.cuh"   // (ScanSmem, cg_pscan_body)
@@ -1221,13 +1223,25 @@ __global__ void __launch_bounds__(CG_NT) cg_trim_listed_kernel(const CgKernelArg
     }
 }
 
+int cg_device_sm_count()
+{
+    // queried once per device (0: not yet); a launch only asks which device is current
+    static std::atomic<int> cached[64];
+    int dev = 0, sms = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess) return 1;
+    if (dev >= 0 && dev < 64 && (sms = cached[dev].load(std::memory_order_relaxed)) > 0) return sms;
+    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms < 1) return 1;
+    if (dev >= 0 && dev < 64) cached[dev].store(sms, std::memory_order_relaxed);
+    return sms;
+}
+
 cudaError_t cg_launch_index(const CgKernelArgs &a, int grid, cudaStream_t st)
 {
     cg_index_kernel<<<grid, CG_NT, 0, st>>>(a);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return e;
     // (few reads are listed: a fixed small grid, grid-stride)
-    cg_trim_listed_kernel<<<148, CG_NT, 0, st>>>(a);
+    cg_trim_listed_kernel<<<cg_device_sm_count(), CG_NT, 0, st>>>(a);
     return cudaGetLastError();
 }
 
@@ -1285,7 +1299,7 @@ cudaError_t cg_launch_kmers_present(const CgEntry *d_entries, int n_entries, con
 {
     const int block = 128;
     long long grid = (n_reads + block - 1) / block;
-    if (grid > 148 * 16) grid = 148 * 16;
+    grid = cg_grid_cap(grid, 16);
     if (grid < 1) grid = 1;
     cg_kmers_present_kernel<<<(int)grid, block, 0, st>>>(d_entries, n_entries, d_masks, d_seq, d_offsets,
                                                          n_reads, d_out, d_err);
@@ -1313,7 +1327,7 @@ cudaError_t cg_launch_quality_trim(const uint8_t *d_qual, const int64_t *d_offse
 {
     const int block = 128;
     long long grid = (n_reads + block - 1) / block;
-    if (grid > 148 * 16) grid = 148 * 16;
+    grid = cg_grid_cap(grid, 16);
     if (grid < 1) grid = 1;
     cg_quality_trim_kernel<<<(int)grid, block, 0, st>>>(d_qual, d_offsets, n_reads, cutoff_front,
                                                         cutoff_back, base, d_out);
@@ -1363,7 +1377,7 @@ cudaError_t cg_launch_expected_errors(const uint8_t *d_qual, const int64_t *d_of
 {
     const int block = 128;
     long long grid = (n_reads + block - 1) / block;
-    if (grid > 148 * 16) grid = 148 * 16;
+    grid = cg_grid_cap(grid, 16);
     if (grid < 1) grid = 1;
     cg_expected_errors_kernel<<<(int)grid, block, 0, st>>>(d_qual, d_offsets, n_reads, base, d_table, d_out);
     return cudaGetLastError();
@@ -1373,7 +1387,7 @@ cudaError_t cg_launch_nextseq_trim(const uint8_t *d_seq, const uint8_t *d_qual, 
 {
     const int block = 128;
     long long grid = (n_reads + block - 1) / block;
-    if (grid > 148 * 16) grid = 148 * 16;
+    grid = cg_grid_cap(grid, 16);
     if (grid < 1) grid = 1;
     cg_nextseq_trim_kernel<<<(int)grid, block, 0, st>>>(d_seq, d_qual, d_offsets, n_reads, cutoff, base, d_out);
     return cudaGetLastError();
@@ -1383,7 +1397,7 @@ cudaError_t cg_launch_poly_a_trim(const uint8_t *d_seq, const int64_t *d_offsets
 {
     const int block = 128;
     long long grid = (n_reads + block - 1) / block;
-    if (grid > 148 * 16) grid = 148 * 16;
+    grid = cg_grid_cap(grid, 16);
     if (grid < 1) grid = 1;
     cg_poly_a_trim_kernel<<<(int)grid, block, 0, st>>>(d_seq, d_offsets, n_reads, revcomp, d_out, nullptr);
     return cudaGetLastError();
@@ -1454,7 +1468,7 @@ cudaError_t cg_launch_unpack3(const uint8_t *d_packed, long long packed_bytes, u
     if (n_vec > 0) {
         const int block = 256;
         long long grid = (n_vec + block - 1) / block;
-        if (grid > 148 * 8) grid = 148 * 8;
+        grid = cg_grid_cap(grid, 8);
         cg_unpack3_kernel<<<(int)grid, block, 0, st>>>((const uint4 *)d_packed, (uint4 *)d_out, n_vec);
         cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) return e;
@@ -1489,7 +1503,7 @@ cudaError_t cg_launch_max_len(const int64_t *d_offsets, long long n_reads, int *
 {
     const int block = 256;
     long long grid = (n_reads + block - 1) / block;
-    if (grid > 148 * 8) grid = 148 * 8;
+    grid = cg_grid_cap(grid, 8);
     if (grid < 1) grid = 1;
     cg_max_len_kernel<<<(int)grid, block, 0, st>>>(d_offsets, n_reads, d_out);
     return cudaGetLastError();
@@ -1566,7 +1580,7 @@ cudaError_t cg_launch_stats(const uint8_t *d_seq, const int64_t *d_offsets, long
 {
     const int block = 256;
     long long grid = (n_reads + block - 1) / block;
-    if (grid > 148 * 8) grid = 148 * 8;
+    grid = cg_grid_cap(grid, 8);
     if (grid < 1) grid = 1;
     const size_t hist_bytes = (size_t)(cg_stats_total(n_adapters, max_len, kmax) - CG_STATS_SCALARS) * sizeof(unsigned int);
     const size_t len_bytes = (size_t)(max_len + 1) * sizeof(unsigned int);

@@ -7,6 +7,14 @@
 
 #include "cg_args.h"
 
+// SMs of the current device: the grid-stride launches are sized in blocks per SM
+int cg_device_sm_count();
+static inline long long cg_grid_cap(long long grid, int blocks_per_sm)
+{
+    const long long cap = (long long)blocks_per_sm * cg_device_sm_count();
+    return grid > cap ? cap : grid;
+}
+
 // Multi-pass schedule (several adapters, one round): every component adapter runs as its own pass into a
 // scratch array of records; cg_select_kernel then applies MultipleAdapters.match_to / LinkedAdapter.match_to
 // to the per-adapter results.

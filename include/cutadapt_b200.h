@@ -1,5 +1,5 @@
 /*
- * cutadapt_b200.h -- C ABI of the B200-native adapter-trimming core.
+ * cutadapt_b200.h -- C ABI of the H100-native adapter-trimming core.
  *
  * Drop-in boundary for ONE hot path of marcelm/cutadapt:
  *     Adapter.match_to -> KmerFinder.kmers_present -> Aligner.locate   (+ quality_trim_index)

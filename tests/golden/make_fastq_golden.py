@@ -1,19 +1,19 @@
 #!/usr/bin/env python3
 """
 Copies the FASTQ known-answer cases of the reference's own command-line tests
-(/root/reference/tests/test_commandline.py: run(params, expected, input) compares cutadapt's output
+($CUTADAPT_REFERENCE/tests/test_commandline.py: run(params, expected, input) compares cutadapt's output
 with tests/cut/<expected>) into tests/golden/fastq_kat.json.gz: the (<case>.in.fastq, <case>.out.fastq) pairs as
 text plus the case lists, which restate each command line in terms of cutadapt_b200's FASTQ entry point.
 These are test vectors (inputs and expected outputs), not source code.
 
-    python tests/golden/make_fastq_golden.py      (needs /root/reference; run once, results committed)
+    python tests/golden/make_fastq_golden.py      (needs $CUTADAPT_REFERENCE, a checkout of the reference; run once, results committed)
 """
 import gzip
 import json
 import os
 import shutil
 
-REF = "/root/reference/tests"
+REF = os.path.join(os.environ.get("CUTADAPT_REFERENCE", ""), "tests")
 OUT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "fastq_kat.json.gz")
 FILES = {}     # fixture name -> content (latin-1 text)
 

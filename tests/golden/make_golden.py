@@ -2,14 +2,14 @@
 """
 Generate the golden fixtures under tests/golden/ from the REFERENCE ITSELF.
 
-Run in the build container only (needs /root/reference, builds oracle/_ref on the fly):
+Needs $CUTADAPT_REFERENCE, a checkout of the reference (builds oracle/_ref on the fly):
 
     python tests/golden/make_golden.py
 
 Everything written here is input/output pairs of the reference's own compiled code
 (cutadapt._align, _kmer_finder, qualtrim, kmer_heuristic, adapters) plus the per-read
 coordinates of the reference's golden files tests/cut/illumina.info.txt and
-illumina5.info.txt.  The fixtures travel to the GPU box, where /root/reference does not exist.
+illumina5.info.txt.  The tests read only the fixtures, never the reference.
 Seeds are fixed; re-running reproduces the files byte for byte.
 """
 import gzip
@@ -32,7 +32,7 @@ from cutadapt.qualtrim import quality_trim_index, nextseq_trim_index, poly_a_tri
 from cutadapt import adapters as RA  # noqa: E402
 from cutadapt import _match_tables as RT  # noqa: E402
 
-REF_TESTS = "/root/reference/tests"
+REF_TESTS = os.path.join(os.environ.get("CUTADAPT_REFERENCE", ""), "tests")
 
 
 def dump(name, obj):

@@ -165,7 +165,7 @@ extern "C" int hs_plane_classify(const cg_adapter_desc *adapters, int n_adapters
 }
 
 // The run-time specialisation of the first stage (cg_jit.cpp): generate the translation unit for this adapter set
-// and compile it with NVRTC for sm_100a (no device needed).  Returns the cubin size, 0 if the set has no plane
+// and compile it with NVRTC for sm_90a (no device needed).  Returns the cubin size, 0 if the set has no plane
 // program, -1 if the compilation failed (log says why), -2 if libnvrtc is not there.
 extern "C" long hs_jit_compile(const cg_adapter_desc *adapters, int n_adapters, const cg_group_desc *groups, int n_groups,
                                int plane_words, int has_qual, char *src, long src_cap, char *log, long log_cap)

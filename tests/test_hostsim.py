@@ -613,7 +613,7 @@ def test_fastq_record_table_of_the_device_functions():
 
 def test_first_stage_specialisation_compiles_without_a_device():
     """cg_jit.cpp: the translation unit generated for an adapter set (straight-line plane_chain_step / plane_emit calls)
-    goes through NVRTC for sm_100a here, for 5- and 8-word planes, with and without qualities; a set without a plane
+    goes through NVRTC for sm_90a here, for 5- and 8-word planes, with and without qualities; a set without a plane
     program (wildcards) yields no source."""
     import cutadapt_b200.adapters as PA
     from util import hostsim_jit_compile, spec_of

@@ -16,22 +16,91 @@ def golden(name):
         return json.load(f)
 
 
-def reference_or_none():
-    """The reference's compiled hot path (oracle/_ref), if it has been built and travels along."""
-    import sys
+# ---- answers of the reference on the tests' own inputs (tests/golden/make_reference_golden.py) ---------------------
 
-    ref_root = os.path.join(ROOT, "oracle", "_ref")
-    if not os.path.isdir(os.path.join(ref_root, "cutadapt")):
-        return None
-    if ref_root not in sys.path:
-        sys.path.insert(0, ref_root)
-    try:
-        import cutadapt.adapters  # noqa: F401
-        import cutadapt
+ANSWER_CHUNK = 1000
 
-        return cutadapt
-    except Exception:
-        return None
+
+def canonical(x):
+    """JSON-ready form of an answer: tuples become lists, numpy scalars Python numbers."""
+    if isinstance(x, (list, tuple)):
+        return [canonical(v) for v in x]
+    if isinstance(x, dict):
+        return {str(k): canonical(v) for k, v in x.items()}
+    if isinstance(x, np.generic):
+        return x.item()
+    return x
+
+
+def answer_digests(answers, chunk=ANSWER_CHUNK):
+    """SHA-256 (first 16 hex digits) of the canonical JSON of every `chunk` consecutive answers."""
+    import hashlib
+
+    out = []
+    for c0 in range(0, len(answers), chunk):
+        text = json.dumps(canonical(list(answers[c0:c0 + chunk])), separators=(",", ":"))
+        out.append(hashlib.sha256(text.encode()).hexdigest()[:16])
+    return out
+
+
+def reference_answers(name):
+    """What the reference answered for test input `name` (tests/golden/reference_kat.json.gz)."""
+    return golden("reference_kat.json.gz")[name]
+
+
+def assert_reference_answers(name, answers):
+    """`answers` (one per input, in order) equal the reference's, compared chunk by chunk through their digests."""
+    want = reference_answers(name)
+    got = answer_digests(answers)
+    assert len(got) == len(want), (name, len(answers))
+    bad = [i for i, (a, b) in enumerate(zip(got, want)) if a != b]
+    assert not bad, f"{name}: answers {bad[0] * ANSWER_CHUNK}..{(bad[0] + 1) * ANSWER_CHUNK - 1} differ from the reference's"
+
+
+def random_locate_cases():
+    """Random Aligner.locate / quality_trim_index inputs: (aligner arguments, 4 queries, qualities) per case."""
+    rng = random.Random(77)
+    cases = []
+    for _ in range(3000):
+        alpha = rng.choice(["ACGT", "AC", "ACGTN", "ACGTacgtNn", "ACGTRYKMN"])
+        m = rng.randint(1, 20)
+        ref = "".join(rng.choice(alpha) for _ in range(m))
+        wr, wq = rng.random() < 0.3, rng.random() < 0.2
+        if wr and set(ref.upper()) <= {"N"}:
+            continue
+        rate = rng.choice([0, 0.1, 0.2, 0.34, 0.5])
+        flags, ic, mo = rng.randint(0, 15), rng.choice([1, 1, 100000, 3]), rng.randint(1, 4)
+        queries = []
+        for _ in range(4):
+            q = "".join(rng.choice(alpha) for _ in range(rng.randint(0, 40)))
+            if rng.random() < 0.5:
+                pos = rng.randint(0, len(q))
+                q = q[:pos] + ref[rng.randint(0, m // 2):] + q[pos:]
+            queries.append(q)
+        qs = "".join(chr(33 + rng.choice([0, 2, 10, 20, 30, 40])) for _ in range(rng.randint(0, 50)))
+        cases.append(((ref, rate, flags, wr, wq, ic, mo), queries, qs))
+    return cases
+
+
+def index_test_reads():
+    """3000 config-5 reads, every 50th with an N in the barcode (the index test of test_oracle.py)."""
+    from cutadapt_b200.configs import make_config_batch
+
+    seq = make_config_batch(5, 3000, seed=77)["seq"]
+    seq[::50, 3] = ord("N")
+    return seq
+
+
+def end_statistics_answer(stats):
+    """An adapter's end statistics (errors, adjacent bases per end) in a form that compares across implementations."""
+    out = []
+    for e in stats.end_statistics():
+        if e is None:
+            out.append(None)
+        else:
+            out.append([sorted([int(k), sorted(dict(v).items())] for k, v in e.errors.items() if v),
+                        sorted(dict(e.adjacent_bases).items())])
+    return canonical(out)
 
 
 # ---- hostsim: the device functions compiled for the host (tests only) ------------------------
@@ -329,7 +398,7 @@ def adapter_from_spec(spec, adapter_type, name=None, **params):
 
 def hostsim_jit_compile(spec, plane_words=5, has_qual=False):
     """(cubin size or error code, generated source, NVRTC log) of the run-time specialisation of the first stage
-    (cg_jit.cpp) for this adapter set -- NVRTC compiles for sm_100a without a device."""
+    (cg_jit.cpp) for this adapter set -- NVRTC compiles for sm_90a without a device."""
     lib = hostsim_lib()
     lib.hs_jit_compile.restype = C.c_long
     lib.hs_jit_compile.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_char_p, C.c_long,

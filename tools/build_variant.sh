@@ -5,7 +5,7 @@ set -e
 cd "$(dirname "$0")/.."
 name=$1; shift
 mkdir -p build_variants
-/usr/local/cuda/bin/nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo -O3 -std=c++17 -Xcompiler -fPIC -shared "$@" \
+/usr/local/cuda/bin/nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -std=c++17 -Xcompiler -fPIC -shared "$@" \
   -Xcompiler -pthread -o build_variants/lib_$name.so cutadapt_b200/csrc/cg_kernels.cu cutadapt_b200/csrc/cg_fastq.cu \
   cutadapt_b200/csrc/cg_api.cu cutadapt_b200/csrc/cg_setbuild.cpp cutadapt_b200/csrc/cg_host_algos.cpp \
   cutadapt_b200/csrc/cg_hostpack.cpp cutadapt_b200/csrc/cg_jit.cpp -lpthread -ldl
