@@ -34,6 +34,9 @@ CG_REMOVE_AUTO = 2
 CG_GROUP_SINGLE = 0
 CG_GROUP_LINKED = 1
 CG_GROUP_INDEXED = 2
+CG_FORMAT_FASTQ = 0              # cg_fastq_params.format: FASTQ in, FASTQ out
+CG_FORMAT_FASTA = 1              # FASTA in, FASTA out
+CG_FORMAT_FASTQ_TO_FASTA = 2     # FASTQ in, FASTA out
 
 
 class cg_kmer_entry(C.Structure):
@@ -122,7 +125,8 @@ class cg_fastq_params(C.Structure):
         ("discard_casava", C.c_int32),
         ("action", C.c_int32),
         ("revcomp", C.c_int32),
-        ("reserved", C.c_int32 * 3),
+        ("format", C.c_int32),
+        ("reserved", C.c_int32 * 2),
     ]
 
 

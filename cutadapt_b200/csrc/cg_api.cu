@@ -121,6 +121,9 @@ struct FastqSlot {
     DevBuf<unsigned long long> d_scan;
     DevBuf<cg_match_rec> d_matches, d_matches_rc;
     DevBuf<uint8_t> d_isrc;
+    DevBuf<uint8_t> d_norm;                     // FASTA: the normalised chunk (swapped into d_in once built)
+    DevBuf<int32_t> d_faline;                   // FASTA: bytes kept and header flag per line, first header line
+    DevBuf<int64_t> d_faoff;                    // FASTA: their exclusive scans
     unsigned long long *d_counters = nullptr;   // [0] newline total, [1..] CG_FQ_COUNTERS
     int *d_err = nullptr;                       // [0] code, [1] record
     PinBuf<uint8_t> h_in, h_out;
@@ -278,6 +281,7 @@ extern "C" int cg_ctx_destroy(cg_ctx *c)
         f.d_offs.release(); f.d_outoff.release(); f.d_scan.release(); f.d_matches.release(); f.d_matches_rc.release();
         f.d_isrc.release(); f.d_dest.release(); f.d_pairkey.release(); f.d_destkeep.release(); f.d_origin.release();
         f.d_names.release(); f.d_infoout.release(); f.d_nameoff.release(); f.d_inforow.release(); f.d_infooff.release();
+        f.d_norm.release(); f.d_faline.release(); f.d_faoff.release();
         f.h_in.release(); f.h_out.release(); f.h_counters.release();
         if (f.d_counters) cudaFree(f.d_counters);
         if (f.d_err) cudaFree(f.d_err);
@@ -1588,6 +1592,11 @@ static void parallel_copy(cg_ctx *c, void *dst, const void *src, size_t n)
 
 static int fastq_format_error(const int err[2])
 {
+    if (err[0] == CG_FA_ERR_BEFORE_HEADER || err[0] == CG_FA_ERR_LATE_COMMENT)
+        return fail(CG_EINVAL, std::string("FASTA format error in line ") + std::to_string((long long)(unsigned)err[1] + 1) +
+                                   (err[0] == CG_FA_ERR_BEFORE_HEADER
+                                        ? ": expected '>' at the beginning of a record"
+                                        : ": a '#' comment line after the first record"));
     static const char *what[] = {"", "a record does not start with '@'", "the third line of a record does not start with '+'",
                                  "sequence and qualities differ in length", "invalid quality value",
                                  "sequence descriptions don't match (the second one must be empty or equal to the first)"};
@@ -1647,6 +1656,9 @@ struct FqStage {
     int max_len = 0;                     // longest packed read
     const uint8_t *d_is_rc = nullptr;    // --revcomp: the record was replaced by its reverse complement
     int rc_suffix = 0;                   // ... and gets " rc" appended to its name
+    int format = CG_FORMAT_FASTQ;        // cg_fastq_params.format
+    bool has_qual() const { return format != CG_FORMAT_FASTA; }
+    bool fasta_out() const { return format != CG_FORMAT_FASTQ; }
 };
 
 static int fastq_enabled_filters(const cg_fastq_params *fp)
@@ -1656,10 +1668,61 @@ static int fastq_enabled_filters(const cg_fastq_params *fp)
            (fp->discard_untrimmed ? 64 : 0);
 }
 
+// FASTA chunk (format 1) -> normalised chunk in f.d_in + record table: line classes, two scans, scatter, records.
+// Returns the number of records in *n_records; reports a format error naming the first bad line.
+static int fasta_stage_normalise(cg_ctx *c, FastqSlot &f, const cg_fastq_params *fp, long long n_lines, cudaStream_t st,
+                                 FqStage &g, long long *n_records)
+{
+    *n_records = 0;
+    const int64_t n_bytes = f.n_bytes;
+    int rc;
+    if ((rc = f.d_nl.ensure((size_t)g.n_nl + 1)) != CG_OK) return rc;
+    if ((rc = f.d_faline.ensure((size_t)n_lines * 2 + 1)) != CG_OK) return rc;
+    if ((rc = f.d_faoff.ensure((size_t)n_lines * 2 + 2)) != CG_OK) return rc;
+    if ((rc = f.d_scan.ensure((size_t)cg_scan_tiles(n_lines) + 1)) != CG_OK) return rc;
+    int32_t *d_keep = f.d_faline.p, *d_hdr = f.d_faline.p + n_lines, *d_first = f.d_faline.p + 2 * n_lines;
+    int64_t *d_off = f.d_faoff.p, *d_idx = f.d_faoff.p + n_lines + 1;
+    const int first_init = 0x7FFFFFFF;
+    CU(cudaMemcpyAsync(d_first, &first_init, sizeof first_init, cudaMemcpyHostToDevice, st));
+    CU(cg_launch_fastq_index(f.d_in.p, n_bytes, f.d_tiles.p, nullptr, f.d_nl.p, 1, st));
+    CU(cg_launch_fasta_classify(f.d_in.p, n_bytes, f.d_nl.p, g.n_nl, n_lines, d_keep, d_hdr, d_first, st));
+    CU(cg_launch_scan_i32(d_keep, n_lines, f.d_scan.p, d_off, st));
+    CU(cg_launch_scan_i32(d_hdr, n_lines, f.d_scan.p, d_idx, st));
+    c->launches += 8;
+    int64_t sizes[2];                           // bytes of the normalised chunk, records
+    CU(cudaMemcpyAsync(&sizes[0], d_off + n_lines, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(&sizes[1], d_idx + n_lines, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    const long long n_norm = sizes[0], n = sizes[1];
+    if ((rc = f.d_norm.ensure((size_t)n_norm + 64)) != CG_OK) return rc;
+    if ((rc = f.d_rec.ensure((size_t)n + 1)) != CG_OK) return rc;
+    if ((rc = f.d_len.ensure((size_t)n + 1)) != CG_OK) return rc;
+    if ((rc = f.d_origin.ensure((size_t)n * 2 + 2)) != CG_OK) return rc;
+    CU(cg_launch_fasta_scatter(f.d_in.p, n_bytes, f.d_nl.p, g.n_nl, n_lines, d_off, d_idx, d_first, f.d_norm.p, f.d_rec.p,
+                               f.d_err, st));
+    CU(cg_launch_fasta_records(f.d_rec.p, n, n_norm, fp->cut_front, fp->cut_back, f.d_len.p, f.d_origin.p, f.d_counters + 1,
+                               st));
+    c->launches += 2;
+    int fa_err[2];
+    CU(cudaMemcpyAsync(fa_err, f.d_err, sizeof fa_err, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    if (fa_err[0]) return fastq_format_error(fa_err);
+    std::swap(f.d_in, f.d_norm);                // every later kernel reads the normalised chunk
+    f.n_bytes = n_norm;
+    *n_records = n;
+    return CG_OK;
+}
+
 // index the chunk, build the record table, run the modifiers (trimming pass included), evaluate the filters
 // Line table -> record table of one mate (format checks, -u, bases read); sizes every per-record buffer.
 static int fastq_stage_records(cg_ctx *c, FastqSlot &f, const cg_fastq_params *fp, bool has_set, cudaStream_t st, FqStage &g)
 {
+    if (fp->format < CG_FORMAT_FASTQ || fp->format > CG_FORMAT_FASTQ_TO_FASTA)
+        return fail(CG_EINVAL, "cg_fastq: format must be 0 (FASTQ), 1 (FASTA) or 2 (FASTQ in, FASTA out)");
+    if (fp->format == CG_FORMAT_FASTA &&
+        (fp->trim.quality_trim || fp->trim.nextseq_trim || fp->max_expected_errors >= 0.0))
+        return fail(CG_EINVAL, "FASTA input has no qualities: quality trimming, --nextseq-trim and --max-ee need FASTQ");
+    g.format = fp->format;
     CU(cudaStreamSynchronize(f.stream));        // upload + newline count of this slot
     const int64_t n_bytes = f.n_bytes;
     g.n_nl = (long long)f.h_counters.p[0];
@@ -1670,10 +1733,16 @@ static int fastq_stage_records(cg_ctx *c, FastqSlot &f, const cg_fastq_params *f
         CU(cudaStreamSynchronize(st));
         if (last != '\n') n_lines += 1;
     }
-    if (n_lines % 4 != 0)
+    const bool fasta = fp->format == CG_FORMAT_FASTA;
+    if (!fasta && n_lines % 4 != 0)
         return fail(CG_EINVAL, "FASTQ chunk does not consist of complete 4-line records (" + std::to_string(n_lines) +
                                    " lines)");
-    const long long n = g.n = n_lines / 4;
+    long long n_fasta = 0;
+    if (fasta && n_lines > 0) {
+        int rc = fasta_stage_normalise(c, f, fp, n_lines, st, g, &n_fasta);
+        if (rc != CG_OK) return rc;
+    }
+    const long long n = g.n = fasta ? n_fasta : n_lines / 4;
     if (n == 0) return CG_OK;
     const cg_params *p = &fp->trim;
     g.want_q = p->quality_trim != 0 || p->nextseq_trim != 0;
@@ -1696,10 +1765,12 @@ static int fastq_stage_records(cg_ctx *c, FastqSlot &f, const cg_fastq_params *f
     if ((rc = f.d_outoff.ensure((size_t)n + 1)) != CG_OK) return rc;
     if ((rc = f.d_scan.ensure((size_t)cg_scan_tiles(n) + 1)) != CG_OK) return rc;
     if (g.want_q && (rc = f.d_qtrim.ensure((size_t)n * 2)) != CG_OK) return rc;
-    CU(cg_launch_fastq_index(f.d_in.p, n_bytes, f.d_tiles.p, nullptr, f.d_nl.p, 1, st));
-    CU(cg_launch_fastq_records(f.d_in.p, n_bytes, f.d_nl.p, g.n_nl, n, fp->cut_front, fp->cut_back, f.d_rec.p, f.d_len.p,
-                               f.d_origin.p, f.d_counters + 1, f.d_err, st));
-    c->launches += 2;
+    if (!fasta) {
+        CU(cg_launch_fastq_index(f.d_in.p, n_bytes, f.d_tiles.p, nullptr, f.d_nl.p, 1, st));
+        CU(cg_launch_fastq_records(f.d_in.p, n_bytes, f.d_nl.p, g.n_nl, n, fp->cut_front, fp->cut_back, f.d_rec.p, f.d_len.p,
+                                   f.d_origin.p, f.d_counters + 1, f.d_err, st));
+        c->launches += 2;
+    }
     g.d_qtrim = g.want_q ? f.d_qtrim.p : nullptr;
     return CG_OK;
 }
@@ -1803,7 +1874,7 @@ static int fastq_stage_evaluate(cg_ctx *c, FastqSlot &f, const cg_adapterset *s,
         rc = launch_trim(c, s, f.d_seq.p, nullptr, f.d_offs.p, n, g.max_len, &pt, f.d_matches_rc.p, nullptr, st, true);
         if (rc != CG_OK) return rc;
         CU(cg_launch_fastq_revcomp_commit(f.d_in.p, f.d_rec.p, f.d_len.p, f.d_origin.p, n, f.d_matches.p, f.d_matches_rc.p, (int)per_read,
-                                          f.d_isrc.p, f.d_counters + 1, st));
+                                          f.d_isrc.p, f.d_counters + 1, st, g.has_qual() ? 1 : 0));
         c->launches += 1;
         g.d_matches = f.d_matches.p;
         g.d_is_rc = f.d_isrc.p;
@@ -1905,7 +1976,7 @@ static int fastq_stage_output(cg_ctx *c, FastqSlot &f, const FqStage &g, cudaStr
         if (!out) return fail(CG_EINVAL, "cg_fastq_collect: out is NULL");
         if ((rc = f.d_out.ensure((size_t)total + 64)) != CG_OK) return rc;
         CU(cg_launch_fastq_write(f.d_in.p, f.d_rec.p, f.d_interval.p, f.d_outoff.p, f.d_outlen.p, n, f.d_out.p, g.action,
-                                 f.d_keep.p, f.d_mask.p, g.rc_suffix, st));
+                                 f.d_keep.p, f.d_mask.p, g.rc_suffix, st, g.fasta_out() ? 1 : 0));
         c->launches += 1;
         if (is_pinned(out)) {
             CU(cudaMemcpyAsync(out, f.d_out.p, (size_t)total, cudaMemcpyDeviceToHost, st));
@@ -1948,7 +2019,7 @@ static int fastq_stage_info(cg_ctx *c, FastqSlot &f, const FqStage &g, const cg_
     const int upper = g.action == CG_FQ_ACTION_LOWERCASE;
     CU(cg_launch_fastq_info(0, f.d_in.p, f.d_rec.p, f.d_origin.p, f.d_interval.p, f.d_mask.p, g.d_matches, g.times, g.slots,
                             f.d_names.p, f.d_nameoff.p, fp->revcomp != 0, g.rc_suffix, upper, n, f.d_inforow.p, nullptr, nullptr,
-                            st, info.kind, g.d_qtrim, f.d_len.p));
+                            st, info.kind, g.d_qtrim, f.d_len.p, g.has_qual() ? 1 : 0));
     CU(cg_launch_scan_i32(f.d_inforow.p, n, f.d_scan.p, f.d_infooff.p, st));
     long long total = 0;
     CU(cudaMemcpyAsync(&total, f.d_infooff.p + n, sizeof total, cudaMemcpyDeviceToHost, st));
@@ -1961,7 +2032,7 @@ static int fastq_stage_info(cg_ctx *c, FastqSlot &f, const FqStage &g, const cg_
     if ((rc = f.d_infoout.ensure((size_t)total + 64)) != CG_OK) return rc;
     CU(cg_launch_fastq_info(1, f.d_in.p, f.d_rec.p, f.d_origin.p, f.d_interval.p, f.d_mask.p, g.d_matches, g.times, g.slots,
                             f.d_names.p, f.d_nameoff.p, fp->revcomp != 0, g.rc_suffix, upper, n, nullptr, f.d_infooff.p,
-                            f.d_infoout.p, st, info.kind, g.d_qtrim, f.d_len.p));
+                            f.d_infoout.p, st, info.kind, g.d_qtrim, f.d_len.p, g.has_qual() ? 1 : 0));
     c->launches += 1;
     CU(cudaMemcpyAsync(info.out, f.d_infoout.p, (size_t)total, cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
@@ -1987,7 +2058,7 @@ static int fastq_collect_impl(cg_ctx *c, int32_t slot, const cg_adapterset *s, c
     if (dm && (rc = fastq_stage_route(c, f, nullptr, g.n, *dm, f.stream)) != CG_OK) return rc;
     CU(cg_launch_fastq_finish(g.n, f.d_rec.p, f.d_interval.p, f.d_mask.p, fastq_enabled_filters(fp), f.d_outlen.p,
                               f.d_counters + 1, nullptr, nullptr, nullptr, 0, nullptr, nullptr, 0, 0, g.rc_suffix,
-                              dm ? dm->d_dest : nullptr, dm ? dm->d_dest_keep : nullptr, f.stream));
+                              dm ? dm->d_dest : nullptr, dm ? dm->d_dest_keep : nullptr, f.stream, g.fasta_out() ? 1 : 0));
     c->launches += 1;
     if ((rc = fastq_stage_output(c, f, g, f.stream, out, out_capacity, res, dm, segments)) != CG_OK) return rc;
     return check_err_flag(c);
@@ -2131,6 +2202,7 @@ static int fastq_collect_paired_impl(cg_ctx *c, int32_t slot1, int32_t slot2, co
     if (!f1.busy || !f2.busy) return fail(CG_EINVAL, "cg_fastq_collect_paired: nothing was submitted to a slot");
     CU(cudaSetDevice(c->device));
     f1.busy = f2.busy = false;
+    if (fp1->format != fp2->format) return fail(CG_EINVAL, "cg_fastq_collect_paired: both mates must have the same format");
     memset(res1, 0, sizeof *res1);
     memset(res2, 0, sizeof *res2);
     // after its upload everything of the second mate runs on the first mate's stream
@@ -2155,7 +2227,7 @@ static int fastq_collect_paired_impl(cg_ctx *c, int32_t slot1, int32_t slot2, co
     CU(cg_launch_fastq_finish(g1.n, f1.d_rec.p, f1.d_interval.p, f1.d_mask.p, fastq_enabled_filters(fp1), f1.d_outlen.p,
                               f1.d_counters + 1, f2.d_rec.p, f2.d_interval.p, f2.d_mask.p, fastq_enabled_filters(fp2),
                               f2.d_outlen.p, f2.d_counters + 1, pair_filter_mode, mode_untrimmed, 0,
-                              dm ? dm->d_dest : nullptr, dm ? dm->d_dest_keep : nullptr, st));
+                              dm ? dm->d_dest : nullptr, dm ? dm->d_dest_keep : nullptr, st, g1.fasta_out() ? 1 : 0));
     c->launches += 1;
     if ((rc = fastq_stage_output(c, f1, g1, st, out1, out_capacity1, res1, dm, segments1)) != CG_OK) return rc;
     if ((rc = fastq_stage_output(c, f2, g2, st, out2, out_capacity2, res2, dm, segments2)) != CG_OK) return rc;

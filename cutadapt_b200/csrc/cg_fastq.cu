@@ -152,6 +152,76 @@ __global__ void fq_records_kernel(const uint8_t *buf, long long n, const uint32_
     if ((threadIdx.x & 31) == 0 && sum && counters) atomicAdd(&counters[1], sum);
 }
 
+// ---- FASTA: line classes -> normalised chunk -> record table (fa_line_core / fa_record_core, cg_fastq_core.cuh) ----
+// pass 1, one thread per line: bytes the line keeps, header flag, first header line (*first_hdr, initialised to INT_MAX)
+__global__ void fa_classify_kernel(const uint8_t *buf, long long n, const uint32_t *nl_pos, long long n_nl, long long n_lines,
+                                   int32_t *keep, int32_t *is_hdr, int *first_hdr)
+{
+    const long long k = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    bool hdr = false;
+    if (k < n_lines) {
+        uint32_t s, e;
+        int kp;
+        hdr = fa_line_core(buf, nl_pos, n_nl, n, k, &s, &e, &kp) == CG_FA_LINE_HEADER;
+        keep[k] = kp;
+        is_hdr[k] = hdr;
+    }
+    const unsigned m = __ballot_sync(0xFFFFFFFFu, hdr);
+    if (m && (threadIdx.x & 31) == 0) atomicMin(first_hdr, (int)(k + __ffs(m) - 1));
+}
+
+// pass 2, one warp per line (after the scans of keep and is_hdr): copy the kept bytes to the normalised buffer, enter
+// every header in the record table, report the first bad line (err as one 64-bit word: line << 32 | code, so that
+// atomicMin keeps the code of the smallest line)
+__global__ void __launch_bounds__(256) fa_scatter_kernel(const uint8_t *buf, long long n, const uint32_t *nl_pos, long long n_nl,
+                                                          long long n_lines, const int64_t *line_off, const int64_t *hdr_idx,
+                                                          const int *first_hdr, uint8_t *norm, CgFastqRecord *rec,
+                                                          unsigned long long *err)
+{
+    const int lane = threadIdx.x & 31;
+    const long long warps = ((long long)gridDim.x * blockDim.x) >> 5;
+    const long long first = *first_hdr;
+    for (long long k = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5; k < n_lines; k += warps) {
+        uint32_t s, e;
+        int kp;
+        const int kind = fa_line_core(buf, nl_pos, n_nl, n, k, &s, &e, &kp);
+        const int bad = fa_line_error(kind, k, first);
+        if (bad && lane == 0) atomicMin(err, ((unsigned long long)k << 32) | (unsigned)bad);
+        const long long o = line_off[k];
+        const int len = (int)(e - s);
+        for (int j = lane; j < len && kind != CG_FA_LINE_COMMENT; j += 32) norm[o + j] = buf[s + j];
+        if (kind == CG_FA_LINE_HEADER && lane == 0) {
+            norm[o + len] = '\n';
+            const long long r = hdr_idx[k];
+            rec[r].hdr_start = (uint32_t)o + 1u;
+            rec[r].hdr_len = len - 1;
+        }
+    }
+}
+
+// pass 3, one thread per record: the sequence of record r ends where the header of record r + 1 begins
+__global__ void fa_records_kernel(CgFastqRecord *rec, long long n_records, long long n_norm, int cut_front, int cut_back,
+                                  int32_t *seq_len, int32_t *origin, unsigned long long *counters)
+{
+    const long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    unsigned long long bp = 0;
+    if (r < n_records) {
+        const uint32_t seq_end = r + 1 < n_records ? rec[r + 1].hdr_start - 1u : (uint32_t)n_norm;
+        CgFastqRecord o;
+        int len, full, cf;
+        fa_record_core(rec[r].hdr_start, rec[r].hdr_len, seq_end, cut_front, cut_back, &o, &len, &full, &cf);
+        // only the fields nobody else reads: the thread of record r - 1 reads hdr_start
+        rec[r].seq_start = o.seq_start;
+        rec[r].qual_start = o.qual_start;
+        seq_len[r] = len;
+        origin[2 * r] = cf;
+        origin[2 * r + 1] = full;
+        bp = (unsigned long long)full;
+    }
+    for (int d = 16; d; d >>= 1) bp += __shfl_down_sync(0xFFFFFFFFu, bp, d);
+    if ((threadIdx.x & 31) == 0 && bp) atomicAdd(&counters[1], bp);
+}
+
 // ---- exclusive scan int32 -> int64 (n+1 outputs), any n: tile sums, one-CTA scan of the sums, apply ----
 constexpr int SC_TILE = 2048;     // elements per CTA (256 threads x 8)
 
@@ -293,7 +363,7 @@ __global__ void fq_fold_qtrim_kernel(CgFastqRecord *rec, int32_t *seq_len, const
 __global__ void __launch_bounds__(256) fq_revcomp_commit_kernel(uint8_t *buf, CgFastqRecord *rec, const int32_t *seq_len,
                                                                  int32_t *origin, long long n_records, cg_match_rec *matches,
                                                                  const cg_match_rec *matches_rc, int per_read,
-                                                                 uint8_t *is_rc, unsigned long long *counters)
+                                                                 uint8_t *is_rc, unsigned long long *counters, int has_qual)
 {
     const int lane = threadIdx.x & 31;
     const long long warps = ((long long)gridDim.x * blockDim.x) >> 5;
@@ -318,9 +388,12 @@ __global__ void __launch_bounds__(256) fq_revcomp_commit_kernel(uint8_t *buf, Cg
         uint8_t *sq = buf + m.seq_start - front, *ql = buf + m.qual_start - front;
         for (int j = lane; 2 * j < full; j += 32) {      // pair (j, full-1-j); the middle of an odd length meets itself
             const int k = full - 1 - j;
-            const uint8_t a = sq[j], b = sq[k], qa = ql[j], qb = ql[k];
+            const uint8_t a = sq[j], b = sq[k];
             sq[j] = fq_complement(b); sq[k] = fq_complement(a);
-            ql[j] = qb; ql[k] = qa;
+            if (has_qual) {                              // FASTA: the quality span is the sequence itself
+                const uint8_t qa = ql[j], qb = ql[k];
+                ql[j] = qb; ql[k] = qa;
+            }
         }
         __syncwarp();
         if (lane == 0) {
@@ -389,13 +462,15 @@ __device__ __constant__ int kFilterCounter[7] = {4, 5, 8, 9, 10, 7, 7};
 // filtered according to PairedEndFilter (steps.py:105-180): a filter given for one mate only tests that mate;
 // otherwise mode 0 "any", 1 "both", 2 "first" (mode_untrimmed: cli.py:859-893 overrides the mode of
 // --discard-untrimmed to "both" when only one mate has adapters).  The first filter that fires gets the count.
-// out_len = size of the formatted record ("@" name "\n" sequence "\n+\n" qualities "\n") or 0.
+// out_len = size of the formatted record ("@" name "\n" sequence "\n+\n" qualities "\n", or with fasta_out
+// ">" name "\n" sequence "\n") or 0.
 __global__ void fq_finish_kernel(long long n_records, const CgFastqRecord *rec1, const int32_t *interval1,
                                  const int32_t *mask1, int enabled1, int32_t *out_len1, unsigned long long *counters1,
                                  const CgFastqRecord *rec2, const int32_t *interval2, const int32_t *mask2, int enabled2,
                                  int32_t *out_len2, unsigned long long *counters2, int mode, int mode_untrimmed,
-                                 int rc_suffix, const int32_t *dest, const uint8_t *dest_keep)
+                                 int rc_suffix, const int32_t *dest, const uint8_t *dest_keep, int fasta_out)
 {
+    const int per_base = fasta_out ? 1 : 2, fixed = fasta_out ? 3 : 6;
     const long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     int fired = -1;
     unsigned long long bp1 = 0, bp2 = 0;
@@ -407,11 +482,11 @@ __global__ void fq_finish_kernel(long long n_records, const CgFastqRecord *rec1,
         const int left1 = interval1[2 * r + 1] - interval1[2 * r];
         // a reverse-complemented read gets " rc" appended to its name (modifiers.py:295-296)
         const int extra1 = (rc_suffix && (mask1[r] & CG_FQ_MASK_RC)) ? 3 : 0;
-        out_len1[r] = fired < 0 ? rec1[r].hdr_len + extra1 + 2 * left1 + 6 : 0;
+        out_len1[r] = fired < 0 ? rec1[r].hdr_len + extra1 + per_base * left1 + fixed : 0;
         if (mask2) {
             const int left2 = interval2[2 * r + 1] - interval2[2 * r];
             const int extra2 = (rc_suffix && (mask2[r] & CG_FQ_MASK_RC)) ? 3 : 0;
-            out_len2[r] = fired < 0 ? rec2[r].hdr_len + extra2 + 2 * left2 + 6 : 0;
+            out_len2[r] = fired < 0 ? rec2[r].hdr_len + extra2 + per_base * left2 + fixed : 0;
             bp2 = fired < 0 ? left2 : 0;
         }
         written = fired < 0;
@@ -437,7 +512,8 @@ __global__ void fq_finish_kernel(long long n_records, const CgFastqRecord *rec1,
     }
 }
 
-// the trimmed records, one warp per record
+// the trimmed records, one warp per record; FASTA_OUT: ">name\nsequence\n", the sequence on one line
+template <bool FASTA_OUT>
 __global__ void __launch_bounds__(256) fq_write_kernel(const uint8_t *buf, const CgFastqRecord *rec, const int32_t *interval,
                                                         const int64_t *out_off, const int32_t *out_len,
                                                         long long n_records, uint8_t *out, int action,
@@ -451,7 +527,7 @@ __global__ void __launch_bounds__(256) fq_write_kernel(const uint8_t *buf, const
         const CgFastqRecord m = rec[r];
         const int start = interval[2 * r], left = interval[2 * r + 1] - start;
         uint8_t *p = out + o;
-        if (lane == 0) p[0] = '@';
+        if (lane == 0) p[0] = FASTA_OUT ? '>' : '@';
         for (int j = lane; j < m.hdr_len; j += 32) p[1 + j] = buf[m.hdr_start + j];
         p += 1 + m.hdr_len;
         if (rc_suffix && (mask[r] & CG_FQ_MASK_RC)) {
@@ -473,6 +549,10 @@ __global__ void __launch_bounds__(256) fq_write_kernel(const uint8_t *buf, const
             for (int j = lane; j < left; j += 32) p[1 + j] = buf[m.seq_start + start + j];
         }
         p += 1 + left;
+        if (FASTA_OUT) {
+            if (lane == 0) p[0] = '\n';
+            continue;
+        }
         if (lane < 3) p[lane] = lane == 1 ? '+' : '\n';
         for (int j = lane; j < left; j += 32) p[3 + j] = buf[m.qual_start + start + j];
         if (lane == 0) p[3 + left] = '\n';
@@ -550,6 +630,7 @@ struct InfoArgs {
     int kind;                    // 0: --info-file rows; 1: --rest-file rows; 2: --wildcard-file rows (names = the adapters' sequences)
     const int32_t *qtrim;        // quality-trimmed interval of the record (the read the cutter saw), or null
     const int32_t *seq_len;
+    int has_qual;                // 0: FASTA input, the quality columns are empty (adapters.py:408-415, steps.py:250)
 };
 
 template <class Sink>
@@ -588,9 +669,9 @@ __device__ void info_rows(const InfoArgs &a, long long r, Sink &out)
                 out.ch('\t'); out.bytes(sq + ws + s1, c1);
                 out.ch('\t'); out.bytes(sq + ws + s2, c2);
                 out.ch('\t'); out.bytes(a.names + a.name_off[h.adapter], a.name_off[h.adapter + 1] - a.name_off[h.adapter]);
-                out.ch('\t'); out.bytes(ql + ws + s0, c0);
-                out.ch('\t'); out.bytes(ql + ws + s1, c1);
-                out.ch('\t'); out.bytes(ql + ws + s2, c2);
+                out.ch('\t'); out.bytes(ql + ws + s0, a.has_qual ? c0 : 0);
+                out.ch('\t'); out.bytes(ql + ws + s1, a.has_qual ? c1 : 0);
+                out.ch('\t'); out.bytes(ql + ws + s2, a.has_qual ? c2 : 0);
                 out.ch('\t');
                 if (a.revcomp) out.ch(is_rc ? '1' : '0');
                 out.ch('\n');
@@ -605,7 +686,7 @@ __device__ void info_rows(const InfoArgs &a, long long r, Sink &out)
         name();
         out.ch('\t'); out.ch('-'); out.ch('1');
         out.ch('\t'); out.bytes(a.buf + m.seq_start + start, left, a.upper_unmatched != 0);
-        out.ch('\t'); out.bytes(a.buf + m.qual_start + start, left);
+        out.ch('\t'); out.bytes(a.buf + m.qual_start + start, a.has_qual ? left : 0);
         out.ch('\n');
     }
 }
@@ -808,6 +889,37 @@ cudaError_t cg_launch_fastq_records(const uint8_t *d_buf, long long n_bytes, con
     return cudaGetLastError();
 }
 
+cudaError_t cg_launch_fasta_classify(const uint8_t *d_buf, long long n_bytes, const uint32_t *d_nl_pos, long long n_newlines,
+                                     long long n_lines, int32_t *d_keep, int32_t *d_is_hdr, int *d_first_hdr, cudaStream_t st)
+{
+    if (n_lines <= 0) return cudaSuccess;
+    fa_classify_kernel<<<(unsigned)((n_lines + 255) / 256), 256, 0, st>>>(d_buf, n_bytes, d_nl_pos, n_newlines, n_lines,
+                                                                          d_keep, d_is_hdr, d_first_hdr);
+    return cudaGetLastError();
+}
+
+cudaError_t cg_launch_fasta_scatter(const uint8_t *d_buf, long long n_bytes, const uint32_t *d_nl_pos, long long n_newlines,
+                                    long long n_lines, const int64_t *d_line_off, const int64_t *d_hdr_idx,
+                                    const int *d_first_hdr, uint8_t *d_norm, CgFastqRecord *d_rec, int *d_err,
+                                    cudaStream_t st)
+{
+    if (n_lines <= 0) return cudaSuccess;
+    long long grid = (n_lines + 7) / 8;
+    grid = cg_grid_cap(grid, 16);
+    fa_scatter_kernel<<<(unsigned)grid, 256, 0, st>>>(d_buf, n_bytes, d_nl_pos, n_newlines, n_lines, d_line_off, d_hdr_idx,
+                                                      d_first_hdr, d_norm, d_rec, (unsigned long long *)d_err);
+    return cudaGetLastError();
+}
+
+cudaError_t cg_launch_fasta_records(CgFastqRecord *d_rec, long long n_records, long long n_norm, int cut_front, int cut_back,
+                                    int32_t *d_seq_len, int32_t *d_origin, unsigned long long *d_counters, cudaStream_t st)
+{
+    if (n_records <= 0) return cudaSuccess;
+    fa_records_kernel<<<(unsigned)((n_records + 255) / 256), 256, 0, st>>>(d_rec, n_records, n_norm, cut_front, cut_back,
+                                                                           d_seq_len, d_origin, d_counters);
+    return cudaGetLastError();
+}
+
 long long cg_scan_tiles(long long n) { return (n + SC_TILE - 1) / SC_TILE; }
 
 cudaError_t cg_launch_scan_i32(const int32_t *d_in, long long n, unsigned long long *d_tile_scratch, int64_t *d_out,
@@ -842,13 +954,14 @@ cudaError_t cg_launch_fastq_fold_qtrim(CgFastqRecord *d_rec, int32_t *d_seq_len,
 
 cudaError_t cg_launch_fastq_revcomp_commit(uint8_t *d_buf, CgFastqRecord *d_rec, const int32_t *d_seq_len, int32_t *d_origin,
                                            long long n_records, cg_match_rec *d_matches, const cg_match_rec *d_matches_rc,
-                                           int per_read, uint8_t *d_is_rc, unsigned long long *d_counters, cudaStream_t st)
+                                           int per_read, uint8_t *d_is_rc, unsigned long long *d_counters, cudaStream_t st,
+                                           int has_qual)
 {
     if (n_records <= 0) return cudaSuccess;
     long long grid = (n_records + 7) / 8;
     grid = cg_grid_cap(grid, 16);
     fq_revcomp_commit_kernel<<<(unsigned)grid, 256, 0, st>>>(d_buf, d_rec, d_seq_len, d_origin, n_records, d_matches,
-                                                             d_matches_rc, per_read, d_is_rc, d_counters);
+                                                             d_matches_rc, per_read, d_is_rc, d_counters, has_qual);
     return cudaGetLastError();
 }
 
@@ -881,26 +994,31 @@ cudaError_t cg_launch_fastq_finish(long long n_records, const CgFastqRecord *d_r
                                    unsigned long long *d_counters1, const CgFastqRecord *d_rec2,
                                    const int32_t *d_interval2, const int32_t *d_mask2, int enabled2, int32_t *d_out_len2,
                                    unsigned long long *d_counters2, int mode, int mode_untrimmed, int rc_suffix,
-                                   const int32_t *d_dest, const uint8_t *d_dest_keep, cudaStream_t st)
+                                   const int32_t *d_dest, const uint8_t *d_dest_keep, cudaStream_t st, int fasta_out)
 {
     if (n_records <= 0) return cudaSuccess;
     fq_finish_kernel<<<(unsigned)((n_records + 255) / 256), 256, 0, st>>>(n_records, d_rec1, d_interval1, d_mask1, enabled1,
                                                                          d_out_len1, d_counters1, d_rec2, d_interval2,
                                                                          d_mask2, enabled2, d_out_len2, d_counters2, mode,
-                                                                         mode_untrimmed, rc_suffix, d_dest, d_dest_keep);
+                                                                         mode_untrimmed, rc_suffix, d_dest, d_dest_keep,
+                                                                         fasta_out);
     return cudaGetLastError();
 }
 
 cudaError_t cg_launch_fastq_write(const uint8_t *d_buf, const CgFastqRecord *d_rec, const int32_t *d_interval,
                                   const int64_t *d_out_off, const int32_t *d_out_len, long long n_records,
                                   uint8_t *d_out, int action, const int32_t *d_keep_interval, const int32_t *d_mask,
-                                  int rc_suffix, cudaStream_t st)
+                                  int rc_suffix, cudaStream_t st, int fasta_out)
 {
     if (n_records <= 0) return cudaSuccess;
     long long grid = (n_records + 7) / 8;
     grid = cg_grid_cap(grid, 16);
-    fq_write_kernel<<<(unsigned)grid, 256, 0, st>>>(d_buf, d_rec, d_interval, d_out_off, d_out_len, n_records, d_out, action,
-                                                    d_keep_interval, d_mask, rc_suffix);
+    if (fasta_out)
+        fq_write_kernel<true><<<(unsigned)grid, 256, 0, st>>>(d_buf, d_rec, d_interval, d_out_off, d_out_len, n_records, d_out,
+                                                              action, d_keep_interval, d_mask, rc_suffix);
+    else
+        fq_write_kernel<false><<<(unsigned)grid, 256, 0, st>>>(d_buf, d_rec, d_interval, d_out_off, d_out_len, n_records, d_out,
+                                                               action, d_keep_interval, d_mask, rc_suffix);
     return cudaGetLastError();
 }
 
@@ -943,11 +1061,12 @@ cudaError_t cg_launch_fastq_info(int phase, const uint8_t *d_buf, const CgFastqR
                                  const int32_t *d_interval, const int32_t *d_mask, const cg_match_rec *d_matches, int times,
                                  int slots, const uint8_t *d_names, const int32_t *d_name_off, int revcomp, int rc_suffix,
                                  int upper_unmatched, long long n_records, int32_t *d_row_bytes, const int64_t *d_row_off,
-                                 uint8_t *d_out, cudaStream_t st, int kind, const int32_t *d_qtrim, const int32_t *d_seq_len)
+                                 uint8_t *d_out, cudaStream_t st, int kind, const int32_t *d_qtrim, const int32_t *d_seq_len,
+                                 int has_qual)
 {
     if (n_records <= 0) return cudaSuccess;
     InfoArgs a;
-    a.kind = kind; a.qtrim = d_qtrim; a.seq_len = d_seq_len;
+    a.kind = kind; a.qtrim = d_qtrim; a.seq_len = d_seq_len; a.has_qual = has_qual;
     a.buf = d_buf; a.rec = d_rec; a.origin = d_origin; a.interval = d_interval; a.mask = d_mask; a.matches = d_matches;
     a.times = times; a.slots = slots; a.names = d_names; a.name_off = d_name_off; a.revcomp = revcomp;
     a.rc_suffix = rc_suffix; a.upper_unmatched = upper_unmatched;

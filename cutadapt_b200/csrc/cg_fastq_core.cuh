@@ -100,6 +100,59 @@ CG_HD int fq_record_core(const uint8_t *buf, long long n, const uint32_t *nl_pos
     return bad;
 }
 
+// ---- FASTA (cg_fastq_params.format 1) ----
+// A chunk is first rewritten into a normalised buffer in which every record is ">name\n" followed by its whole
+// sequence (no line breaks, no '\r'); the record table then describes that buffer with an empty quality span.
+#define CG_FA_LINE_SEQUENCE 0
+#define CG_FA_LINE_HEADER 1
+#define CG_FA_LINE_COMMENT 2
+#define CG_FA_ERR_BEFORE_HEADER 6     // a line before the first header that is not a '#' comment
+#define CG_FA_ERR_LATE_COMMENT 7      // a '#' line after the first header
+
+// Line k of a FASTA chunk: its kind and how many bytes it keeps in the normalised buffer (a header keeps itself,
+// '>' included, plus '\n'; a sequence line its characters; a '#' line nothing).  [*start, *end): the line without
+// its terminator ("\n" or "\r\n").
+CG_HD int fa_line_core(const uint8_t *buf, const uint32_t *nl_pos, long long n_nl, long long n, long long k, uint32_t *start,
+                       uint32_t *end, int *keep)
+{
+    fq_line_span(buf, nl_pos, n_nl, n, k, start, end);
+    const int len = (int)(*end - *start);
+    const uint8_t c = len ? buf[*start] : 0;
+    if (c == '>') { *keep = len + 1; return CG_FA_LINE_HEADER; }
+    if (c == '#') { *keep = 0; return CG_FA_LINE_COMMENT; }
+    *keep = len;
+    return CG_FA_LINE_SEQUENCE;
+}
+
+// Is line k (of kind `kind`) allowed, given the first header line of the chunk (first_hdr: larger than every line
+// number if there is none)?  '#' lines are comments only in front of the first record; any other line there is an
+// error.  Returns 0 or CG_FA_ERR_*.
+CG_HD int fa_line_error(int kind, long long k, long long first_hdr)
+{
+    if (kind == CG_FA_LINE_COMMENT) return k > first_hdr ? CG_FA_ERR_LATE_COMMENT : 0;
+    if (kind == CG_FA_LINE_SEQUENCE && k < first_hdr) return CG_FA_ERR_BEFORE_HEADER;
+    return 0;
+}
+
+// Record of the normalised buffer whose name is [hdr_start, hdr_start + hdr_len) and whose sequence runs from
+// hdr_start + hdr_len + 1 to seq_end; -u and the bases read as in fq_record_core.
+CG_HD void fa_record_core(uint32_t hdr_start, int hdr_len, uint32_t seq_end, int cut_front, int cut_back, CgFastqRecord *rec,
+                          int *seq_len, int *full_len, int *cut_applied)
+{
+    const uint32_t ss = hdr_start + (uint32_t)hdr_len + 1u;
+    int len = (int)(seq_end - ss);
+    *full_len = len;
+    const int cf = cut_front < len ? cut_front : len;
+    len -= cf;
+    len = cut_back < len ? len - cut_back : 0;
+    *cut_applied = cf;
+    rec->hdr_start = hdr_start;
+    rec->hdr_len = hdr_len;
+    rec->seq_start = ss + (uint32_t)cf;
+    rec->qual_start = rec->seq_start;           // no qualities
+    *seq_len = len;
+}
+
 struct FqVerdict {
     int start, stop;         // what is written: read[start:stop] (relative to the record's sequence after -u)
     int k0, k1;              // the part the action leaves untouched ("remainder")

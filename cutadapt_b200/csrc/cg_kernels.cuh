@@ -92,6 +92,18 @@ cudaError_t cg_launch_fastq_records(const uint8_t *d_buf, long long n_bytes, con
                                     long long n_records, int cut_front, int cut_back, CgFastqRecord *d_rec,
                                     int32_t *d_seq_len, int32_t *d_origin, unsigned long long *d_counters, int *d_err,
                                     cudaStream_t st);
+// FASTA chunk -> normalised chunk + record table (fa_line_core / fa_record_core): classify every line (bytes it keeps,
+// header flag, first header line: *d_first_hdr must start at INT_MAX); after exclusive scans of keep (line offsets in
+// the normalised buffer) and is_hdr (record of each header) the scatter writes the normalised buffer, hdr_start /
+// hdr_len of every record and the first bad line (d_err as one 64-bit word: line << 32 | code); then the records.
+cudaError_t cg_launch_fasta_classify(const uint8_t *d_buf, long long n_bytes, const uint32_t *d_nl_pos, long long n_newlines,
+                                     long long n_lines, int32_t *d_keep, int32_t *d_is_hdr, int *d_first_hdr, cudaStream_t st);
+cudaError_t cg_launch_fasta_scatter(const uint8_t *d_buf, long long n_bytes, const uint32_t *d_nl_pos, long long n_newlines,
+                                    long long n_lines, const int64_t *d_line_off, const int64_t *d_hdr_idx,
+                                    const int *d_first_hdr, uint8_t *d_norm, CgFastqRecord *d_rec, int *d_err,
+                                    cudaStream_t st);
+cudaError_t cg_launch_fasta_records(CgFastqRecord *d_rec, long long n_records, long long n_norm, int cut_front, int cut_back,
+                                    int32_t *d_seq_len, int32_t *d_origin, unsigned long long *d_counters, cudaStream_t st);
 // exclusive scan int32 -> int64, n + 1 outputs; d_tile_scratch: cg_scan_tiles(n) words
 cudaError_t cg_launch_scan_i32(const int32_t *d_in, long long n, unsigned long long *d_tile_scratch, int64_t *d_out,
                                cudaStream_t st);
@@ -103,7 +115,8 @@ cudaError_t cg_launch_fastq_fold_qtrim(CgFastqRecord *d_rec, int32_t *d_seq_len,
 // --revcomp: choose the orientation per record, rewrite the chosen reads in place (counters[11] += replaced)
 cudaError_t cg_launch_fastq_revcomp_commit(uint8_t *d_buf, CgFastqRecord *d_rec, const int32_t *d_seq_len, int32_t *d_origin,
                                            long long n_records, cg_match_rec *d_matches, const cg_match_rec *d_matches_rc,
-                                           int per_read, uint8_t *d_is_rc, unsigned long long *d_counters, cudaStream_t st);
+                                           int per_read, uint8_t *d_is_rc, unsigned long long *d_counters, cudaStream_t st,
+                                           int has_qual = 1);
 cudaError_t cg_launch_fastq_pretrim(const uint8_t *d_buf, const CgFastqRecord *d_rec, const int32_t *d_seq_len,
                                     long long n_records, int flags, int cutoff_front, int cutoff_back, int qbase,
                                     int32_t *d_qtrim, cudaStream_t st);
@@ -120,11 +133,11 @@ cudaError_t cg_launch_fastq_finish(long long n_records, const CgFastqRecord *d_r
                                    unsigned long long *d_counters1, const CgFastqRecord *d_rec2,
                                    const int32_t *d_interval2, const int32_t *d_mask2, int enabled2, int32_t *d_out_len2,
                                    unsigned long long *d_counters2, int mode, int mode_untrimmed, int rc_suffix,
-                                   const int32_t *d_dest, const uint8_t *d_dest_keep, cudaStream_t st);
+                                   const int32_t *d_dest, const uint8_t *d_dest_keep, cudaStream_t st, int fasta_out = 0);
 cudaError_t cg_launch_fastq_write(const uint8_t *d_buf, const CgFastqRecord *d_rec, const int32_t *d_interval,
                                   const int64_t *d_out_off, const int32_t *d_out_len, long long n_records,
                                   uint8_t *d_out, int action, const int32_t *d_keep_interval, const int32_t *d_mask,
-                                  int rc_suffix, cudaStream_t st);
+                                  int rc_suffix, cudaStream_t st, int fasta_out = 0);
 // demultiplexing: cg_launch_fastq_dest gives every record its destination (adapter of the most recent match of R1, or
 // of both mates: d1 * (n_named2 + 1) + d2; reads without a match: the last value of the dimension); phase 0 fills
 // d_bytes[n_dest][tiles] (output bytes per destination and tile of 256 records); after an exclusive scan of that
@@ -141,7 +154,8 @@ cudaError_t cg_launch_fastq_info(int phase, const uint8_t *d_buf, const CgFastqR
                                  int slots, const uint8_t *d_names, const int32_t *d_name_off, int revcomp, int rc_suffix,
                                  int upper_unmatched, long long n_records, int32_t *d_row_bytes, const int64_t *d_row_off,
                                  uint8_t *d_out, cudaStream_t st, int kind = 0, const int32_t *d_qtrim = nullptr,
-                                 const int32_t *d_seq_len = nullptr);   // kind 1 / 2: --rest-file / --wildcard-file rows
+                                 const int32_t *d_seq_len = nullptr,    // kind 1 / 2: --rest-file / --wildcard-file rows
+                                 int has_qual = 1);                     // 0: FASTA input, empty quality columns
 // --pair-adapters: fold the records of adapter pair `pair` into the best pair per read (modifiers.py:480-503)
 cudaError_t cg_launch_fastq_pair_select(long long n_records, int pair, const cg_match_rec *d_cur1, int slots1,
                                         const cg_match_rec *d_cur2, int slots2, cg_match_rec *d_best1, cg_match_rec *d_best2,

@@ -625,11 +625,107 @@ def read_paired_fastq_chunks(f1, f2, buffer_size: int = 4 * 1024 * 1024):
         yield bytes(bufs[0][:starts[0]]), bytes(bufs[1][:starts[1]])
 
 
+def _fasta_head(buf, end: int) -> int:
+    """Length of the longest prefix of buf[:end] that ends in front of a header line (a line starting with '>'),
+    not counting a header at offset 0: the complete records of a FASTA buffer (plus any leading '#' lines)."""
+    return buf.rfind(b"\n>", 0, end) + 1
+
+
+def _fasta_headers(buf, end: int) -> int:
+    """Number of header lines that start in buf[:end]."""
+    return (1 if end and buf[:1] == b">" else 0) + buf.count(b"\n>", 0, end)
+
+
+def _fasta_cut(buf, end: int, n_records: int) -> int:
+    """Offset of header number n_records (0-based) of buf[:end]: just behind the first n_records records."""
+    pos = 0 if buf[:1] == b">" else buf.find(b"\n>", 0, end) + 1
+    for _ in range(n_records):
+        pos = buf.find(b"\n>", pos, end) + 1
+    return pos
+
+
+def read_fasta_chunks(f, buffer_size: int = 4 * 1024 * 1024):
+    """
+    Chunks of complete FASTA records from a binary file object, for ``FastqTrimmer(input_format="fasta")``.  A chunk
+    ends in front of a line that starts with '>'; the first chunk carries any '#' lines in front of the first record.
+    A record larger than the buffer makes the buffer grow.
+    """
+    buf = bytearray(buffer_size)
+    start = 0
+    while True:
+        if start == len(buf):
+            buf.extend(bytes(len(buf)))
+        n = f.readinto(memoryview(buf)[start:])
+        if not n:
+            break
+        end = start + n
+        head = _fasta_head(buf, end)
+        if head:
+            yield bytes(buf[:head])
+            buf[0:end - head] = buf[head:end]
+            start = end - head
+        else:
+            start = end
+    if start:
+        yield bytes(buf[:start])
+
+
+def read_paired_fasta_chunks(f1, f2, buffer_size: int = 4 * 1024 * 1024):
+    """Pairs of FASTA chunks with the same number of complete records each (see read_fasta_chunks)."""
+    bufs = [bytearray(buffer_size), bytearray(buffer_size)]
+    starts = [0, 0]
+    files = (f1, f2)
+    eof = [False, False]
+    while True:
+        ends = list(starts)
+        for k in (0, 1):
+            if starts[k] == len(bufs[k]):
+                bufs[k].extend(bytes(len(bufs[k])))
+            n = 0 if eof[k] else files[k].readinto(memoryview(bufs[k])[starts[k]:])
+            eof[k] = eof[k] or not n
+            ends[k] = starts[k] + (n or 0)
+        if eof[0] and eof[1]:
+            break
+        records = min(_fasta_headers(bufs[k], _fasta_head(bufs[k], ends[k])) for k in (0, 1))
+        if records:
+            cuts = [_fasta_cut(bufs[k], ends[k], records) for k in (0, 1)]
+            yield bytes(bufs[0][:cuts[0]]), bytes(bufs[1][:cuts[1]])
+            for k in (0, 1):
+                bufs[k][0:ends[k] - cuts[k]] = bufs[k][cuts[k]:ends[k]]
+                starts[k] = ends[k] - cuts[k]
+        else:
+            starts = ends
+    if starts[0] or starts[1]:
+        yield bytes(bufs[0][:starts[0]]), bytes(bufs[1][:starts[1]])
+
+
+_FORMATS = {("fastq", None): _lib.CG_FORMAT_FASTQ, ("fastq", "fastq"): _lib.CG_FORMAT_FASTQ,
+            ("fasta", None): _lib.CG_FORMAT_FASTA, ("fasta", "fasta"): _lib.CG_FORMAT_FASTA,
+            ("fastq", "fasta"): _lib.CG_FORMAT_FASTQ_TO_FASTA}
+
+
+def _format_code(input_format: str, output_format: Optional[str]) -> int:
+    """cg_fastq_params.format of (input format, output format or None for the input's)."""
+    if (input_format, output_format) not in _FORMATS:
+        raise ValueError(f"unsupported formats: {input_format!r} in, {output_format!r} out "
+                         "(input 'fastq' or 'fasta'; output None, 'fasta', or 'fastq' for FASTQ input)")
+    return _FORMATS[(input_format, output_format)]
+
+
+def _output_capacity(n_bytes: int, fmt: int) -> int:
+    """Output bytes a chunk of n_bytes can need: trimming only shortens a record ("\\r\\n" -> "\\n" and "+name" -> "+"
+    too), except for the newline a chunk without a final one gets and, in FASTA, the empty line of a record without
+    sequence (">a\\n" -> ">a\\n\\n", at most 1.5 x)."""
+    return (n_bytes + n_bytes // 2 if fmt == _lib.CG_FORMAT_FASTA else n_bytes) + 16
+
+
 def _fastq_params(times=1, quality_cutoff=None, quality_base=33, nextseq_cutoff=None, minimum_length=0,
                   maximum_length=None, max_n=None, max_expected_errors=None, discard_trimmed=False,
                   discard_untrimmed=False, cut=(), poly_a=False, length=None, trim_n=False,
-                  discard_casava=False, action="trim", revcomp=False, rc_suffix=True) -> "_lib.cg_fastq_params":
+                  discard_casava=False, action="trim", revcomp=False, rc_suffix=True, input_format="fastq",
+                  output_format=None) -> "_lib.cg_fastq_params":
     fp = _lib.cg_fastq_params()
+    fp.format = _format_code(input_format, output_format)
     fp.trim = _lib.make_params(
         quality_trim=quality_cutoff is not None,
         cutoff_front=quality_cutoff[0] if quality_cutoff else 0,
@@ -706,11 +802,13 @@ class FastqTrimmer:
     revcomp, rc_suffix  --revcomp: adapters are searched on the read and on its reverse complement and the better
                         orientation is written (" rc" appended to the name unless rc_suffix is False;
                         ReverseComplementer, modifiers.py:264-308), all on the device
+    input_format        "fastq" (default) or "fasta" (read_fasta_chunks; no quality options then)
+    output_format       None (the input's format) or "fasta" (FASTQ in, FASTA out: a .fasta / .fa output or --fasta)
 
     ``process_chunk(bytes) -> bytes``; ``process_chunks(iterable)`` keeps one chunk in flight so that the
     upload of chunk i+1 overlaps the download of chunk i.  ``statistics`` accumulates the counters of
     ``cg_fastq_result`` over all chunks.  Chunks must consist of complete records (what
-    ``dnaio.read_chunks`` yields).
+    ``dnaio.read_chunks`` yields; read_fastq_chunks / read_fasta_chunks).
     """
 
     def __init__(self, adapters=None, times: int = 1, quality_cutoff: Optional[Tuple[int, int]] = None,
@@ -720,12 +818,13 @@ class FastqTrimmer:
                  discard_untrimmed: bool = False, cut: Sequence[int] = (), poly_a: bool = False,
                  length: Optional[int] = None, trim_n: bool = False, discard_casava: bool = False,
                  action: Optional[str] = "trim", revcomp: bool = False, rc_suffix: bool = True,
+                 input_format: str = "fastq", output_format: Optional[str] = None,
                  ctx: Optional[_lib.Context] = None):
         self.ctx = ctx or _lib.default_context()
         self.adapters, self._set = _device_set(adapters, self.ctx)
         self.params = _fastq_params(times, quality_cutoff, quality_base, nextseq_cutoff, minimum_length, maximum_length,
                                     max_n, max_expected_errors, discard_trimmed, discard_untrimmed, cut, poly_a, length,
-                                    trim_n, discard_casava, action, revcomp, rc_suffix)
+                                    trim_n, discard_casava, action, revcomp, rc_suffix, input_format, output_format)
         self.statistics = {}
         self._out_bufs, self._out_keep = {}, {}
 
@@ -752,14 +851,20 @@ class FastqTrimmer:
         return buf
 
     def _collect(self, ticket, copy: bool = True):
-        slot, n_bytes, _ = ticket
-        # trimming only ever shortens a record ("\r\n" -> "\n" and "+name" -> "+" too); the one byte a record
-        # can grow by is the newline that a chunk without a final newline gets
-        out = self._out_buffer(slot, n_bytes + 16)
-        res = _lib.cg_fastq_result()
-        _lib.check(_lib.lib().cg_fastq_collect(
-            self.ctx.handle, slot, self._set.handle if self._set is not None else None, C.byref(self.params),
-            out.ctypes.data, out.size, C.byref(res)))
+        slot, n_bytes, chunk = ticket
+        out = self._out_buffer(slot, _output_capacity(n_bytes, self.params.format))
+        while True:
+            res = _lib.cg_fastq_result()
+            rc = _lib.lib().cg_fastq_collect(
+                self.ctx.handle, slot, self._set.handle if self._set is not None else None, C.byref(self.params),
+                out.ctypes.data, out.size, C.byref(res))
+            # FASTA output: " rc" suffixes can exceed the bound; the call says how much it needs, run the chunk again
+            if rc != 0 and self.params.format != _lib.CG_FORMAT_FASTQ and res.out_bytes > out.size:
+                slot, _, chunk = self._submit(chunk)
+                out = self._out_buffer(slot, res.out_bytes)
+                continue
+            _lib.check(rc)
+            break
         for k, v in res.as_dict().items():
             self.statistics[k] = self.statistics.get(k, 0) + v
         return out[: res.out_bytes].tobytes() if copy else out[: res.out_bytes]
@@ -775,7 +880,7 @@ class FastqTrimmer:
         for this chunk (every output in input order); ``cg_fastq_collect_demux``."""
         outputs, dest = self._demux_names()
         slot, n_bytes, _ = self._submit(chunk)
-        out = self._out_buffer(slot, n_bytes + 16)
+        out = self._out_buffer(slot, _output_capacity(n_bytes, self.params.format))
         res = _lib.cg_fastq_result()
         segments = np.zeros(len(outputs) + 2, dtype=np.int64)
         _lib.check(_lib.lib().cg_fastq_collect_demux(
@@ -807,7 +912,7 @@ class FastqTrimmer:
         capacity = per_read * 2 * n_bytes + (1 << 20)
         while True:
             slot, _, _ = self._submit(chunk)
-            out = self._out_buffer(slot, n_bytes + 16)
+            out = self._out_buffer(slot, _output_capacity(n_bytes, self.params.format))
             rows = np.empty(capacity, dtype=np.uint8)
             res = _lib.cg_fastq_result()
             n_rows = C.c_int64(0)
@@ -861,7 +966,8 @@ class PairedFastqTrimmer:
     ``options1`` / ``options2`` dicts with FastqTrimmer's keyword arguments for each mate (-q / -Q, -u / -U,
     -l / -L ...; filters such as ``minimum_length`` or ``discard_trimmed`` go into both unless the command
     line gives them for one mate only).  ``pair_filter`` is "any" (default), "both" or "first"
-    (PairedEndFilter, steps.py:105-180).  ``process_chunk(chunk1, chunk2) -> (bytes, bytes)``;
+    (PairedEndFilter, steps.py:105-180).  ``input_format`` / ``output_format`` as for FastqTrimmer, for both
+    mates (read_paired_fasta_chunks).  ``process_chunk(chunk1, chunk2) -> (bytes, bytes)``;
     ``statistics`` = (dict for R1, dict for R2).
     """
 
@@ -869,12 +975,14 @@ class PairedFastqTrimmer:
 
     def __init__(self, adapters1=None, adapters2=None, options1: Optional[dict] = None,
                  options2: Optional[dict] = None, pair_filter: str = "any", pair_adapters: bool = False,
+                 input_format: str = "fastq", output_format: Optional[str] = None,
                  ctx: Optional[_lib.Context] = None):
         if pair_filter not in self.MODES:
             raise ValueError("pair_filter must be 'any', 'both' or 'first'")
         self.ctx = ctx or _lib.default_context()
-        self.params1 = _fastq_params(**(options1 or {}))
-        self.params2 = _fastq_params(**(options2 or {}))
+        formats = dict(input_format=input_format, output_format=output_format)
+        self.params1 = _fastq_params(**{**(options1 or {}), **formats})
+        self.params2 = _fastq_params(**{**(options2 or {}), **formats})
         self.mode = self.MODES[pair_filter]
         self.statistics = ({}, {})
         self._pairs = None
@@ -913,8 +1021,8 @@ class PairedFastqTrimmer:
 
     def process_chunk(self, chunk1, chunk2) -> Tuple[bytes, bytes]:
         (s1, b1), (s2, b2) = self._submit(chunk1), self._submit(chunk2)
-        out1 = np.empty(b1.size + 16, dtype=np.uint8)
-        out2 = np.empty(b2.size + 16, dtype=np.uint8)
+        out1 = np.empty(_output_capacity(b1.size, self.params1.format), dtype=np.uint8)
+        out2 = np.empty(_output_capacity(b2.size, self.params2.format), dtype=np.uint8)
         r1, r2 = _lib.cg_fastq_result(), _lib.cg_fastq_result()
         if self._pairs is not None:
             _lib.check(_lib.lib().cg_fastq_collect_pair_adapters(
@@ -954,8 +1062,8 @@ class PairedFastqTrimmer:
             keys = names1 + [unknown]
             keep = np.array([1] * n1 + [0 if discard_untrimmed else 1], dtype=np.uint8)
         (s1, b1), (s2, b2) = self._submit(chunk1), self._submit(chunk2)
-        out1 = np.empty(b1.size + 16, dtype=np.uint8)
-        out2 = np.empty(b2.size + 16, dtype=np.uint8)
+        out1 = np.empty(_output_capacity(b1.size, self.params1.format), dtype=np.uint8)
+        out2 = np.empty(_output_capacity(b2.size, self.params2.format), dtype=np.uint8)
         r1, r2 = _lib.cg_fastq_result(), _lib.cg_fastq_result()
         seg1 = np.zeros(len(keys) + 1, dtype=np.int64)
         seg2 = np.zeros(len(keys) + 1, dtype=np.int64)

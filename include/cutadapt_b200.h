@@ -331,7 +331,8 @@ typedef struct cg_fastq_params {
                                     adapters are searched on the read and on its reverse complement, the better
                                     orientation is kept.  1 = append " rc" to the name of a replaced read, 2 = do not
                                     (--rename given, cli.py:1082-1116)                                  */
-    int32_t reserved[3];
+    int32_t format;              /* CG_FORMAT_*: what the chunk is and what is written (below); 0 = FASTQ    */
+    int32_t reserved[2];
 } cg_fastq_params;
 typedef struct cg_fastq_result {
     int64_t n_records, n_written;
@@ -342,8 +343,29 @@ typedef struct cg_fastq_result {
     int64_t reverse_complemented; /* --revcomp: reads replaced by their reverse complement             */
     int64_t reserved[2];
 } cg_fastq_result;
+/* Formats (cg_fastq_params.format; both mates of a pair must have the same one, else CG_EINVAL):
+ *   CG_FORMAT_FASTQ           FASTQ in, FASTQ out (zeroed parameters)
+ *   CG_FORMAT_FASTA           FASTA in, FASTA out
+ *   CG_FORMAT_FASTQ_TO_FASTA  FASTQ in, FASTA out (what the reference writes to a .fasta / .fa path or with --fasta,
+ *                             files.py:238-285, cli.py:925-931)
+ * A FASTA chunk is a sequence of records: a header line that starts with '>' (the name is the rest of the line)
+ * followed by any number of sequence lines, which are joined without separator; a record may have no sequence line
+ * at all (">a\n>b\n" is two empty reads).  Lines end in "\n" or "\r\n", the last one may lack its terminator.  Lines
+ * that start with '#' in front of the first header are comments and are skipped (a chunk of comments alone holds no
+ * record).  Rejected with CG_EINVAL, the message naming the line (1-based, within the chunk): any other line in front
+ * of the first header (an empty one included), and a '#' line after the first header (the reference's test vectors
+ * do not say what dnaio does with it).  A chunk must start at a header or at those comments.  FASTA has no qualities:
+ * with CG_FORMAT_FASTA, quality_trim, nextseq_trim and max_expected_errors >= 0 are CG_EINVAL (the reference's CLI drops
+ * --max-ee with a warning, cli.py:756-760; that is the caller's decision), the info-file rows have empty quality
+ * columns (adapters.py:408-415, steps.py:250).  FASTA output is ">name\nsequence\n", the sequence on one line.  It can
+ * be LARGER than the input: a record without sequence line (">a" plus a line break) is written as ">a\n\n", so the
+ * output of a FASTA chunk is at most 1.5 x its size plus 2 bytes; FASTQ -> FASTA output is never larger than the
+ * FASTQ bound below. */
+#define CG_FORMAT_FASTQ 0
+#define CG_FORMAT_FASTA 1
+#define CG_FORMAT_FASTQ_TO_FASTA 2
 /* set may be NULL: quality trimming and filters only.  fastq / out: HOST pointers (pinned or pageable).
- * Errors: CG_EINVAL for malformed FASTQ (message names the record), a too small output buffer (out_bytes in
+ * Errors: CG_EINVAL for malformed FASTQ (message names the record) or FASTA (names the line), a too small output buffer (out_bytes in
  * *res says what is needed), CG_ENONASCII like cg_process_batch. */
 int cg_fastq_trim_chunk(cg_ctx *ctx, const cg_adapterset *set, const uint8_t *fastq, int64_t n_bytes,
                         const cg_fastq_params *params, uint8_t *out, int64_t out_capacity, cg_fastq_result *res);

@@ -1,11 +1,13 @@
-"""End-to-end throughput of the FASTQ entry point (not a bench line; see DESIGN.md section 4.6).
+"""End-to-end throughput of the FASTQ entry point (not a bench line; see DESIGN.md sections 4.6, 4.7).
 
-  python tools/measure_fastq.py [n_reads] [chunk_megabytes]
+  python tools/measure_fastq.py [n_reads] [chunk_megabytes] [fastq | fasta | fasta60]
 
 Builds n_reads synthetic FASTQ records of BASELINE configs[1]'s shape (150 bp, Phred+33 qualities, names
 "@SIM2:000000123") in pinned host memory, cuts the buffer into chunks of whole records and streams them
 through FastqTrimmer.process_chunks (-a AGATCGGAAGAGC -q 20 -m 20): raw FASTQ bytes in, trimmed FASTQ bytes
-out, host -> device -> host inside the timed region.  Prints one JSON line.
+out, host -> device -> host inside the timed region.  Prints one JSON line.  "fasta" / "fasta60": the same reads as
+FASTA (">SIM2:000000123" and the sequence on one line / wrapped at 60 columns) through the FASTA path
+(input_format="fasta", -a AGATCGGAAGAGC -m 20: FASTA has no qualities to trim).
 """
 import json
 import sys
@@ -44,13 +46,49 @@ def build_fastq(n, pinned=True):
     return host.numpy(), rec_len
 
 
+def build_fasta(n, wrap=None, pinned=True):
+    """The reads of build_fastq as FASTA records of equal size: one sequence line, or lines of `wrap` columns."""
+    seq, _ = make_read_tensor(n, config=2, device="cuda", with_qualities=True)
+    name_len = 6 + 9
+    cuts = list(range(0, 150, wrap or 150))
+    rec_len = 1 + name_len + 1 + 150 + len(cuts)
+    rec = torch.empty((n, rec_len), dtype=torch.uint8, device="cuda")
+    rec[:, 0] = ord(">")
+    rec[:, 1:6] = torch.tensor(list(b"SIM2:"), dtype=torch.uint8, device="cuda")
+    idx = torch.arange(n, device="cuda")
+    for d in range(10):
+        rec[:, 6 + 9 - d] = (48 + (idx // 10 ** d) % 10).to(torch.uint8)
+    o = 1 + name_len
+    rec[:, o] = 10
+    o += 1
+    for c in cuts:
+        w = min(150, c + (wrap or 150)) - c
+        rec[:, o:o + w] = seq[:, c:c + w]
+        rec[:, o + w] = 10
+        o += w + 1
+    host = torch.empty(n * rec_len, dtype=torch.uint8, pin_memory=pinned)
+    host.copy_(rec.view(-1))
+    torch.cuda.synchronize()
+    return host.numpy(), rec_len
+
+
 def main():
     n = int(sys.argv[1]) if len(sys.argv) > 1 else 4_000_000
     chunk_mb = int(sys.argv[2]) if len(sys.argv) > 2 else 64
-    data, rec_len = build_fastq(n)
+    variant = sys.argv[3] if len(sys.argv) > 3 else "fastq"
+    if variant == "fastq":
+        data, rec_len = build_fastq(n)
+    else:
+        data, rec_len = build_fasta(n, wrap=60 if variant == "fasta60" else None)
     per_chunk = max(1, (chunk_mb << 20) // rec_len)
     chunks = [data[i * rec_len:min(n, i + per_chunk) * rec_len] for i in range(0, n, per_chunk)]
-    t = FastqTrimmer([PA.BackAdapter("AGATCGGAAGAGC", max_errors=0.1)], quality_cutoff=(0, 20), minimum_length=20)
+    adapters = [PA.BackAdapter("AGATCGGAAGAGC", max_errors=0.1)]
+    if variant == "fastq":
+        t = FastqTrimmer(adapters, quality_cutoff=(0, 20), minimum_length=20)
+        what = "FASTQ bytes in -> trimmed FASTQ bytes out (-a AGATCGGAAGAGC -q 20 -m 20), host to host"
+    else:
+        t = FastqTrimmer(adapters, minimum_length=20, input_format="fasta")
+        what = f"FASTA ({variant}) bytes in -> trimmed FASTA bytes out (-a AGATCGGAAGAGC -m 20), host to host"
     out_bytes = sum(len(o) for o in t.process_chunks(chunks[:9], copy=False))   # warm-up: every slot's buffers, pool
     t.statistics.clear()
     t0 = time.perf_counter()
@@ -60,7 +98,7 @@ def main():
     wall = time.perf_counter() - t0
     st = t.statistics
     print(json.dumps({
-        "what": "FASTQ bytes in -> trimmed FASTQ bytes out (-a AGATCGGAAGAGC -q 20 -m 20), host to host",
+        "what": what,
         "reads": n, "chunk_mb": chunk_mb, "chunks": len(chunks), "reads_per_s": n / wall,
         "in_GB_per_s": data.size / wall / 1e9, "out_GB_per_s": out_bytes / wall / 1e9,
         "in_bytes": int(data.size), "out_bytes": out_bytes, "wall_s": wall,

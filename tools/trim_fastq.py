@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
 """
-Trim FASTQ files on the GPU: a minimal driver around cutadapt_b200.pipeline.FastqTrimmer / PairedFastqTrimmer
+Trim FASTQ and FASTA files on the GPU: a minimal driver around cutadapt_b200.pipeline.FastqTrimmer / PairedFastqTrimmer
 that understands the subset of cutadapt's options the device path implements.  Not a replacement for cutadapt's
 command line (no reports, no compressed files): it shows the per-chunk worker of INTEGRATION.md section 3 running
 on real files.
@@ -8,6 +8,11 @@ on real files.
   python tools/trim_fastq.py -a AGATCGGAAGAGC -q 20 -m 20 -o out.fastq in.fastq
   python tools/trim_fastq.py -a ADAPT1 -A ADAPT2 -q 20 -m 20 -o out.1.fastq -p out.2.fastq in.1.fastq in.2.fastq
   python tools/trim_fastq.py -g bc1=^ACGTACGTAC -g bc2=^TTGCATTGCA -o 'demux-{name}.fastq' in.fastq     (demultiplex)
+  python tools/trim_fastq.py -a AGATCGGAAGAGC -m 20 -o out.fasta in.fasta           (FASTA; also FASTQ -> FASTA)
+
+The input format comes from the first byte of the (first) input, as cutadapt's files.detect_file_format does: '>' or
+'#' is FASTA, anything else (an empty file included) FASTQ.  The output is FASTA when the input is, when -o ends in
+.fasta / .fa, or with --fasta.
 """
 import argparse
 import json
@@ -15,8 +20,14 @@ import sys
 
 sys.path.insert(0, __file__.rsplit("/", 2)[0])
 import cutadapt_b200.adapters as PA  # noqa: E402
-from cutadapt_b200.pipeline import (FastqTrimmer, PairedFastqTrimmer, read_fastq_chunks,  # noqa: E402
-                                    read_paired_fastq_chunks)
+from cutadapt_b200.pipeline import (FastqTrimmer, PairedFastqTrimmer, read_fasta_chunks,  # noqa: E402
+                                    read_fastq_chunks, read_paired_fasta_chunks, read_paired_fastq_chunks)
+
+
+def detect_format(path):
+    """"fasta" or "fastq" from the first byte (files.py:314-333)."""
+    with open(path, "rb") as f:
+        return "fasta" if f.read(1) in (b">", b"#") else "fastq"
 
 
 def make_adapters(specs, kind, error_rate, overlap):
@@ -59,11 +70,20 @@ def main():
     ap.add_argument("--discard-untrimmed", action="store_true")
     ap.add_argument("--action", default="trim", choices=["trim", "none", "mask", "lowercase", "retain", "crop"])
     ap.add_argument("--pair-filter", default="any", choices=["any", "both", "first"])
+    ap.add_argument("--fasta", action="store_true", help="write FASTA even for FASTQ input")
     ap.add_argument("--buffer-size", type=int, default=64 << 20)
     ap.add_argument("-o", "--output", required=True, help="output FASTQ; with {name}: one file per adapter name")
     ap.add_argument("-p", "--paired-output")
     ap.add_argument("inputs", nargs="+")
     args = ap.parse_args()
+    input_format = detect_format(args.inputs[0])
+    fasta_out = input_format == "fasta" or args.fasta or args.output.endswith((".fasta", ".fa"))
+    output_format = "fasta" if fasta_out and input_format == "fastq" else None
+    if input_format == "fasta" and args.max_ee is not None:
+        print("WARNING: Ignoring option --max-ee because input does not provide quality values", file=sys.stderr)
+        args.max_ee = None
+    reader = read_fasta_chunks if input_format == "fasta" else read_fastq_chunks
+    paired_reader = read_paired_fasta_chunks if input_format == "fasta" else read_paired_fastq_chunks
 
     qc = None
     if args.quality_cutoff is not None:
@@ -74,6 +94,7 @@ def main():
                   max_expected_errors=args.max_ee, discard_trimmed=args.discard_trimmed,
                   discard_untrimmed=args.discard_untrimmed, cut=args.cut, poly_a=args.poly_a, length=args.length,
                   trim_n=args.trim_n, discard_casava=args.discard_casava, action=args.action)
+    formats = dict(input_format=input_format, output_format=output_format)
     ads1 = (make_adapters(args.back, "back", args.error_rate, args.overlap)
             + make_adapters(args.front, "front", args.error_rate, args.overlap)
             + make_adapters(args.anywhere, "anywhere", args.error_rate, args.overlap))
@@ -84,19 +105,21 @@ def main():
     if len(args.inputs) == 2:
         if not args.paired_output:
             ap.error("paired-end input needs -p")
-        t = PairedFastqTrimmer(ads1, ads2, common, common, args.pair_filter)
+        if detect_format(args.inputs[1]) != input_format:
+            ap.error("both inputs must have the same format")
+        t = PairedFastqTrimmer(ads1, ads2, common, common, args.pair_filter, **formats)
         with open(args.inputs[0], "rb") as f1, open(args.inputs[1], "rb") as f2, \
                 open(args.output, "wb") as o1, open(args.paired_output, "wb") as o2:
-            for c1, c2 in read_paired_fastq_chunks(f1, f2, args.buffer_size):
+            for c1, c2 in paired_reader(f1, f2, args.buffer_size):
                 r1, r2 = t.process_chunk(c1, c2)
                 o1.write(r1)
                 o2.write(r2)
         stats = {"read1": t.statistics[0], "read2": t.statistics[1]}
     elif "{name}" in args.output:
-        t = FastqTrimmer(ads1, **common)
+        t = FastqTrimmer(ads1, **common, **formats)
         files = {}
         with open(args.inputs[0], "rb") as f:
-            for chunk in read_fastq_chunks(f, args.buffer_size):
+            for chunk in reader(f, args.buffer_size):
                 for name, data in t.process_chunk_demux(chunk).items():
                     if name == "unknown" and args.discard_untrimmed:
                         continue
@@ -107,9 +130,9 @@ def main():
             fh.close()
         stats = t.statistics
     else:
-        t = FastqTrimmer(ads1, **common)
+        t = FastqTrimmer(ads1, **common, **formats)
         with open(args.inputs[0], "rb") as f, open(args.output, "wb") as o:
-            for out in t.process_chunks(read_fastq_chunks(f, args.buffer_size), copy=False):
+            for out in t.process_chunks(reader(f, args.buffer_size), copy=False):
                 o.write(out.tobytes() if hasattr(out, "tobytes") else out)
         stats = t.statistics
     print(json.dumps(stats), file=sys.stderr)
