@@ -126,7 +126,8 @@ class cg_fastq_params(C.Structure):
         ("action", C.c_int32),
         ("revcomp", C.c_int32),
         ("format", C.c_int32),
-        ("reserved", C.c_int32 * 2),
+        ("stats", C.c_int32),
+        ("reserved", C.c_int32),
     ]
 
 
@@ -195,6 +196,9 @@ def _declare(lib) -> None:
                                                   C.POINTER(cg_fastq_params), i32, vp, i32, vp, i32, vp, vp, i64, vp, i64,
                                                   C.POINTER(cg_fastq_result), C.POINTER(cg_fastq_result), vp, vp]
     lib.cg_fastq_collect.argtypes = [vp, i32, vp, C.POINTER(cg_fastq_params), vp, i64, C.POINTER(cg_fastq_result)]
+    lib.cg_fastq_stats_create.argtypes = [vp, i32, C.POINTER(i32)]
+    lib.cg_fastq_stats_read.argtypes = [vp, i32, C.POINTER(i32), C.POINTER(i32), vp, i64, C.POINTER(i64), C.c_int]
+    lib.cg_fastq_stats_destroy.argtypes = [vp, i32]
     lib.cg_adapterset_create.argtypes = [
         vp, C.POINTER(cg_adapter_desc), i32, C.POINTER(cg_group_desc), i32, C.POINTER(vp),
     ]
@@ -418,6 +422,39 @@ def make_params(quality_trim=False, cutoff_front=0, cutoff_back=0, quality_base=
 
 
 # ---- context ---------------------------------------------------------------------------------
+
+
+class FastqStatistics:
+    """A statistics accumulator of the FASTQ path on a context (cg_fastq_stats_*): the collects whose parameters
+    name ``handle`` in ``stats`` add their statistics to it."""
+
+    def __init__(self, ctx: "Context", n_adapters: int):
+        h = C.c_int32(0)
+        check(lib().cg_fastq_stats_create(ctx.handle, int(n_adapters), C.byref(h)))
+        self.ctx, self.handle, self.n_adapters = ctx, h.value, int(n_adapters)
+
+    def read(self, reset: bool = False) -> Tuple[np.ndarray, int, int]:
+        """(the int64 vector, max_len, kmax) of its current layout."""
+        max_len, kmax, size = C.c_int32(), C.c_int32(), C.c_int64()
+        check(lib().cg_fastq_stats_read(self.ctx.handle, self.handle, C.byref(max_len), C.byref(kmax), None, 0,
+                                        C.byref(size), 0))
+        out = np.zeros(size.value, dtype=np.int64)
+        check(lib().cg_fastq_stats_read(self.ctx.handle, self.handle, C.byref(max_len), C.byref(kmax),
+                                        out.ctypes.data, out.size, C.byref(size), int(reset)))
+        return out, max_len.value, kmax.value
+
+    def close(self) -> None:
+        if self.handle:
+            check(lib().cg_fastq_stats_destroy(self.ctx.handle, self.handle))
+            self.handle = 0
+
+    def __del__(self):
+        # the accumulator keeps its context alive (self.ctx), so the handle is still valid here
+        try:
+            self.close()
+        except Exception:
+            pass
+
 
 
 class Context:

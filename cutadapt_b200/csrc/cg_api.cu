@@ -11,6 +11,7 @@
 
 #include <algorithm>
 #include <chrono>
+#include <map>
 #include <string>
 #include <vector>
 
@@ -124,10 +125,20 @@ struct FastqSlot {
     DevBuf<uint8_t> d_norm;                     // FASTA: the normalised chunk (swapped into d_in once built)
     DevBuf<int32_t> d_faline;                   // FASTA: bytes kept and header flag per line, first header line
     DevBuf<int64_t> d_faoff;                    // FASTA: their exclusive scans
+    DevBuf<unsigned long long> d_fqstats;       // statistics on: the chunk's statistics vector (added on success)
+    DevBuf<int32_t> d_polya;                    // statistics with --poly-a: bases PolyATrimmer removed, per record
+    PinBuf<unsigned long long> h_fqstats;
     unsigned long long *d_counters = nullptr;   // [0] newline total, [1..] CG_FQ_COUNTERS
     int *d_err = nullptr;                       // [0] code, [1] record
     PinBuf<uint8_t> h_in, h_out;
     PinBuf<unsigned long long> h_counters;
+};
+
+// A statistics accumulator of the FASTQ path (cg_fastq_stats_create): the vector of cg_fastq_stats_read at
+// (n_adapters, max_len, kmax); both sizes grow when a chunk needs more.
+struct FqStatsAcc {
+    int32_t n_adapters = 0, max_len = 0, kmax = 0;
+    std::vector<int64_t> v;
 };
 
 struct cg_ctx {
@@ -177,6 +188,8 @@ struct cg_ctx {
     bool scratch_busy = false;
     FastqSlot fq[CG_FQ_SLOTS];
     int fq_next = 0;
+    std::map<int32_t, FqStatsAcc> fq_stats;      // cg_fastq_stats_* by handle
+    int32_t fq_stats_next = 1;
 };
 
 struct cg_adapterset {
@@ -282,6 +295,7 @@ extern "C" int cg_ctx_destroy(cg_ctx *c)
         f.d_isrc.release(); f.d_dest.release(); f.d_pairkey.release(); f.d_destkeep.release(); f.d_origin.release();
         f.d_names.release(); f.d_infoout.release(); f.d_nameoff.release(); f.d_inforow.release(); f.d_infooff.release();
         f.d_norm.release(); f.d_faline.release(); f.d_faoff.release();
+        f.d_fqstats.release(); f.d_polya.release(); f.h_fqstats.release();
         f.h_in.release(); f.h_out.release(); f.h_counters.release();
         if (f.d_counters) cudaFree(f.d_counters);
         if (f.d_err) cudaFree(f.d_err);
@@ -1657,6 +1671,10 @@ struct FqStage {
     const uint8_t *d_is_rc = nullptr;    // --revcomp: the record was replaced by its reverse complement
     int rc_suffix = 0;                   // ... and gets " rc" appended to its name
     int format = CG_FORMAT_FASTQ;        // cg_fastq_params.format
+    bool packed = false;                 // d_offs / d_seq / max_len hold this mate's reads
+    FqStatsAcc *acc = nullptr;           // statistics on: the accumulator of this mate ...
+    int st_len = 0, st_kmax = 0;         // ... and the layout of the chunk's vector in d_fqstats
+    bool st_poly_a = false;              // d_polya was filled
     bool has_qual() const { return format != CG_FORMAT_FASTA; }
     bool fasta_out() const { return format != CG_FORMAT_FASTQ; }
 };
@@ -1814,6 +1832,7 @@ static int fastq_stage_pack(cg_ctx *c, FastqSlot &f, cudaStream_t st, FqStage &g
                               reverse_complement ? 1 : 0, st));
     c->launches += 1;
     if (reverse_complement) return CG_OK;       // offsets, longest read and format are those of the forward pass
+    g.packed = true;
     CU(cudaMemsetAsync(c->d_err + 1, 0, sizeof(int), st));
     CU(cg_launch_max_len(f.d_offs.p, n, c->d_err + 1, st));
     c->launches += 1;
@@ -1827,8 +1846,15 @@ static int fastq_stage_pack(cg_ctx *c, FastqSlot &f, cudaStream_t st, FqStage &g
 
 // What is left of every record and which filters it fails (fq_evaluate_core)
 static int fastq_stage_verdict(cg_ctx *c, FastqSlot &f, const cg_fastq_params *fp, int poly_a_mode, cudaStream_t st,
-                               const FqStage &g)
+                               FqStage &g)
 {
+    int32_t *d_poly_a = nullptr;                // statistics: PolyATrimmer.trimmed_bases per record
+    if (g.acc && fp->poly_a) {
+        int rc = f.d_polya.ensure((size_t)g.n);
+        if (rc != CG_OK) return rc;
+        d_poly_a = f.d_polya.p;
+        g.st_poly_a = true;
+    }
     CgFastqFilter flt;
     flt.minimum_length = fp->minimum_length;
     flt.maximum_length = fp->maximum_length;
@@ -1843,9 +1869,119 @@ static int fastq_stage_verdict(cg_ctx *c, FastqSlot &f, const cg_fastq_params *f
     flt.action = g.action;
     CU(cg_launch_fastq_evaluate(f.d_in.p, f.d_rec.p, f.d_len.p, g.n, g.d_matches, g.times, g.slots, g.d_qtrim, flt,
                                 c->d_phred, g.d_is_rc, f.d_interval.p, f.d_keep.p, f.d_mask.p, f.d_counters + 1, f.d_err,
-                                st));
+                                st, d_poly_a));
     c->launches += 1;
     return CG_OK;
+}
+
+// ---- statistics of the FASTQ path (cg_fastq_stats_*) ----
+// Vector: the cg_stats_* layout at (n_adapters, max_len, kmax), then reverse_complemented[n_adapters], then the
+// poly-A histogram [max_len + 1].
+static long long fqstats_total(int n_adapters, int max_len, int kmax)
+{
+    return cg_stats_total(n_adapters, max_len, kmax) + n_adapters + (max_len + 1);
+}
+
+// Lay the accumulator out at a larger (max_len, kmax); every count keeps its (length, errors) cell.
+static void fqstats_grow(FqStatsAcc &a, int max_len, int kmax)
+{
+    max_len = std::max(max_len, a.max_len);
+    kmax = std::max(kmax, a.kmax);
+    if (max_len == a.max_len && kmax == a.kmax) return;
+    const int n = a.n_adapters, L0 = a.max_len, K0 = a.kmax;
+    std::vector<int64_t> v((size_t)fqstats_total(n, max_len, kmax), 0);
+    for (int i = 0; i < CG_STATS_SCALARS; ++i) v[i] = a.v[i];
+    for (int l = 0; l <= L0; ++l) v[CG_STATS_SCALARS + l] = a.v[CG_STATS_SCALARS + l];
+    const long long e0 = cg_stats_end_size(L0, K0), e1 = cg_stats_end_size(max_len, kmax);
+    const long long b0 = cg_stats_adapters_off(L0), b1 = cg_stats_adapters_off(max_len);
+    for (long long e = 0; e < 2LL * n; ++e) {
+        const int64_t *src = a.v.data() + b0 + e * e0;
+        int64_t *dst = v.data() + b1 + e * e1;
+        for (int j = 0; j < CG_STATS_ADJ; ++j) dst[j] = src[j];
+        for (int l = 0; l <= L0; ++l)
+            for (int k = 0; k <= K0; ++k)
+                dst[CG_STATS_ADJ + (long long)l * (kmax + 1) + k] = src[CG_STATS_ADJ + (long long)l * (K0 + 1) + k];
+    }
+    const long long t0 = cg_stats_total(n, L0, K0), t1 = cg_stats_total(n, max_len, kmax);
+    for (int i = 0; i < n; ++i) v[t1 + i] = a.v[t0 + i];
+    for (int l = 0; l <= L0; ++l) v[t1 + n + l] = a.v[t0 + n + l];
+    a.v.swap(v);
+    a.max_len = max_len;
+    a.kmax = kmax;
+}
+
+// The accumulator a collect adds to (*out = nullptr: statistics off); it must count as many adapters as the set has.
+static int fqstats_lookup(cg_ctx *c, int32_t handle, int n_adapters, FqStatsAcc **out)
+{
+    *out = nullptr;
+    if (handle == 0) return CG_OK;
+    auto it = c->fq_stats.find(handle);
+    if (it == c->fq_stats.end()) return fail(CG_EINVAL, "cg_fastq: unknown statistics handle " + std::to_string(handle));
+    if (it->second.n_adapters != n_adapters)
+        return fail(CG_EINVAL, "cg_fastq: the statistics accumulator was created for " +
+                                   std::to_string(it->second.n_adapters) + " adapters, the adapter set has " +
+                                   std::to_string(n_adapters));
+    *out = &it->second;
+    return CG_OK;
+}
+
+// Per-adapter statistics of a mate's reads from their final match records (cg_stats_kernel on the packed reads in the
+// orientation that was kept; the read-length histogram is left to the written records) into the slot's vector, laid
+// out at the accumulator's (max_len, kmax) grown to this chunk's longest read and the set's largest error count.
+static int fastq_stage_stats(cg_ctx *c, FastqSlot &f, FqStage &g, int kmax, cudaStream_t st)
+{
+    if (!g.acc || g.n == 0) return CG_OK;
+    int rc;
+    if (!g.packed && (rc = fastq_stage_pack(c, f, st, g, false)) != CG_OK) return rc;   // the longest read
+    FqStatsAcc &a = *g.acc;
+    fqstats_grow(a, g.max_len, kmax);
+    g.st_len = a.max_len;
+    g.st_kmax = a.kmax;
+    const size_t total = (size_t)fqstats_total(a.n_adapters, a.max_len, a.kmax);
+    if ((rc = f.d_fqstats.ensure(total)) != CG_OK) return rc;
+    if ((rc = f.h_fqstats.ensure(total)) != CG_OK) return rc;
+    CU(cudaMemsetAsync(f.d_fqstats.p, 0, total * sizeof(unsigned long long), st));
+    if (g.d_matches && a.n_adapters > 0) {
+        CU(cg_launch_stats(f.d_seq.p, f.d_offs.p, g.n, g.d_qtrim != nullptr, g.times, g.slots, g.d_matches, g.d_qtrim,
+                           a.n_adapters, a.max_len, a.kmax, f.d_fqstats.p, st, nullptr, 0, nullptr, 0,
+                           g.action == CG_FQ_ACTION_LOWERCASE ? 1 : 0));
+        c->launches += 1;
+    }
+    return CG_OK;
+}
+
+// After the finish kernel: written lengths, poly-A lengths, reverse_complemented per adapter; then the vector goes to
+// the host (the output stage waits for it).
+static int fastq_stage_stats_tail(cg_ctx *c, FastqSlot &f, const FqStage &g, cudaStream_t st)
+{
+    if (!g.acc || g.n == 0) return CG_OK;
+    const int n_ad = g.acc->n_adapters;
+    unsigned long long *v = f.d_fqstats.p;
+    const long long tail = cg_stats_total(n_ad, g.st_len, g.st_kmax);
+    CU(cg_launch_fastq_stats_tail(g.n, f.d_interval.p, f.d_outlen.p, g.st_poly_a ? f.d_polya.p : nullptr, g.d_matches,
+                                  g.times, g.slots, g.d_is_rc, n_ad, g.st_len, v + CG_STATS_SCALARS, v + tail + n_ad,
+                                  v + tail, st));
+    c->launches += 1;
+    const size_t total = (size_t)fqstats_total(n_ad, g.st_len, g.st_kmax);
+    CU(cudaMemcpyAsync(f.h_fqstats.p, v, total * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+    return CG_OK;
+}
+
+// The call succeeded: add the chunk's vector; the scalars are those of cg_fastq_result (Statistics.collect takes
+// them from the pipeline and the filters, report.py:128-160), the removed adapter bases from the records.
+static void fastq_stats_commit(const FastqSlot &f, const FqStage &g, const cg_fastq_params *fp, const cg_fastq_result &res)
+{
+    if (!g.acc || g.n == 0) return;
+    FqStatsAcc &a = *g.acc;
+    const unsigned long long *h = f.h_fqstats.p;
+    for (size_t i = CG_STATS_SCALARS; i < a.v.size(); ++i) a.v[i] += (int64_t)h[i];
+    int64_t *v = a.v.data();
+    v[0] += res.n_records; v[1] += res.bp_in; v[2] += res.with_adapters; v[3] += res.quality_trimmed_bp;
+    v[4] += (int64_t)h[4]; v[5] += res.reverse_complemented; v[6] += res.n_written; v[7] += res.bp_out;
+    v[8] += res.too_short; v[9] += res.too_long; v[10] += res.too_many_n; v[11] += res.too_many_expected_errors;
+    v[12] += res.casava_filtered;
+    // --discard-trimmed and --discard-untrimmed exclude each other (cli.py:798-808)
+    v[fp->discard_trimmed ? 13 : 14] += res.discarded;
 }
 
 static int fastq_stage_evaluate(cg_ctx *c, FastqSlot &f, const cg_adapterset *s, const cg_fastq_params *fp, int poly_a_mode,
@@ -1879,6 +2015,10 @@ static int fastq_stage_evaluate(cg_ctx *c, FastqSlot &f, const cg_adapterset *s,
         g.d_matches = f.d_matches.p;
         g.d_is_rc = f.d_isrc.p;
         g.rc_suffix = fp->revcomp == 1;
+        if (g.acc) {                            // the statistics see the reads in the orientation that was kept
+            CU(cg_launch_fastq_gather(f.d_in.p, f.d_rec.p, f.d_offs.p, n, f.d_seq.p, nullptr, 0, st));
+            c->launches += 1;
+        }
     } else if (s) {
         if ((rc = f.d_matches.ensure((size_t)n * g.times * g.slots)) != CG_OK) return rc;
         if ((rc = fastq_stage_pack(c, f, st, g, false)) != CG_OK) return rc;
@@ -1889,6 +2029,7 @@ static int fastq_stage_evaluate(cg_ctx *c, FastqSlot &f, const cg_adapterset *s,
     } else if (g.want_q) {
         if ((rc = fastq_stage_pretrim(c, f, p, st, g)) != CG_OK) return rc;
     }
+    if ((rc = fastq_stage_stats(c, f, g, s ? s->host.max_k : 0, st)) != CG_OK) return rc;
     return fastq_stage_verdict(c, f, fp, poly_a_mode, st, g);
 }
 
@@ -2052,7 +2193,9 @@ static int fastq_collect_impl(cg_ctx *c, int32_t slot, const cg_adapterset *s, c
     f.busy = false;
     memset(res, 0, sizeof *res);
     FqStage g;
-    int rc = fastq_stage_evaluate(c, f, s, fp, 1, f.stream, g);
+    int rc = fqstats_lookup(c, fp->stats, s ? s->host.n_adapters : 0, &g.acc);
+    if (rc != CG_OK) return rc;
+    rc = fastq_stage_evaluate(c, f, s, fp, 1, f.stream, g);
     if (rc != CG_OK || g.n == 0) return rc;
     if (info && (rc = fastq_stage_info(c, f, g, fp, *info, f.stream)) != CG_OK) return rc;
     if (dm && (rc = fastq_stage_route(c, f, nullptr, g.n, *dm, f.stream)) != CG_OK) return rc;
@@ -2060,8 +2203,11 @@ static int fastq_collect_impl(cg_ctx *c, int32_t slot, const cg_adapterset *s, c
                               f.d_counters + 1, nullptr, nullptr, nullptr, 0, nullptr, nullptr, 0, 0, g.rc_suffix,
                               dm ? dm->d_dest : nullptr, dm ? dm->d_dest_keep : nullptr, f.stream, g.fasta_out() ? 1 : 0));
     c->launches += 1;
+    if ((rc = fastq_stage_stats_tail(c, f, g, f.stream)) != CG_OK) return rc;
     if ((rc = fastq_stage_output(c, f, g, f.stream, out, out_capacity, res, dm, segments)) != CG_OK) return rc;
-    return check_err_flag(c);
+    if ((rc = check_err_flag(c)) != CG_OK) return rc;
+    fastq_stats_commit(f, g, fp, *res);
+    return CG_OK;
 }
 
 extern "C" int cg_fastq_collect(cg_ctx *c, int32_t slot, const cg_adapterset *s, const cg_fastq_params *fp,
@@ -2182,6 +2328,13 @@ static int fastq_stage_pair_adapters(cg_ctx *c, FastqSlot &f1, FastqSlot &f2, co
     }
     g1.d_matches = f1.d_matches.p;
     g2.d_matches = f2.d_matches.p;
+    int kmax1 = 0, kmax2 = 0;
+    for (int i = 0; i < pa.n_pairs; ++i) {
+        kmax1 = std::max(kmax1, pa.sets1[i]->host.max_k);
+        kmax2 = std::max(kmax2, pa.sets2[i]->host.max_k);
+    }
+    if ((rc = fastq_stage_stats(c, f1, g1, kmax1, st)) != CG_OK) return rc;
+    if ((rc = fastq_stage_stats(c, f2, g2, kmax2, st)) != CG_OK) return rc;
     if ((rc = fastq_stage_verdict(c, f1, fp1, 1, st, g1)) != CG_OK) return rc;
     return fastq_stage_verdict(c, f2, fp2, 2, st, g2);
 }
@@ -2209,6 +2362,16 @@ static int fastq_collect_paired_impl(cg_ctx *c, int32_t slot1, int32_t slot2, co
     cudaStream_t st = f1.stream;
     FqStage g1, g2;
     int rc;
+    // one statistics accumulator per mate, as the reference keeps per-mate statistics (report.py:162-208)
+    if (fp1->stats != 0 && fp1->stats == fp2->stats) {
+        cudaStreamSynchronize(f2.stream);
+        return fail(CG_EINVAL, "cg_fastq_collect_paired: the two mates need different statistics handles");
+    }
+    if ((rc = fqstats_lookup(c, fp1->stats, pa ? pa->n_pairs : (s1 ? s1->host.n_adapters : 0), &g1.acc)) != CG_OK ||
+        (rc = fqstats_lookup(c, fp2->stats, pa ? pa->n_pairs : (s2 ? s2->host.n_adapters : 0), &g2.acc)) != CG_OK) {
+        cudaStreamSynchronize(f2.stream);
+        return rc;
+    }
     if (pa) {
         CU(cudaStreamSynchronize(f2.stream));
         if ((rc = fastq_stage_pair_adapters(c, f1, f2, *pa, fp1, fp2, st, g1, g2)) != CG_OK) return rc;
@@ -2229,9 +2392,14 @@ static int fastq_collect_paired_impl(cg_ctx *c, int32_t slot1, int32_t slot2, co
                               f2.d_outlen.p, f2.d_counters + 1, pair_filter_mode, mode_untrimmed, 0,
                               dm ? dm->d_dest : nullptr, dm ? dm->d_dest_keep : nullptr, st, g1.fasta_out() ? 1 : 0));
     c->launches += 1;
+    if ((rc = fastq_stage_stats_tail(c, f1, g1, st)) != CG_OK) return rc;
+    if ((rc = fastq_stage_stats_tail(c, f2, g2, st)) != CG_OK) return rc;
     if ((rc = fastq_stage_output(c, f1, g1, st, out1, out_capacity1, res1, dm, segments1)) != CG_OK) return rc;
     if ((rc = fastq_stage_output(c, f2, g2, st, out2, out_capacity2, res2, dm, segments2)) != CG_OK) return rc;
-    return check_err_flag(c);
+    if ((rc = check_err_flag(c)) != CG_OK) return rc;
+    fastq_stats_commit(f1, g1, fp1, *res1);
+    fastq_stats_commit(f2, g2, fp2, *res2);
+    return CG_OK;
 }
 
 extern "C" int cg_fastq_collect_paired(cg_ctx *c, int32_t slot1, int32_t slot2, const cg_adapterset *s1,
@@ -2292,4 +2460,42 @@ extern "C" int cg_fastq_trim_chunk(cg_ctx *c, const cg_adapterset *s, const uint
     int rc = cg_fastq_submit(c, fastq, n_bytes, &slot);
     if (rc != CG_OK) return rc;
     return cg_fastq_collect(c, slot, s, fp, out, out_capacity, res);
+}
+
+extern "C" int cg_fastq_stats_create(cg_ctx *c, int32_t n_adapters, int32_t *handle)
+{
+    if (!c || !handle || n_adapters < 0) return fail(CG_EINVAL, "cg_fastq_stats_create: bad argument");
+    FqStatsAcc a;
+    a.n_adapters = n_adapters;
+    a.v.assign((size_t)fqstats_total(n_adapters, 0, 0), 0);
+    const int32_t h = c->fq_stats_next++;
+    c->fq_stats[h] = std::move(a);
+    *handle = h;
+    return CG_OK;
+}
+
+extern "C" int cg_fastq_stats_read(cg_ctx *c, int32_t handle, int32_t *max_len, int32_t *kmax, int64_t *out, int64_t capacity,
+                                   int64_t *size, int reset)
+{
+    if (!c) return fail(CG_EINVAL, "cg_fastq_stats_read: ctx is NULL");
+    auto it = c->fq_stats.find(handle);
+    if (it == c->fq_stats.end()) return fail(CG_EINVAL, "cg_fastq_stats_read: unknown handle " + std::to_string(handle));
+    FqStatsAcc &a = it->second;
+    const int64_t n = (int64_t)a.v.size();
+    if (max_len) *max_len = a.max_len;
+    if (kmax) *kmax = a.kmax;
+    if (size) *size = n;
+    if (!out) return CG_OK;
+    if (capacity < n)
+        return fail(CG_EINVAL, "cg_fastq_stats_read: the vector has " + std::to_string(n) + " entries, capacity is " +
+                                   std::to_string(capacity));
+    memcpy(out, a.v.data(), (size_t)n * sizeof(int64_t));
+    if (reset) std::fill(a.v.begin(), a.v.end(), 0);
+    return CG_OK;
+}
+
+extern "C" int cg_fastq_stats_destroy(cg_ctx *c, int32_t handle)
+{
+    if (!c || !c->fq_stats.erase(handle)) return fail(CG_EINVAL, "cg_fastq_stats_destroy: unknown handle");
+    return CG_OK;
 }

@@ -1334,12 +1334,15 @@ CG_HD void process_read(const SetView &S, const uint8_t *seq, const uint8_t *qua
 //   recs  : times x slots records of this read
 // Window bookkeeping as the reference does it: the rounds work on what the previous ones left
 // (modifiers.py:225-231), a linked adapter's 3' part on what its 5' part left (adapters.py:1220-1222).
+// upper: the adjacent base is read from the upper-cased read (--action=lowercase upper-cases the read before
+// matching, modifiers.py:222-223).
 // ---------------------------------------------------------------------------------------
 struct StatsScalars { unsigned long long bp, with_adapters, qtrim_bp, adapter_bp; };
 
 template <class Add>
 CG_HD void stats_read_core(const uint8_t *seq, int len, bool have_qtrim, int qs, int qe, const cg_match_rec *recs,
-                           int times, int slots, int n_adapters, int max_len, int kmax, StatsScalars &sc, Add add)
+                           int times, int slots, int n_adapters, int max_len, int kmax, StatsScalars &sc, Add add,
+                           bool upper = false)
 {
     sc.bp += (unsigned long long)len;
     int ws = 0, we = len;                                   // current window [ws, we) of the original read
@@ -1367,7 +1370,8 @@ CG_HD void stats_read_core(const uint8_t *seq, int len, bool have_qtrim, int qs,
                     int k = 4;
                     const int pos = ws + m.rstart - 1;
                     if (m.rstart > 0 && pos >= 0 && pos < len) {
-                        const uint8_t c = seq[pos];
+                        uint8_t c = seq[pos];
+                        if (upper && c >= 'a' && c <= 'z') c = (uint8_t)(c - 32);
                         k = c == 'A' ? 0 : (c == 'C' ? 1 : (c == 'G' ? 2 : (c == 'T' ? 3 : 4)));
                     }
                     add(blk + k, 1u);

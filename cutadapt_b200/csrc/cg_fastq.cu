@@ -429,7 +429,8 @@ __global__ void fq_pretrim_kernel(const uint8_t *buf, const CgFastqRecord *rec, 
 __global__ void fq_evaluate_kernel(const uint8_t *buf, const CgFastqRecord *rec, const int32_t *seq_len, long long n_records,
                                    const cg_match_rec *matches, int times, int slots, const int32_t *qtrim,
                                    CgFastqFilter f, const double *phred, const uint8_t *is_rc, int32_t *interval,
-                                   int32_t *keep_interval, int32_t *fail_mask, unsigned long long *counters, int *err)
+                                   int32_t *keep_interval, int32_t *fail_mask, unsigned long long *counters, int *err,
+                                   int32_t *poly_a_len)
 {
     const long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     unsigned long long c_adapt = 0, c_qbp = 0;
@@ -445,6 +446,7 @@ __global__ void fq_evaluate_kernel(const uint8_t *buf, const CgFastqRecord *rec,
         if (keep_interval) { keep_interval[2 * r] = v.k0; keep_interval[2 * r + 1] = v.k1; }
         fail_mask[r] = v.mask | ((v.last_adapter + 1) << 8) | ((is_rc && is_rc[r]) ? CG_FQ_MASK_RC : 0);
         c_adapt = v.matched;
+        if (poly_a_len) poly_a_len[r] = v.poly_a_removed;
     }
     c_adapt = __reduce_add_sync(0xFFFFFFFFu, (unsigned)c_adapt);
     for (int d = 16; d; d >>= 1) c_qbp += __shfl_down_sync(0xFFFFFFFFu, c_qbp, d);
@@ -509,6 +511,54 @@ __global__ void fq_finish_kernel(long long n_records, const CgFastqRecord *rec1,
         if (w) { atomicAdd(&counters1[0], (unsigned long long)w); if (counters2) atomicAdd(&counters2[0], (unsigned long long)w); }
         if (bp1) atomicAdd(&counters1[2], bp1);
         if (bp2 && counters2) atomicAdd(&counters2[2], bp2);
+    }
+}
+
+// The parts of the FASTQ statistics vector that the match records do not give, one thread per record:
+//   lengths[L]  written records by written length (ReadLengthStatistics of the writers, statistics.py:5-48)
+//   poly_a[L]   bases removed by PolyATrimmer, 0 included (PolyATrimmer.trimmed_bases, modifiers.py:861-879)
+//   rc[a]       matches on reads that were replaced by their reverse complement (modifiers.py:301-306), counted
+//               for the adapter of the first record of the match (the front part of a linked match)
+// The two histograms are privatised per CTA in shared memory when SMEM (2 x (max_len + 1) counters fit).
+template <bool SMEM>
+__global__ void fq_stats_tail_kernel(long long n_records, const int32_t *interval, const int32_t *out_len,
+                                     const int32_t *poly_a_len, const cg_match_rec *matches, int times, int slots,
+                                     const uint8_t *is_rc, int n_adapters, int max_len, unsigned long long *lengths,
+                                     unsigned long long *poly_a, unsigned long long *rc)
+{
+    extern __shared__ unsigned int s_tail[];
+    const int bins = max_len + 1;
+    if (SMEM) {
+        for (int i = threadIdx.x; i < 2 * bins; i += blockDim.x) s_tail[i] = 0;
+        __syncthreads();
+    }
+    const long long nthreads = (long long)gridDim.x * blockDim.x;
+    for (long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x; r < n_records; r += nthreads) {
+        if (out_len[r] != 0) {
+            int w = interval[2 * r + 1] - interval[2 * r];
+            w = w < 0 ? 0 : (w > max_len ? max_len : w);
+            if (SMEM) atomicAdd(&s_tail[w], 1u); else atomicAdd(&lengths[w], 1ull);
+        }
+        if (poly_a_len) {
+            int p = poly_a_len[r];
+            p = p < 0 ? 0 : (p > max_len ? max_len : p);
+            if (SMEM) atomicAdd(&s_tail[bins + p], 1u); else atomicAdd(&poly_a[p], 1ull);
+        }
+        if (is_rc && is_rc[r] && matches)
+            for (int t = 0; t < times; ++t)            // one match per round: a linked match counts once, for
+                for (int k = 0; k < slots; ++k) {      // the part that comes first
+                    const int a = matches[((size_t)r * times + t) * slots + k].adapter;
+                    if (a < 0) continue;
+                    if (a < n_adapters) atomicAdd(&rc[a], 1ull);
+                    break;
+                }
+    }
+    if (SMEM) {
+        __syncthreads();
+        for (int i = threadIdx.x; i < 2 * bins; i += blockDim.x) {
+            const unsigned v = s_tail[i];
+            if (v) atomicAdd(i < bins ? &lengths[i] : &poly_a[i - bins], (unsigned long long)v);
+        }
     }
 }
 
@@ -979,13 +1029,35 @@ cudaError_t cg_launch_fastq_evaluate(const uint8_t *d_buf, const CgFastqRecord *
                                      long long n_records, const cg_match_rec *d_matches, int times, int slots,
                                      const int32_t *d_qtrim, CgFastqFilter f, const double *d_phred, const uint8_t *d_is_rc,
                                      int32_t *d_interval, int32_t *d_keep_interval, int32_t *d_fail_mask,
-                                     unsigned long long *d_counters, int *d_err, cudaStream_t st)
+                                     unsigned long long *d_counters, int *d_err, cudaStream_t st, int32_t *d_poly_a_len)
 {
     if (n_records <= 0) return cudaSuccess;
     fq_evaluate_kernel<<<(unsigned)((n_records + 255) / 256), 256, 0, st>>>(d_buf, d_rec, d_seq_len, n_records, d_matches,
                                                                            times, slots, d_qtrim, f, d_phred, d_is_rc,
                                                                            d_interval, d_keep_interval, d_fail_mask,
-                                                                           d_counters, d_err);
+                                                                           d_counters, d_err, d_poly_a_len);
+    return cudaGetLastError();
+}
+
+cudaError_t cg_launch_fastq_stats_tail(long long n_records, const int32_t *d_interval, const int32_t *d_out_len,
+                                       const int32_t *d_poly_a_len, const cg_match_rec *d_matches, int times, int slots,
+                                       const uint8_t *d_is_rc, int n_adapters, int max_len, unsigned long long *d_lengths,
+                                       unsigned long long *d_poly_a, unsigned long long *d_rc, cudaStream_t st)
+{
+    if (n_records <= 0) return cudaSuccess;
+    const int block = 256;
+    long long grid = (n_records + block - 1) / block;
+    grid = cg_grid_cap(grid, 8);
+    const size_t smem = (size_t)2 * (max_len + 1) * sizeof(unsigned int);
+    // a CTA counts at most n_records / grid records, so 32-bit shared counters cannot overflow below 2^31 of them
+    if (smem <= 48 * 1024 && n_records / grid < (1LL << 31))
+        fq_stats_tail_kernel<true><<<(unsigned)grid, block, smem, st>>>(n_records, d_interval, d_out_len, d_poly_a_len,
+                                                                       d_matches, times, slots, d_is_rc, n_adapters, max_len,
+                                                                       d_lengths, d_poly_a, d_rc);
+    else
+        fq_stats_tail_kernel<false><<<(unsigned)grid, block, 0, st>>>(n_records, d_interval, d_out_len, d_poly_a_len,
+                                                                     d_matches, times, slots, d_is_rc, n_adapters, max_len,
+                                                                     d_lengths, d_poly_a, d_rc);
     return cudaGetLastError();
 }
 

@@ -158,6 +158,7 @@ struct FqVerdict {
     int k0, k1;              // the part the action leaves untouched ("remainder")
     int mask;                // one bit per failed filter (see below)
     int last_adapter;        // adapter of the most recent match, -1 = none
+    int poly_a_removed;      // bases PolyATrimmer removed (0 without --poly-a): its trimmed_bases key
     bool matched;
     bool bad_quality;        // --max-ee met a quality character outside [33, 126]
 };
@@ -175,6 +176,7 @@ CG_HD FqVerdict fq_evaluate_core(const uint8_t *buf, const CgFastqRecord &rec, i
 {
     FqVerdict v;
     v.bad_quality = false;
+    v.poly_a_removed = 0;
     int start = 0, stop = n;
     if (has_qtrim) { start = qs; stop = qe; }
     bool matched = false;
@@ -252,6 +254,7 @@ CG_HD FqVerdict fq_evaluate_core(const uint8_t *buf, const CgFastqRecord &rec, i
             }
             if (best_index < 3) best_index = 0;
             start += best_index;
+            v.poly_a_removed = best_index;
         } else {                                       // poly-A tail: read[:index]
             int best_index = len;
             for (int i = len - 1; i >= 0; --i) {
@@ -260,6 +263,7 @@ CG_HD FqVerdict fq_evaluate_core(const uint8_t *buf, const CgFastqRecord &rec, i
             }
             if (best_index > len - 3) best_index = len;
             stop = start + best_index;
+            v.poly_a_removed = len - best_index;
         }
     }
     if (f.shorten > 0) {                               // Shortener (modifiers.py:882-899): read[:length]

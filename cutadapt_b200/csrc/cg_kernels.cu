@@ -1517,14 +1517,15 @@ template <bool SMEM_HIST>
 __global__ void cg_stats_kernel(const uint8_t *seq, const int64_t *offsets, long long n_reads, int quality_trim, int times,
                                 int slots, const cg_match_rec *matches, const int32_t *qtrim,
                                 int n_adapters, int max_len, int kmax, unsigned long long *stats,
-                                const uint4 *task_list, int task_rec, const unsigned long long *task_count)
+                                const uint4 *task_list, int task_rec, const unsigned long long *task_count,
+                                int count_lengths, int upper)
 {
     // per-CTA histograms in shared memory (32-bit counts, flushed once): the read-length histogram always (every
     // read adds to it, mostly to the same few bins), the per-adapter part if it fits (SMEM_HIST); a global
     // histogram would otherwise take one contended atomic per read
     extern __shared__ unsigned int s_hist[];
     const long long nbins = cg_stats_total(n_adapters, max_len, kmax) - CG_STATS_SCALARS;
-    const long long n_local = SMEM_HIST ? nbins : (long long)(max_len + 1);
+    const long long n_local = SMEM_HIST ? nbins : (count_lengths ? (long long)(max_len + 1) : 0);
     for (long long i = threadIdx.x; i < n_local; i += blockDim.x) s_hist[i] = 0;
     __syncthreads();
     const long long nthreads = (long long)gridDim.x * blockDim.x;
@@ -1550,9 +1551,11 @@ __global__ void cg_stats_kernel(const uint8_t *seq, const int64_t *offsets, long
         stats_read_core(seq ? seq + o0 : nullptr, len, hq, hq ? qtrim[2 * r] : 0, hq ? qtrim[2 * r + 1] : len,
                         matches + (size_t)r * times * slots, times, slots, n_adapters, max_len, kmax, sc,
                         [&](long long idx, unsigned int v) {
+                            if (!count_lengths && idx <= max_len) return;
                             if (idx < n_local) atomicAdd(&s_hist[idx], v);
                             else atomicAdd(&hist[idx], (unsigned long long)v);
-                        });
+                        },
+                        upper != 0);
     }
     // warp-reduce the scalar counters, one atomic per warp
     for (int o = 16; o > 0; o >>= 1) {
@@ -1576,23 +1579,26 @@ __global__ void cg_stats_kernel(const uint8_t *seq, const int64_t *offsets, long
 cudaError_t cg_launch_stats(const uint8_t *d_seq, const int64_t *d_offsets, long long n_reads, int quality_trim, int times,
                             int slots, const cg_match_rec *d_matches, const int32_t *d_qtrim,
                             int n_adapters, int max_len, int kmax, unsigned long long *d_stats,
-                            cudaStream_t st, const uint4 *d_task_list, int task_rec, const unsigned long long *d_task_count)
+                            cudaStream_t st, const uint4 *d_task_list, int task_rec, const unsigned long long *d_task_count,
+                            int count_lengths, int upper)
 {
     const int block = 256;
     long long grid = (n_reads + block - 1) / block;
     grid = cg_grid_cap(grid, 8);
     if (grid < 1) grid = 1;
     const size_t hist_bytes = (size_t)(cg_stats_total(n_adapters, max_len, kmax) - CG_STATS_SCALARS) * sizeof(unsigned int);
-    const size_t len_bytes = (size_t)(max_len + 1) * sizeof(unsigned int);
+    const size_t len_bytes = count_lengths ? (size_t)(max_len + 1) * sizeof(unsigned int) : 0;
     if (len_bytes > 48 * 1024) return cudaErrorInvalidValue;
     // a CTA handles n_reads / grid reads, so 32-bit per-CTA counts cannot overflow below 2^32 reads per CTA
     if (hist_bytes <= 48 * 1024 && n_reads / grid < (1LL << 31))
         cg_stats_kernel<true><<<(int)grid, block, hist_bytes, st>>>(d_seq, d_offsets, n_reads, quality_trim, times, slots,
                                                                      d_matches, d_qtrim, n_adapters, max_len, kmax, d_stats,
-                                                                     d_task_list, task_rec, d_task_count);
+                                                                     d_task_list, task_rec, d_task_count, count_lengths,
+                                                                     upper);
     else
         cg_stats_kernel<false><<<(int)grid, block, len_bytes, st>>>(d_seq, d_offsets, n_reads, quality_trim, times, slots,
                                                                      d_matches, d_qtrim, n_adapters, max_len, kmax, d_stats,
-                                                                     d_task_list, task_rec, d_task_count);
+                                                                     d_task_list, task_rec, d_task_count, count_lengths,
+                                                                     upper);
     return cudaGetLastError();
 }

@@ -66,7 +66,9 @@ cudaError_t cg_launch_stats(const uint8_t *d_seq, const int64_t *d_offsets, long
                             int slots, const cg_match_rec *d_matches, const int32_t *d_qtrim,
                             int n_adapters, int max_len, int kmax, unsigned long long *d_stats,
                             cudaStream_t st, const uint4 *d_task_list = nullptr, int task_rec = 0,
-                            const unsigned long long *d_task_count = nullptr);   // task list: only its reads
+                            const unsigned long long *d_task_count = nullptr,    // task list: only its reads
+                            int count_lengths = 1,     // 0: leave the read-length histogram alone
+                            int upper = 0);            // adjacent bases of the upper-cased read (--action=lowercase)
 cudaError_t cg_launch_nextseq_trim(const uint8_t *d_seq, const uint8_t *d_qual, const int64_t *d_offsets,
                                    long long n_reads, int cutoff, int base, int32_t *d_out, cudaStream_t st);
 cudaError_t cg_launch_poly_a_trim(const uint8_t *d_seq, const int64_t *d_offsets, long long n_reads, int revcomp,
@@ -126,7 +128,15 @@ cudaError_t cg_launch_fastq_evaluate(const uint8_t *d_buf, const CgFastqRecord *
                                      long long n_records, const cg_match_rec *d_matches, int times, int slots,
                                      const int32_t *d_qtrim, CgFastqFilter f, const double *d_phred, const uint8_t *d_is_rc,
                                      int32_t *d_interval, int32_t *d_keep_interval, int32_t *d_fail_mask,
-                                     unsigned long long *d_counters, int *d_err, cudaStream_t st);
+                                     unsigned long long *d_counters, int *d_err, cudaStream_t st,
+                                     int32_t *d_poly_a_len = nullptr);   // optional: bases PolyATrimmer removed, per read
+// statistics of the FASTQ path beyond the match records (after the finish kernel): written lengths of the records with
+// d_out_len != 0, the poly-A histogram (d_poly_a_len may be null), reverse_complemented per adapter (per match of the
+// records with d_is_rc set; d_is_rc may be null); every histogram has max_len + 1 bins
+cudaError_t cg_launch_fastq_stats_tail(long long n_records, const int32_t *d_interval, const int32_t *d_out_len,
+                                       const int32_t *d_poly_a_len, const cg_match_rec *d_matches, int times, int slots,
+                                       const uint8_t *d_is_rc, int n_adapters, int max_len, unsigned long long *d_lengths,
+                                       unsigned long long *d_poly_a, unsigned long long *d_rc, cudaStream_t st);
 // verdict per read (second mate = nullptr) or pair -> sizes of the output records, filter counters
 cudaError_t cg_launch_fastq_finish(long long n_records, const CgFastqRecord *d_rec1, const int32_t *d_interval1,
                                    const int32_t *d_mask1, int enabled1, int32_t *d_out_len1,

@@ -812,6 +812,8 @@ int cg_build_set(const cg_adapter_desc *ads, int n_adapters, const cg_group_desc
         memcpy(out.blob.data() + H.plane_off, plane_kmers.data(), plane_kmers.size());
     if (!pool.empty()) memcpy(out.blob.data() + H.pool_off, pool.data(), pool.size());
     out.n_adapters = n_adapters; out.n_groups = n_groups; out.simple_ok = simple_ok;
+    out.max_k = 0;
+    for (int a = 0; a < n_adapters; ++a) out.max_k = std::max(out.max_k, std::max(0, (int)(ads[a].max_error_rate * ads[a].length)));
     out.all_indexed = n_groups > 0;
     for (int g = 0; g < n_groups; ++g) out.all_indexed = out.all_indexed && G[g].type == CG_GROUP_INDEXED;
     if (out.masks64.empty()) out.masks64.assign(128, 0);   // never hand the kernel a null table

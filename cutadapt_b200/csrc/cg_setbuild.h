@@ -16,6 +16,7 @@ struct CgBuiltSet {
     int slots = 1;
     int n_adapters = 0, n_groups = 0, max_m = 0, any_wide = 0, simple_ok = 0;
     int all_indexed = 0;             // every group is an index lookup (IndexedPrefixAdapters / IndexedSuffixAdapters)
+    int max_k = 0;                   // most errors any adapter can report: max (int)(max_error_rate * length)
 };
 
 // 3 x 256 bytes: upper, acgt, iupac  (src/cutadapt/_match_tables.py:4-66)

@@ -91,6 +91,109 @@ def adapter_statistics_from_vector(stats, adapters, max_len: int, kmax: int):
     return out
 
 
+# ---- statistics of the FASTQ path (include/cutadapt_b200.h: cg_fastq_stats_read) ----------------------------------
+
+def fastq_stats_layout(n_adapters: int, max_len: int, kmax: int) -> dict:
+    """``stats_layout`` plus the tail of the FASTQ path's vector: reverse_complemented per adapter, then the poly-A
+    histogram (max_len + 1 entries)."""
+    lay = stats_layout(n_adapters, max_len, kmax)
+    lay["reverse_complemented"] = lay["size"]
+    lay["poly_a"] = lay["size"] + n_adapters
+    lay["size"] = lay["poly_a"] + max_len + 1
+    return lay
+
+
+def relayout_statistics(stats, n_adapters: int, max_len: int, kmax: int, new_max_len: int, new_kmax: int,
+                        tail: bool = True) -> np.ndarray:
+    """The statistics vector laid out at a larger (new_max_len, new_kmax): every count keeps its (length, errors)
+    cell, the new cells are 0.  ``tail``: the vector of the FASTQ path (fastq_stats_layout), else stats_layout."""
+    if new_max_len < max_len or new_kmax < kmax:
+        raise ValueError("relayout_statistics only grows the layout")
+    stats = np.asarray(stats)
+    layout = fastq_stats_layout if tail else stats_layout
+    old, new = layout(n_adapters, max_len, kmax), layout(n_adapters, new_max_len, new_kmax)
+    if stats.size != old["size"]:
+        raise ValueError(f"the vector has {stats.size} entries, the layout {old['size']}")
+    out = np.zeros(new["size"], dtype=stats.dtype)
+    out[:_SCALARS + max_len + 1] = stats[:_SCALARS + max_len + 1]
+    for block in range(2 * n_adapters):
+        src = old["adapters"] + block * old["end_size"]
+        dst = new["adapters"] + block * new["end_size"]
+        out[dst:dst + _ADJ] = stats[src:src + _ADJ]
+        hist = stats[src + _ADJ:src + old["end_size"]].reshape(old["hist_shape"])
+        out[dst + _ADJ:dst + new["end_size"]].reshape(new["hist_shape"])[:max_len + 1, :kmax + 1] = hist
+    if tail:
+        out[new["reverse_complemented"]:new["reverse_complemented"] + n_adapters] = \
+            stats[old["reverse_complemented"]:old["reverse_complemented"] + n_adapters]
+        out[new["poly_a"]:new["poly_a"] + max_len + 1] = stats[old["poly_a"]:old["poly_a"] + max_len + 1]
+    return out
+
+
+def _histogram(counts) -> dict:
+    return {int(i): int(counts[i]) for i in np.nonzero(np.asarray(counts))[0]}
+
+
+def fastq_adapter_statistics(stats, adapters, max_len: int, kmax: int):
+    """AdapterStatistics of every adapter from a vector of the FASTQ path, ``reverse_complemented`` filled in from
+    its tail (a linked adapter's count is on its front or back part, whichever its match starts with)."""
+    from .adapters import LinkedAdapter
+
+    stats = np.asarray(stats)
+    singles = adapters._flatten()[0]
+    number = {id(s): i for i, s in enumerate(singles)}
+    rc = stats[fastq_stats_layout(len(singles), max_len, kmax)["reverse_complemented"]:][:len(singles)]
+    out = adapter_statistics_from_vector(stats, adapters, max_len, kmax)
+    for st in out:
+        a = st.adapter
+        parts = (a.front_adapter, a.back_adapter) if isinstance(a, LinkedAdapter) else (a,)
+        st.reverse_complemented = int(sum(rc[number[id(p)]] for p in parts))
+    return out
+
+
+def pair_adapter_statistics_from_vector(stats, adapters: Sequence, max_len: int, kmax: int):
+    """One mate's AdapterStatistics under --pair-adapters (PairedAdapterCutter.adapter_statistics[i],
+    modifiers.py:437-442): adapter i of the list is block i of the vector."""
+    stats = np.asarray(stats)
+    lay = stats_layout(len(adapters), max_len, kmax)
+    out = []
+    for i, adapter in enumerate(adapters):
+        st = adapter.create_statistics()
+        for end_stats, end in ((st.front, 0), (st.back, 1)):
+            if end_stats is not None:
+                adjacent, hist = end_block(stats, lay, i, end)
+                end_stats.add_counts(hist, adjacent if end == 1 else None)
+        out.append(st)
+    return out
+
+
+def poly_a_trimmed_lengths(stats, n_adapters: int, max_len: int, kmax: int) -> dict:
+    """{bases removed: reads} of PolyATrimmer (its trimmed_bases, modifiers.py:861-879), from a FASTQ-path vector."""
+    off = fastq_stats_layout(n_adapters, max_len, kmax)["poly_a"]
+    return _histogram(np.asarray(stats)[off:off + max_len + 1])
+
+
+def written_lengths(stats, max_len: int) -> dict:
+    """{length: records} of the written records (ReadLengthStatistics, statistics.py:5-48)."""
+    return _histogram(np.asarray(stats)[_SCALARS:_SCALARS + max_len + 1])
+
+
+def allreduce_fastq_statistics_vector(stats, n_adapters: int, max_len: int, kmax: int, group=None, device=None):
+    """Merge the FASTQ-path statistics vectors of all ranks: one MAX all-reduce of (max_len, kmax), every rank lays
+    its vector out at the result, then one SUM all-reduce.  Returns (vector, max_len, kmax)."""
+    import torch
+    import torch.distributed as dist
+
+    if dist.is_available() and dist.is_initialized() and dist.get_world_size(group) > 1:
+        shape = torch.tensor([max_len, kmax], dtype=torch.int64, device=device)
+        dist.all_reduce(shape, op=dist.ReduceOp.MAX, group=group)
+        new_len, new_kmax = (int(x) for x in shape.tolist())
+    else:
+        new_len, new_kmax = max_len, kmax
+    t = torch.from_numpy(relayout_statistics(stats, n_adapters, max_len, kmax, new_len, new_kmax)).to(device)
+    allreduce_statistics(t, group)
+    return t.cpu().numpy(), new_len, new_kmax
+
+
 def shard_range(n_items: int, rank: int, world_size: int) -> Tuple[int, int]:
     """Contiguous, near-equal split of ``n_items`` reads over ``world_size`` ranks."""
     base, extra = divmod(n_items, world_size)
@@ -804,6 +907,9 @@ class FastqTrimmer:
                         ReverseComplementer, modifiers.py:264-308), all on the device
     input_format        "fastq" (default) or "fasta" (read_fasta_chunks; no quality options then)
     output_format       None (the input's format) or "fasta" (FASTQ in, FASTA out: a .fasta / .fa output or --fasta)
+    collect_statistics  also collect what the report needs beyond the counters (cg_fastq_stats_*): per-adapter
+                        statistics, the poly-A and written-length histograms; ``statistics_vector()``,
+                        ``adapter_statistics()``, ``poly_a_trimmed_lengths``, ``written_lengths``
 
     ``process_chunk(bytes) -> bytes``; ``process_chunks(iterable)`` keeps one chunk in flight so that the
     upload of chunk i+1 overlaps the download of chunk i.  ``statistics`` accumulates the counters of
@@ -819,12 +925,17 @@ class FastqTrimmer:
                  length: Optional[int] = None, trim_n: bool = False, discard_casava: bool = False,
                  action: Optional[str] = "trim", revcomp: bool = False, rc_suffix: bool = True,
                  input_format: str = "fastq", output_format: Optional[str] = None,
-                 ctx: Optional[_lib.Context] = None):
+                 ctx: Optional[_lib.Context] = None, collect_statistics: bool = False):
         self.ctx = ctx or _lib.default_context()
         self.adapters, self._set = _device_set(adapters, self.ctx)
         self.params = _fastq_params(times, quality_cutoff, quality_base, nextseq_cutoff, minimum_length, maximum_length,
                                     max_n, max_expected_errors, discard_trimmed, discard_untrimmed, cut, poly_a, length,
                                     trim_n, discard_casava, action, revcomp, rc_suffix, input_format, output_format)
+        self._stats = None
+        if collect_statistics:
+            n = len(self.adapters._flatten()[0]) if self.adapters is not None else 0
+            self._stats = _lib.FastqStatistics(self.ctx, n)
+            self.params.stats = self._stats.handle
         self.statistics = {}
         self._out_bufs, self._out_keep = {}, {}
 
@@ -947,6 +1058,43 @@ class FastqTrimmer:
         offsets[1:] = np.cumsum([len(b) for b in blobs])
         return self._process_chunk_rows(chunk, 2, b"".join(blobs), offsets)
 
+    @property
+    def collect_statistics(self) -> bool:
+        return self._stats is not None
+
+    @property
+    def statistics_adapters(self) -> int:
+        """Number of adapters the statistics vector has blocks for (its n_adapters)."""
+        if self._stats is None:
+            raise ValueError("this trimmer does not collect statistics (collect_statistics=False)")
+        return self._stats.n_adapters
+
+    def close(self) -> None:
+        """Release the statistics accumulator now rather than when the trimmer is collected."""
+        if self._stats is not None:
+            self._stats.close()
+
+    def statistics_vector(self) -> Tuple[np.ndarray, int, int]:
+        """(vector, max_len, kmax) of everything trimmed so far (layout: fastq_stats_layout)."""
+        if self._stats is None:
+            raise ValueError("this trimmer does not collect statistics (collect_statistics=False)")
+        return self._stats.read()
+
+    def adapter_statistics(self):
+        """AdapterStatistics of every adapter (AdapterCutter.adapter_statistics / ReverseComplementer's)."""
+        stats, max_len, kmax = self.statistics_vector()
+        return fastq_adapter_statistics(stats, self.adapters, max_len, kmax) if self.adapters is not None else []
+
+    @property
+    def poly_a_trimmed_lengths(self) -> dict:
+        stats, max_len, kmax = self.statistics_vector()
+        return poly_a_trimmed_lengths(stats, self._stats.n_adapters, max_len, kmax)
+
+    @property
+    def written_lengths(self) -> dict:
+        stats, max_len, _ = self.statistics_vector()
+        return written_lengths(stats, max_len)
+
     def process_chunks(self, chunks, copy: bool = True):
         """copy=False yields uint8 array views into per-slot buffers: valid until the next-but-one result."""
         pending = None
@@ -968,7 +1116,9 @@ class PairedFastqTrimmer:
     line gives them for one mate only).  ``pair_filter`` is "any" (default), "both" or "first"
     (PairedEndFilter, steps.py:105-180).  ``input_format`` / ``output_format`` as for FastqTrimmer, for both
     mates (read_paired_fasta_chunks).  ``process_chunk(chunk1, chunk2) -> (bytes, bytes)``;
-    ``statistics`` = (dict for R1, dict for R2).
+    ``statistics`` = (dict for R1, dict for R2).  ``collect_statistics``: as for FastqTrimmer, one accumulator per
+    mate; ``statistics_vector()``, ``adapter_statistics()``, ``poly_a_trimmed_lengths`` and ``written_lengths`` give
+    one value per mate.
     """
 
     MODES = {"any": 0, "both": 1, "first": 2}
@@ -976,7 +1126,7 @@ class PairedFastqTrimmer:
     def __init__(self, adapters1=None, adapters2=None, options1: Optional[dict] = None,
                  options2: Optional[dict] = None, pair_filter: str = "any", pair_adapters: bool = False,
                  input_format: str = "fastq", output_format: Optional[str] = None,
-                 ctx: Optional[_lib.Context] = None):
+                 ctx: Optional[_lib.Context] = None, collect_statistics: bool = False):
         if pair_filter not in self.MODES:
             raise ValueError("pair_filter must be 'any', 'both' or 'first'")
         self.ctx = ctx or _lib.default_context()
@@ -1006,6 +1156,49 @@ class PairedFastqTrimmer:
         else:
             self.adapters1, self._set1 = _device_set(adapters1, self.ctx)
             self.adapters2, self._set2 = _device_set(adapters2, self.ctx)
+        self._stats = None
+        if collect_statistics:
+            if self._pairs is not None:
+                counts = (len(self._pairs), len(self._pairs))
+            else:
+                counts = tuple(len(a._flatten()[0]) if a is not None else 0 for a in (self.adapters1, self.adapters2))
+            self._stats = tuple(_lib.FastqStatistics(self.ctx, n) for n in counts)
+            self.params1.stats, self.params2.stats = self._stats[0].handle, self._stats[1].handle
+
+    @property
+    def collect_statistics(self) -> bool:
+        return self._stats is not None
+
+    def close(self) -> None:
+        """Release the two statistics accumulators now rather than when the trimmer is collected."""
+        for st in self._stats or ():
+            st.close()
+
+    def statistics_vector(self):
+        """((vector, max_len, kmax) of R1, the same of R2)."""
+        if self._stats is None:
+            raise ValueError("this trimmer does not collect statistics (collect_statistics=False)")
+        return tuple(st.read() for st in self._stats)
+
+    def adapter_statistics(self):
+        """(AdapterStatistics of R1's adapters, of R2's): the two lists of PairedAdapterCutter.adapter_statistics
+        under --pair-adapters, else those of the two AdapterCutters."""
+        out = []
+        for (stats, max_len, kmax), adapters in zip(self.statistics_vector(), (self.adapters1, self.adapters2)):
+            if self._pairs is not None:
+                out.append(pair_adapter_statistics_from_vector(stats, adapters, max_len, kmax))
+            else:
+                out.append(fastq_adapter_statistics(stats, adapters, max_len, kmax) if adapters is not None else [])
+        return tuple(out)
+
+    @property
+    def poly_a_trimmed_lengths(self):
+        return tuple(poly_a_trimmed_lengths(v, st.n_adapters, max_len, kmax)
+                     for (v, max_len, kmax), st in zip(self.statistics_vector(), self._stats))
+
+    @property
+    def written_lengths(self):
+        return tuple(written_lengths(v, max_len) for v, max_len, _ in self.statistics_vector())
 
     def _submit(self, chunk):
         buf = np.frombuffer(chunk, dtype=np.uint8) if not isinstance(chunk, np.ndarray) else chunk

@@ -13,14 +13,15 @@ rank with a GPU:
 * the outputs go to rank 0 round by round (one round = ``world`` consecutive chunks) over a host-side gloo group
   -- they are host bytes already -- and rank 0 writes them in chunk order: byte for byte what a single GPU writes;
 * the counters of all ranks are summed once at the end (``allreduce_fastq_statistics``), where the reference adds up
-  the workers' Statistics objects (runners.py:372-373).
+  the workers' Statistics objects (runners.py:372-373); a trimmer that collects statistics also has its statistics
+  vector merged (``allreduce_fastq_statistics_vector``), returned as ``statistics_vector`` = (vector, max_len, kmax).
 
 ``SerialRunner`` is the one-GPU form (``SerialPipelineRunner``, runners.py:415-436).
 """
 import io
 from typing import BinaryIO, Callable, Iterable, Optional
 
-from .pipeline import FastqTrimmer, allreduce_fastq_statistics, read_fastq_chunks
+from .pipeline import FastqTrimmer, allreduce_fastq_statistics, allreduce_fastq_statistics_vector, read_fastq_chunks
 
 
 def _chunks_of(source, buffer_size: int) -> Iterable:
@@ -52,6 +53,8 @@ class SerialRunner:
             n += 1
         stats = dict(self.trimmer.statistics)
         stats["chunks"] = n
+        if getattr(self.trimmer, "collect_statistics", False):
+            stats["statistics_vector"] = self.trimmer.statistics_vector()
         return stats
 
 
@@ -118,4 +121,8 @@ class RoundRobinRunner:
         local = dict(self.trimmer.statistics) if self.trimmer is not None else {}
         total = allreduce_fastq_statistics(local, self._host_group)
         total["chunks"] = n_chunks
+        if getattr(self.trimmer, "collect_statistics", False):
+            vector, max_len, kmax = self.trimmer.statistics_vector()
+            total["statistics_vector"] = allreduce_fastq_statistics_vector(
+                vector, self.trimmer.statistics_adapters, max_len, kmax, self._host_group)
         return total

@@ -332,7 +332,9 @@ typedef struct cg_fastq_params {
                                     orientation is kept.  1 = append " rc" to the name of a replaced read, 2 = do not
                                     (--rename given, cli.py:1082-1116)                                  */
     int32_t format;              /* CG_FORMAT_*: what the chunk is and what is written (below); 0 = FASTQ    */
-    int32_t reserved[2];
+    int32_t stats;               /* 0 = off, else a handle of cg_fastq_stats_create: the call ADDS this mate's
+                                    statistics to that accumulator if it succeeds (cg_fastq_stats_read, below) */
+    int32_t reserved;
 } cg_fastq_params;
 typedef struct cg_fastq_result {
     int64_t n_records, n_written;
@@ -467,6 +469,34 @@ int cg_stats_accumulate_device(cg_ctx *ctx, const cg_adapterset *set, const uint
 int cg_process_batch_stats(cg_ctx *ctx, const cg_adapterset *set, const uint8_t *seq, const uint8_t *qual,
                            const int64_t *offsets, int64_t n_reads, const cg_params *params,
                            cg_match *matches, int32_t *qtrim, int32_t max_len, int32_t kmax, int64_t *stats);
+
+/* ---- statistics of the FASTQ path ------------------------------------------------------------------------
+ * What a worker of the reference collects for its report while it runs a chunk (Statistics.collect, report.py:128-208):
+ * AdapterCutter.adapter_statistics (modifiers.py:109, 200-207), ReverseComplementer's per-adapter reverse_complemented
+ * (modifiers.py:301-306), PolyATrimmer.trimmed_bases (modifiers.py:861-879) and the ReadLengthStatistics of the
+ * writers (report.py:155-157).  An accumulator belongs to a context; a collect adds to the one named by
+ * cg_fastq_params.stats when it returns CG_OK (a failed call, e.g. "output buffer too small", adds nothing).  Every
+ * collect honours it; paired calls take params1.stats / params2.stats, one accumulator per mate (the same handle on
+ * both is CG_EINVAL).  n_adapters must be the number of adapters of the set (cg_adapter_desc entries; 0 without a
+ * set), for --pair-adapters the number of pairs (`adapter` = pair number); otherwise the collect is CG_EINVAL.
+ * Nothing is clamped: max_len grows to the longest read (after -u) seen, kmax to the largest error count any adapter
+ * of the sets can report ((int)(max_error_rate * length)); the vector is laid out anew when they grow.
+ * Vector (int64): the cg_stats_* layout below at (n_adapters, max_len, kmax), with
+ *   [0] n_records [1] bp_in [2] with_adapters [3] quality_trimmed_bp [4] bases removed by the adapter matches
+ *   [5] reverse_complemented [6] n_written [7] bp_out [8..14] the filter counts of the result struct; discarded goes
+ *   to [13] with discard_trimmed, else to [14]
+ *   read-length histogram: WRITTEN records by written length, all outputs of a demultiplexing call together (pairs
+ *   dropped through dest_keep are not counted)
+ *   per adapter and end: every match of every read that went through the cutter, filtered or not; adjacent bases
+ *   as the reference reads them (upper-cased read with CG_ACTION_LOWERCASE)
+ * then the tail: reverse_complemented[n_adapters] (matches on reads that were replaced by their reverse complement),
+ * poly_a[max_len + 1] (bases PolyATrimmer removed per read, 0 included; empty without --poly-a).
+ * cg_fastq_stats_read reports (max_len, kmax) and the size; with out != NULL it copies the vector (capacity must
+ * hold it) and with reset != 0 then zeroes it. */
+int cg_fastq_stats_create(cg_ctx *ctx, int32_t n_adapters, int32_t *handle);   /* handle > 0 */
+int cg_fastq_stats_read(cg_ctx *ctx, int32_t handle, int32_t *max_len, int32_t *kmax, int64_t *out, int64_t capacity,
+                        int64_t *size, int reset);
+int cg_fastq_stats_destroy(cg_ctx *ctx, int32_t handle);
 
 /* ---- host-side index helpers (adapters.py:1416-1442 use these to build AdapterIndex) ----
  * edit_environment (_align.pyx:785-882) / hamming_sphere-based environment

@@ -1,13 +1,15 @@
 """End-to-end throughput of the FASTQ entry point (not a bench line; see DESIGN.md sections 4.6, 4.7).
 
-  python tools/measure_fastq.py [n_reads] [chunk_megabytes] [fastq | fasta | fasta60]
+  python tools/measure_fastq.py [n_reads] [chunk_megabytes] [fastq | fasta | fasta60 | barcodes] [--statistics]
 
 Builds n_reads synthetic FASTQ records of BASELINE configs[1]'s shape (150 bp, Phred+33 qualities, names
 "@SIM2:000000123") in pinned host memory, cuts the buffer into chunks of whole records and streams them
 through FastqTrimmer.process_chunks (-a AGATCGGAAGAGC -q 20 -m 20): raw FASTQ bytes in, trimmed FASTQ bytes
 out, host -> device -> host inside the timed region.  Prints one JSON line.  "fasta" / "fasta60": the same reads as
 FASTA (">SIM2:000000123" and the sequence on one line / wrapped at 60 columns) through the FASTA path
-(input_format="fasta", -a AGATCGGAAGAGC -m 20: FASTA has no qualities to trim).
+(input_format="fasta", -a AGATCGGAAGAGC -m 20: FASTA has no qualities to trim).  "barcodes": the FASTQ reads with
+the 96 anchored 5' barcodes of config 5 (-g ^BARCODE..., IndexedPrefixAdapters) instead of the 3' adapter.
+--statistics: the trimmer also collects the report's statistics (collect_statistics=True; cg_fastq_stats_*).
 """
 import json
 import sys
@@ -73,10 +75,12 @@ def build_fasta(n, wrap=None, pinned=True):
 
 
 def main():
-    n = int(sys.argv[1]) if len(sys.argv) > 1 else 4_000_000
-    chunk_mb = int(sys.argv[2]) if len(sys.argv) > 2 else 64
-    variant = sys.argv[3] if len(sys.argv) > 3 else "fastq"
-    if variant == "fastq":
+    collect = "--statistics" in sys.argv
+    argv = [a for a in sys.argv if a != "--statistics"]
+    n = int(argv[1]) if len(argv) > 1 else 4_000_000
+    chunk_mb = int(argv[2]) if len(argv) > 2 else 64
+    variant = argv[3] if len(argv) > 3 else "fastq"
+    if variant in ("fastq", "barcodes"):
         data, rec_len = build_fastq(n)
     else:
         data, rec_len = build_fasta(n, wrap=60 if variant == "fasta60" else None)
@@ -84,10 +88,18 @@ def main():
     chunks = [data[i * rec_len:min(n, i + per_chunk) * rec_len] for i in range(0, n, per_chunk)]
     adapters = [PA.BackAdapter("AGATCGGAAGAGC", max_errors=0.1)]
     if variant == "fastq":
-        t = FastqTrimmer(adapters, quality_cutoff=(0, 20), minimum_length=20)
+        t = FastqTrimmer(adapters, quality_cutoff=(0, 20), minimum_length=20, collect_statistics=collect)
         what = "FASTQ bytes in -> trimmed FASTQ bytes out (-a AGATCGGAAGAGC -q 20 -m 20), host to host"
+    elif variant == "barcodes":
+        from cutadapt_b200.configs import config5_barcodes
+
+        barcodes = [PA.PrefixAdapter(b, max_errors=0.1, min_overlap=3, indels=True, name=f"bc{i}")
+                    for i, b in enumerate(config5_barcodes())]
+        t = FastqTrimmer(PA.MultipleAdapters([PA.IndexedPrefixAdapters(barcodes)]), quality_cutoff=(0, 20),
+                         minimum_length=20, collect_statistics=collect)
+        what = "FASTQ bytes in -> trimmed FASTQ bytes out (96 barcodes -g ^BC -q 20 -m 20), host to host"
     else:
-        t = FastqTrimmer(adapters, minimum_length=20, input_format="fasta")
+        t = FastqTrimmer(adapters, minimum_length=20, input_format="fasta", collect_statistics=collect)
         what = f"FASTA ({variant}) bytes in -> trimmed FASTA bytes out (-a AGATCGGAAGAGC -m 20), host to host"
     out_bytes = sum(len(o) for o in t.process_chunks(chunks[:9], copy=False))   # warm-up: every slot's buffers, pool
     t.statistics.clear()
@@ -99,7 +111,7 @@ def main():
     st = t.statistics
     print(json.dumps({
         "what": what,
-        "reads": n, "chunk_mb": chunk_mb, "chunks": len(chunks), "reads_per_s": n / wall,
+        "reads": n, "chunk_mb": chunk_mb, "collect_statistics": collect, "chunks": len(chunks), "reads_per_s": n / wall,
         "in_GB_per_s": data.size / wall / 1e9, "out_GB_per_s": out_bytes / wall / 1e9,
         "in_bytes": int(data.size), "out_bytes": out_bytes, "wall_s": wall,
         "statistics": {k: int(v) for k, v in st.items()},

@@ -12,7 +12,9 @@ on real files.
 
 The input format comes from the first byte of the (first) input, as cutadapt's files.detect_file_format does: '>' or
 '#' is FASTA, anything else (an empty file included) FASTQ.  The output is FASTA when the input is, when -o ends in
-.fasta / .fa, or with --fasta.
+.fasta / .fa, or with --fasta.  --json FILE also writes what the report shows per adapter (removed length x errors,
+bases preceding the adapter, reverse-complemented count), the poly-A and written-length histograms and the counters,
+collected on the device (collect_statistics=True); the stderr line stays as it is.
 """
 import argparse
 import json
@@ -46,6 +48,23 @@ def make_adapters(specs, kind, error_rate, overlap):
     return out
 
 
+def _end(e):
+    if e is None:
+        return None
+    return {"errors": {str(length): {str(k): n for k, n in sorted(row.items())} for length, row in sorted(e.errors.items())},
+            "adjacent_bases": dict(e.adjacent_bases)}
+
+
+def report_json(counters, adapter_statistics, poly_a, written):
+    """One mate's statistics as --json writes them."""
+    return {"counters": counters,
+            "adapters": [{"name": st.name, "reverse_complemented": int(st.reverse_complemented),
+                          "five_prime_end": _end(st.front), "three_prime_end": _end(st.back)}
+                         for st in adapter_statistics],
+            "poly_a_trimmed_lengths": {str(k): v for k, v in sorted(poly_a.items())},
+            "written_lengths": {str(k): v for k, v in sorted(written.items())}}
+
+
 def main():
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     for flag, dest in (("-a", "back"), ("-g", "front"), ("-b", "anywhere"), ("-A", "back2"), ("-G", "front2"),
@@ -74,6 +93,7 @@ def main():
     ap.add_argument("--buffer-size", type=int, default=64 << 20)
     ap.add_argument("-o", "--output", required=True, help="output FASTQ; with {name}: one file per adapter name")
     ap.add_argument("-p", "--paired-output")
+    ap.add_argument("--json", default=None, metavar="FILE", help="write the report's statistics as JSON")
     ap.add_argument("inputs", nargs="+")
     args = ap.parse_args()
     input_format = detect_format(args.inputs[0])
@@ -94,7 +114,7 @@ def main():
                   max_expected_errors=args.max_ee, discard_trimmed=args.discard_trimmed,
                   discard_untrimmed=args.discard_untrimmed, cut=args.cut, poly_a=args.poly_a, length=args.length,
                   trim_n=args.trim_n, discard_casava=args.discard_casava, action=args.action)
-    formats = dict(input_format=input_format, output_format=output_format)
+    formats = dict(input_format=input_format, output_format=output_format, collect_statistics=args.json is not None)
     ads1 = (make_adapters(args.back, "back", args.error_rate, args.overlap)
             + make_adapters(args.front, "front", args.error_rate, args.overlap)
             + make_adapters(args.anywhere, "anywhere", args.error_rate, args.overlap))
@@ -136,6 +156,14 @@ def main():
                 o.write(out.tobytes() if hasattr(out, "tobytes") else out)
         stats = t.statistics
     print(json.dumps(stats), file=sys.stderr)
+    if args.json is not None:
+        if len(args.inputs) == 2:
+            report = {f"read{k + 1}": report_json(t.statistics[k], t.adapter_statistics()[k], t.poly_a_trimmed_lengths[k],
+                                                  t.written_lengths[k]) for k in (0, 1)}
+        else:
+            report = report_json(t.statistics, t.adapter_statistics(), t.poly_a_trimmed_lengths, t.written_lengths)
+        with open(args.json, "w") as f:
+            json.dump(report, f, indent=1)
 
 
 if __name__ == "__main__":
