@@ -209,7 +209,7 @@ def _declare(lib) -> None:
     lib.cg_adapterset_destroy.argtypes = [vp]
     lib.cg_ctx_stage_times.argtypes = [vp, C.POINTER(C.c_double), C.c_int]
     lib.cg_adapterset_jit_status.argtypes = [vp]
-    lib.cg_adapterset_jit_source.argtypes = [vp, C.c_int32, C.c_int32, C.c_char_p, C.c_int64]
+    lib.cg_adapterset_jit_source.argtypes = [vp, C.c_int32, C.c_int32, C.c_int32, C.c_char_p, C.c_int64]
     lib.cg_adapterset_jit_source.restype = C.c_int64
     lib.cg_adapterset_slots.argtypes = [vp]
     lib.cg_adapterset_effective_length.argtypes = [vp, i32, C.POINTER(i32)]
@@ -555,13 +555,14 @@ class AdapterSet:
         (the precompiled kernel runs; last_error() says why)."""
         return int(lib().cg_adapterset_jit_status(self._h))
 
-    def jit_source(self, plane_words: int = 5, has_qual: bool = False) -> str:
-        """The translation unit the run-time specialisation compiles for this set ('' if it has no plane program)."""
-        n = int(lib().cg_adapterset_jit_source(self._h, plane_words, int(has_qual), None, 0))
+    def jit_source(self, plane_words: int = 5, has_qual: bool = False, statistics: bool = False) -> str:
+        """The translation unit the run-time specialisation compiles for this set ('' if it has no plane program);
+        statistics=True: the variant that counts the trim statistics inside the first stage (run_with_statistics)."""
+        n = int(lib().cg_adapterset_jit_source(self._h, plane_words, int(has_qual), int(statistics), None, 0))
         if n == 0:
             return ""
         buf = C.create_string_buffer(n + 1)
-        lib().cg_adapterset_jit_source(self._h, plane_words, int(has_qual), buf, n + 1)
+        lib().cg_adapterset_jit_source(self._h, plane_words, int(has_qual), int(statistics), buf, n + 1)
         return buf.value.decode()
 
     def effective_length(self, adapter: int = 0) -> int:

@@ -210,9 +210,10 @@ struct cg_adapterset {
     std::vector<int32_t> pass_map;
     int32_t *d_pass_map = nullptr;
     CgSelectTables select_tables;
-    // run-time specialisation of the bit-plane first stage (cg_jit.h): one kernel per (plane words, qualities)
-    mutable CgJitKernel *jit[2][2] = {{nullptr, nullptr}, {nullptr, nullptr}};
-    mutable int jit_state[2][2] = {{0, 0}, {0, 0}};      // 0 not tried, 1 ready, -1 failed
+    // run-time specialisation of the bit-plane first stage (cg_jit.h): one kernel per (plane words, qualities,
+    // statistics counted in the stage or not)
+    mutable CgJitKernel *jit[2][2][2] = {};
+    mutable int jit_state[2][2][2] = {};                // 0 not tried, 1 ready, -1 failed
     mutable long long plane_reads = 0;                  // reads that went through the plane stage so far
     mutable std::string jit_error;
 };
@@ -440,7 +441,8 @@ extern "C" int cg_adapterset_destroy(cg_adapterset *s)
     if (s->d_masks) cudaFree(s->d_masks);
     if (s->d_index) cudaFree(s->d_index);
     for (int w = 0; w < 2; ++w)
-        for (int q = 0; q < 2; ++q) cg_jit_destroy(s->jit[w][q]);
+        for (int q = 0; q < 2; ++q)
+            for (int v = 0; v < 2; ++v) cg_jit_destroy(s->jit[w][q][v]);
     destroy_passes(s);
     delete s;
     return CG_OK;
@@ -454,20 +456,22 @@ extern "C" int cg_adapterset_jit_status(const cg_adapterset *s)
     const cg_adapterset *t = (!s->passes.empty() && s->passes[0].sub) ? s->passes[0].sub : s;
     int st = 0;
     for (int w = 0; w < 2; ++w)
-        for (int q = 0; q < 2; ++q) {
-            if (t->jit_state[w][q] == 1) st = 1;
-            else if (t->jit_state[w][q] == -1 && st == 0) st = -1;
-        }
+        for (int q = 0; q < 2; ++q)
+            for (int v = 0; v < 2; ++v) {
+                if (t->jit_state[w][q][v] == 1) st = 1;
+                else if (t->jit_state[w][q][v] == -1 && st == 0) st = -1;
+            }
     if (st == -1) g_err = "first-stage specialisation failed: " + t->jit_error;
     return st;
 }
 
-// The translation unit cg_jit.cpp would compile for this set (plane_words 5 or 8); returns its length (0: the
-// set has no plane program) and copies at most cap - 1 characters.
-extern "C" int64_t cg_adapterset_jit_source(const cg_adapterset *s, int32_t plane_words, int32_t has_qual, char *buf, int64_t cap)
+// The translation unit cg_jit.cpp would compile for this set (plane_words 5 or 8; stats: the variant that counts the
+// trim statistics); returns its length (0: the set has no plane program) and copies at most cap - 1 characters.
+extern "C" int64_t cg_adapterset_jit_source(const cg_adapterset *s, int32_t plane_words, int32_t has_qual, int32_t stats,
+                                            char *buf, int64_t cap)
 {
     if (!s) return 0;
-    const std::string src = cg_jit_pscan_source(s->host, plane_words, has_qual != 0);
+    const std::string src = cg_jit_pscan_source(s->host, plane_words, has_qual != 0, stats != 0);
     if (buf && cap > 0) {
         const size_t n = std::min<size_t>(src.size(), (size_t)cap - 1);
         memcpy(buf, src.data(), n);
@@ -552,7 +556,7 @@ static int launch_trim_single(cg_ctx *c, const cg_adapterset *s, const uint8_t *
                                 : cg_scan_smem_bytes(a.blob_bytes, a.mini_cap, want_q);
             list_smem = cg_dp_smem_bytes(a.blob_bytes, a.carry_slot);
             if (scan_smem <= c->smem_optin && list_smem <= c->smem_optin) {
-                if (plane_w) CU(cg_pscan_occupancy(want_q, plane_w, scan_smem, &scan_occ));
+                if (plane_w) CU(cg_pscan_occupancy(want_q, plane_w, false, scan_smem, &scan_occ));
                 else CU(cg_scan_occupancy(want_q, scan_smem, &scan_occ));
                 CU(cg_list_occupancy(true, s->host.max_m, list_smem, &plan_occ));
                 CU(cg_list_occupancy(false, s->host.max_m, list_smem, &run_occ));
@@ -576,25 +580,44 @@ static int launch_trim_single(cg_ctx *c, const cg_adapterset *s, const uint8_t *
             }
         }
     }
+    // statistics counted inside the pass: one plain adapter, one round, the whole set in this call (not a pass of the
+    // multi-pass schedule), no quality trimming, and the first stage keeps its CTAs per SM with the histogram in shared
+    // memory.  The first stage counts the reads it settles (88 % on the benchmark's reads) while they are in shared
+    // memory, one cg_stats_kernel launch per sub-batch counts the rest from the task list; otherwise
+    // launch_trim_with_stats runs cg_stats_kernel over all records after the pass.  Measured on an H100 (DESIGN.md
+    // section 4.1): 1.4 ms less per step of config 2; with quality trimming (config 4) the first stage grew by more than
+    // the statistics kernel costs, so quality-trimmed passes keep the kernel.
+    bool fuse_stats = split && plane_w && c->fuse.armed && !d_view && s->host.n_adapters == 1 && times == 1 &&
+                      s->host.slots == 1 && !want_q && !getenv("CUTADAPT_B200_TWO_LISTS") && c->fuse.max_len <= 4096;
+    if (fuse_stats) {
+        const size_t fsmem = cg_pscan_smem_bytes(a.blob_bytes, a.mini_cap, want_q, c->fuse.max_len);
+        int focc = 0;
+        if (fsmem <= c->smem_optin) CU(cg_pscan_occupancy(want_q, plane_w, true, fsmem, &focc));
+        fuse_stats = focc >= 1 && focc >= scan_occ;
+        if (fuse_stats) {
+            a.stats = c->fuse.d_stats; a.stats_max_len = c->fuse.max_len; a.stats_kmax = c->fuse.kmax;
+            scan_smem = fsmem; scan_occ = focc;
+        }
+    }
     // Run-time specialisation of the first stage for this adapter set (cg_jit.h): compiled once the set has seen
-    // enough reads to pay for the ~1 s of NVRTC (CUTADAPT_B200_JIT=1: at once, =0: never); any failure keeps the
-    // precompiled interpreter kernel.
+    // enough reads to pay for the ~1 s of NVRTC (CUTADAPT_B200_JIT=1: at once, =0: never), one kernel per variant
+    // (with or without the statistics); any failure keeps the precompiled interpreter kernel.
     CgJitKernel *jit_kernel = nullptr;
     int jit_occ = 0;
     if (split && plane_w) {
-        const int wi = plane_w <= 5 ? 0 : 1, qi = want_q ? 1 : 0;
+        const int wi = plane_w <= 5 ? 0 : 1, qi = want_q ? 1 : 0, vi = fuse_stats ? 1 : 0;
         s->plane_reads += n_reads;
         const char *je = getenv("CUTADAPT_B200_JIT");
         const bool never = je && strcmp(je, "0") == 0, always = je && strcmp(je, "1") == 0;
-        if (!never && s->jit_state[wi][qi] == 0 && (always || s->plane_reads >= (4LL << 20))) {
+        if (!never && s->jit_state[wi][qi][vi] == 0 && (always || s->plane_reads >= (4LL << 20))) {
             std::string err;
-            s->jit[wi][qi] = cg_jit_build_pscan(s->host, plane_w, want_q, err);
-            s->jit_state[wi][qi] = s->jit[wi][qi] ? 1 : -1;
-            if (!s->jit[wi][qi]) s->jit_error = err;
+            s->jit[wi][qi][vi] = cg_jit_build_pscan(s->host, plane_w, want_q, fuse_stats, err);
+            s->jit_state[wi][qi][vi] = s->jit[wi][qi][vi] ? 1 : -1;
+            if (!s->jit[wi][qi][vi]) s->jit_error = err;
         }
-        if (!never && s->jit_state[wi][qi] == 1) {
-            jit_occ = cg_jit_occupancy(s->jit[wi][qi], CG_NT, scan_smem);
-            if (jit_occ >= 1) jit_kernel = s->jit[wi][qi];
+        if (!never && s->jit_state[wi][qi][vi] == 1) {
+            jit_occ = cg_jit_occupancy(s->jit[wi][qi][vi], CG_NT, scan_smem);
+            if (jit_occ >= 1) jit_kernel = s->jit[wi][qi][vi];
         }
     }
     const bool stage_times = getenv("CUTADAPT_B200_STAGE_TIMES") != nullptr;
@@ -605,21 +628,6 @@ static int launch_trim_single(cg_ctx *c, const cg_adapterset *s, const uint8_t *
             else CU(cudaEventCreate(ev));
         }
         CU(cudaEventRecord(ev0, st));
-    }
-    // fused statistics: one plain adapter, one round, the whole set in this call (not a pass of the multi-pass schedule).
-    // Opt-in (CUTADAPT_B200_FUSED_STATS=1, read when the set's kernel is specialised): measured on the 100 M-read bench
-    // it saves 1.1 ms of statistics kernel and costs 0.6 ms in the first stage -- +5 % reads/s for the step, but the
-    // trimming pass itself gets 11 % slower, and the pass is what the roofline is quoted on.
-    const bool fuse_stats = split && plane_w && c->fuse.armed && !d_view && s->host.n_adapters == 1 && times == 1 &&
-                            s->host.slots == 1 && (!want_q || d_qtrim) && !getenv("CUTADAPT_B200_TWO_LISTS") &&
-                            c->fuse.max_len <= 4096 && getenv("CUTADAPT_B200_FUSED_STATS") != nullptr;
-    if (fuse_stats) {
-        a.stats = c->fuse.d_stats; a.stats_max_len = c->fuse.max_len; a.stats_kmax = c->fuse.kmax;
-        scan_smem = cg_pscan_smem_bytes(a.blob_bytes, a.mini_cap, want_q, a.stats_max_len);
-        if (scan_smem > c->smem_optin) return fail(CG_EINVAL, "statistics histogram does not fit the first stage's shared memory");
-        if (jit_kernel) jit_occ = cg_jit_occupancy(jit_kernel, CG_NT, scan_smem);
-        else CU(cg_pscan_occupancy(want_q, plane_w, scan_smem, &scan_occ));
-        if ((jit_kernel ? jit_occ : scan_occ) < 1) return fail(CG_ECUDA, "first stage does not fit with the statistics histogram");
     }
     // sets of index lookups only (demultiplexing), no quality trimming: the light kernel -- nothing to stage
     const bool light = s->host.all_indexed && !want_q && !s->host.any_wide && s->host.max_m + 1 <= CG_LIGHT_ROWS &&
@@ -726,8 +734,8 @@ static int launch_trim_single(cg_ctx *c, const cg_adapterset *s, const uint8_t *
             }
             if (sev[0]) { CU(cudaEventRecord(sev[3], st)); c->stage_events.push_back(sev); }
             if (fuse_stats) {
-                // the reads the first stage handed on: their records are final now
-                if (ev0 && r0 + SUB >= n_reads) { CU(cudaEventRecord(ev1, st)); c->timing.emplace_back(ev0, ev1); ev0 = nullptr; }
+                // the reads the first stage handed on: their records are final now (the event pair of the call
+                // brackets these launches too)
                 CU(cg_launch_stats(b.seq, b.offsets, n_sub, want_q && b.qtrim, 1, 1, b.out, b.qtrim, 1, a.stats_max_len,
                                    a.stats_kmax, a.stats, st, c->tasks.p, plane_rec, cnt));
                 c->launches += 1;

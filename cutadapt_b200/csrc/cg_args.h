@@ -49,7 +49,8 @@ struct CgKernelArgs {
     unsigned long long *task3_count;  //   A/C/G/T go here (2 x uint4, CG_TASK_RESCAN) for a second, dense plan launch
     int no_band;                      // 1: the DP runs keep all rows (CUTADAPT_B200_NO_BAND=1, for A/B runs)
     // statistics fused into the first stage (cg_pscan.cuh): the reads it settles are counted here, the rest by
-    // cg_stats_tasks_kernel over the task list once their records are final.  null = not fused.
+    // cg_stats_kernel over the task list once their records are final.  null = not fused (the variant of the first
+    // stage without the statistics code runs).
     unsigned long long *stats;
     int stats_max_len, stats_kmax;
     // generic-kernel scratch

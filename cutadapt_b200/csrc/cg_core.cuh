@@ -949,6 +949,7 @@ struct RuntimePlaneProg {
     }
     CG_HD static int adapter_length(int m) { return m; }
     CG_HD static unsigned long long overlap_ok(unsigned long long from_blob) { return from_blob; }
+    CG_HD static int remove_kind(int from_blob) { return from_blob; }     // CgAdapter::remove
     template <int W>
     CG_HD static void run(PlaneState<W> &st, const uint32_t *ops, int n_ops, int m)
     {

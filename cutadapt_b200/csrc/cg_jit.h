@@ -14,15 +14,16 @@
 
 struct CgJitKernel;   // a loaded module + entry point
 
-// Compile the plane program of `set` for W plane words.  Returns nullptr on failure (err filled).
-CgJitKernel *cg_jit_build_pscan(const CgBuiltSet &set, int W, bool has_qual, std::string &err);
+// Compile the plane program of `set` for W plane words; stats: the variant that counts the trim statistics of the
+// reads it settles (cg_pscan.cuh).  Returns nullptr on failure (err filled).
+CgJitKernel *cg_jit_build_pscan(const CgBuiltSet &set, int W, bool has_qual, bool stats, std::string &err);
 void cg_jit_destroy(CgJitKernel *k);
 // the generated translation unit (for inspection and the tests)
-std::string cg_jit_pscan_source(const CgBuiltSet &set, int W, bool has_qual);
+std::string cg_jit_pscan_source(const CgBuiltSet &set, int W, bool has_qual, bool stats = false);
 // resident CTAs per SM for the given launch shape; <= 0 on error
 int cg_jit_occupancy(CgJitKernel *k, int block, size_t smem);
 // launches kernel(const CgKernelArgs) -- `args` points at the argument block; returns 0 or a CUresult
 int cg_jit_launch(CgJitKernel *k, int grid, int block, size_t smem, void *stream, const void *args);
 // compile only (no device needed): PTX/cubin size or -1; used by the CPU tests to check that the generated
 // source builds for sm_90a
-long cg_jit_compile_only(const CgBuiltSet &set, int W, bool has_qual, std::string &log);
+long cg_jit_compile_only(const CgBuiltSet &set, int W, bool has_qual, std::string &log, bool stats = false);

@@ -714,28 +714,30 @@ size_t cg_pscan_smem_bytes(uint32_t blob_bytes, int mini_cap, bool has_qual, int
     return pscan_smem_layout(blob_bytes, mini_cap, has_qual, stats_max_len).total;
 }
 
-template <bool HAS_QUAL, int W>
+template <bool HAS_QUAL, int W, bool STATS>
 __global__ void __launch_bounds__(CG_NT, W <= 5 ? CG_PSCAN_BLOCKS : 5) cg_pscan_kernel(const CgKernelArgs a)
 {
-    cg_pscan_body<HAS_QUAL, W, RuntimePlaneProg>(a);
+    cg_pscan_body<HAS_QUAL, W, RuntimePlaneProg, STATS>(a);
 }
 
 typedef void (*pscan_kernel_t)(const CgKernelArgs);
-static pscan_kernel_t pick_pscan(bool has_qual, int w)
+static pscan_kernel_t pick_pscan(bool has_qual, int w, bool stats)
 {
-    if (w <= 5) return has_qual ? cg_pscan_kernel<true, 5> : cg_pscan_kernel<false, 5>;
-    return has_qual ? cg_pscan_kernel<true, 8> : cg_pscan_kernel<false, 8>;
+    // (the statistics are counted in this stage only for passes without quality trimming: launch_trim_single)
+    if (stats) return w <= 5 ? cg_pscan_kernel<false, 5, true> : cg_pscan_kernel<false, 8, true>;
+    if (w <= 5) return has_qual ? cg_pscan_kernel<true, 5, false> : cg_pscan_kernel<false, 5, false>;
+    return has_qual ? cg_pscan_kernel<true, 8, false> : cg_pscan_kernel<false, 8, false>;
 }
-cudaError_t cg_pscan_occupancy(bool has_qual, int w, size_t smem, int *blocks_per_sm)
+cudaError_t cg_pscan_occupancy(bool has_qual, int w, bool stats, size_t smem, int *blocks_per_sm)
 {
-    pscan_kernel_t k = pick_pscan(has_qual, w);
+    pscan_kernel_t k = pick_pscan(has_qual, w, stats);
     cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
     return cudaOccupancyMaxActiveBlocksPerMultiprocessor(blocks_per_sm, k, CG_NT, smem);
 }
 cudaError_t cg_launch_pscan(const CgKernelArgs &a, bool has_qual, int w, int grid, size_t smem, cudaStream_t st)
 {
-    pick_pscan(has_qual, w)<<<grid, CG_NT, smem, st>>>(a);
+    pick_pscan(has_qual, w, a.stats != nullptr)<<<grid, CG_NT, smem, st>>>(a);
     return cudaGetLastError();
 }
 

@@ -47,7 +47,9 @@ cudaError_t cg_launch_light(const CgKernelArgs &a, int grid, cudaStream_t st);
 // a.tasks (32-bit read numbers, counted in a.task_count, which must be zero)
 cudaError_t cg_launch_index(const CgKernelArgs &a, int grid, cudaStream_t st);
 size_t cg_pscan_smem_bytes(uint32_t blob_bytes, int mini_cap, bool has_qual, int stats_max_len = -1);   // >= 0: + fused statistics
-cudaError_t cg_pscan_occupancy(bool has_qual, int w, size_t smem, int *blocks_per_sm);
+// stats: the variant that counts the trim statistics of the reads it settles (without qualities only); cg_launch_pscan
+// runs it when a.stats is set
+cudaError_t cg_pscan_occupancy(bool has_qual, int w, bool stats, size_t smem, int *blocks_per_sm);
 cudaError_t cg_launch_pscan(const CgKernelArgs &a, bool has_qual, int w, int grid, size_t smem, cudaStream_t st);
 size_t cg_dp_smem_bytes(uint32_t blob_bytes, int slot_bytes);
 cudaError_t cg_list_occupancy(bool plan, int mr, size_t smem, int *blocks_per_sm);

@@ -24,10 +24,6 @@ struct ScanSmem { size_t blob_off, enc_off, stats_off, warp_off, warp_stride, ba
 #ifndef CG_PSCAN_BLOCKS
 #define CG_PSCAN_BLOCKS 8     // resident CTAs per SM the 5-word variant is compiled for (64 registers)
 #endif
-#ifndef CG_PSCAN_STATS
-#define CG_PSCAN_STATS 1      // 0: the statistics fused into this stage are compiled out (the specialised kernels unless
-                              // CUTADAPT_B200_FUSED_STATS is set: the code costs 3 % even when it is not used)
-#endif
 #define CG_TASK_RESCAN 0x100u     // the plan stage must scan the read itself (shift-and scan_core)
 #define CG_TASK_BYTES 0x400u      // the task carries the read window itself: 2 W + 1 16-byte pieces after the four header
                                   // words (the aligned stretch of shared memory that covers the 32 W characters in front
@@ -134,11 +130,13 @@ __device__ __forceinline__ void pre_trim_warp(const uint8_t *seq, const uint8_t 
     *s_out = start; *e_out = stop;
 }
 
-template <bool HAS_QUAL, int W, class Prog>
+// STATS: the variant that counts the statistics of the reads it settles (a.stats, see below); the other variant carries
+// none of that code.
+template <bool HAS_QUAL, int W, class Prog, bool STATS = false>
 __device__ __forceinline__ void cg_pscan_body(const CgKernelArgs &a)
 {
     extern __shared__ __align__(128) uint8_t smem[];
-    const ScanSmem L = pscan_smem_layout(a.blob_bytes, a.mini_cap, HAS_QUAL, a.stats ? a.stats_max_len : -1);
+    const ScanSmem L = pscan_smem_layout(a.blob_bytes, a.mini_cap, HAS_QUAL, (STATS && a.stats) ? a.stats_max_len : -1);
     uint8_t *s_blob = smem + L.blob_off;
     uint8_t *s_enc = smem + L.enc_off;
     const int tid = threadIdx.x, lane = tid & 31, wib = tid >> 5;
@@ -154,13 +152,12 @@ __device__ __forceinline__ void cg_pscan_body(const CgKernelArgs &a)
     uint32_t *s_hrem = s_hlen + (st_len + 1);   /* removed lengths at 0 errors: 5' matches, then 3' matches */           \
     uint32_t *s_hadj = s_hrem + 2 * (st_len + 1);                                                                        \
     unsigned long long *s_scal = (unsigned long long *)((uint8_t *)s_hlen + cg_align_up((size_t)(3 * (st_len + 1) + 8) * sizeof(uint32_t), 8));
-    if (CG_PSCAN_STATS && a.stats) {
+    if (STATS && a.stats) {
         CG_PSCAN_STATS_VIEW
         (void)s_hrem; (void)s_hadj;
         for (int i = threadIdx.x; i < 3 * (st_len + 1) + 8; i += CG_NT) s_hlen[i] = 0;
         if (threadIdx.x < 8) s_scal[threadIdx.x] = 0;     // reads, bases, with adapters, quality-trimmed, adapter bases
     }
-    unsigned long long st_acc = 0;     // fused statistics: lane L of a warp accumulates scalar L (see the tile loop)
     for (uint32_t i = tid; i < a.blob_bytes / 16; i += CG_NT) ((uint4 *)s_blob)[i] = ((const uint4 *)a.blob)[i];
     for (uint32_t i = tid; i < 768 / 16; i += CG_NT) ((uint4 *)s_enc)[i] = ((const uint4 *)a.enc)[i];
     if (lane == 0) {
@@ -258,7 +255,7 @@ __device__ __forceinline__ void cg_pscan_body(const CgKernelArgs &a)
                 if (cls == CG_PLANE_EXACT) hit_exact(A, nn, s0, hit);
                 else if (cls == CG_PLANE_OVERLAP) hit_end_overlap(A, nn, s0, hit);
                 store_hit(a.out + (size_t)r * a.slots, hit, 0, nn);
-                if (CG_PSCAN_STATS && a.stats) {
+                if (STATS && a.stats) {
                     // what stats_read_core adds for this read (one round, one slot), packed for three warp sums:
                     // p1 = bases | quality-trimmed bases << 16, p2 = adapter bases | read << 16 | match << 22,
                     // p3 = one 6-bit count per adjacent-base class
@@ -268,7 +265,9 @@ __device__ __forceinline__ void cg_pscan_body(const CgKernelArgs &a)
                     st_p2 = 1u << 16;
                     int fin = nn;
                     if (hit.adapter >= 0) {
-                        const bool after = hit.remove == CGK_REMOVE_AFTER;
+                        // (a literal where the program fixes the adapter's kind: one of the two branches is dead)
+                        const int kind = Prog::remove_kind(A.remove);
+                        const bool after = kind == CGK_REMOVE_AUTO ? hit.remove == CGK_REMOVE_AFTER : kind == CGK_REMOVE_AFTER;
                         int removed = after ? nn - hit.rstart : hit.rstop;
                         removed = removed < 0 ? 0 : removed;
                         st_p2 |= (uint32_t)removed | (1u << 22);
@@ -289,9 +288,9 @@ __device__ __forceinline__ void cg_pscan_body(const CgKernelArgs &a)
                 }
             }
         }
-        if (CG_PSCAN_STATS && a.stats) {
+        if (STATS && a.stats) {
             CG_PSCAN_STATS_VIEW
-            (void)s_hrem; (void)s_hadj; (void)s_scal;
+            (void)s_hrem;
             // most reads of a tile end in the same length bin: one shared-memory atomic for the bin of the first
             // counted lane and its peers, one each for the others
             const uint32_t counted = __ballot_sync(0xffffffffu, st_fin >= 0);
@@ -304,7 +303,8 @@ __device__ __forceinline__ void cg_pscan_body(const CgKernelArgs &a)
                 const uint32_t s1 = __reduce_add_sync(0xffffffffu, st_p1);
                 const uint32_t s2 = __reduce_add_sync(0xffffffffu, st_p2);
                 const uint32_t s3 = __reduce_add_sync(0xffffffffu, st_p3);
-                // lane L keeps scalar L of the warp: reads, matches, bases, quality-trimmed, adapter bases, adjacent x 5
+                // lane L adds scalar L of the warp to the CTA's counters (no register held across the tile loop):
+                // reads, matches, bases, quality-trimmed, adapter bases, adjacent x 5
                 uint32_t mine_add = 0;
                 switch (lane) {
                 case 0: mine_add = (s2 >> 16) & 63u; break;
@@ -314,7 +314,10 @@ __device__ __forceinline__ void cg_pscan_body(const CgKernelArgs &a)
                 case 4: mine_add = s2 & 0xffffu; break;
                 default: if (lane < 10) mine_add = (s3 >> (6 * (lane - 5))) & 63u; break;
                 }
-                st_acc += mine_add;
+                if (mine_add) {
+                    if (lane < 5) atomicAdd(&s_scal[lane], (unsigned long long)mine_add);
+                    else atomicAdd(&s_hadj[lane - 5], mine_add);
+                }
             }
         }
         const bool slow = mine && cls == CG_PLANE_SLOW;
@@ -361,14 +364,12 @@ __device__ __forceinline__ void cg_pscan_body(const CgKernelArgs &a)
             if (next < n_mt) issue(next);
         }
     }
-    if (CG_PSCAN_STATS && a.stats) {
+    if (STATS && a.stats) {
         CG_PSCAN_STATS_VIEW
-        if (st_acc) {
-            // lanes 0..4: reads, matches, bases, quality-trimmed, adapter bases -> stats[0, 2, 1, 3, 4]; 5..9: adjacent bases
-            if (lane < 5) atomicAdd(&a.stats[lane == 1 ? 2 : (lane == 2 ? 1 : lane)], st_acc);
-            else if (lane < 10) atomicAdd(&s_hadj[lane - 5], (uint32_t)st_acc);
-        }
         __syncthreads();
+        // reads, matches, bases, quality-trimmed, adapter bases -> stats[0, 2, 1, 3, 4]
+        if (threadIdx.x < 5 && s_scal[threadIdx.x])
+            atomicAdd(&a.stats[threadIdx.x == 1 ? 2 : (threadIdx.x == 2 ? 1 : threadIdx.x)], s_scal[threadIdx.x]);
         // one adapter: lengths, then its 5' block and its 3' block (adjacent bases, removed length x errors)
         unsigned long long *hist = a.stats + CG_STATS_SCALARS;
         const long long end_size = cg_stats_end_size(st_len, a.stats_kmax);

@@ -215,7 +215,8 @@ int cg_adapterset_destroy(cg_adapterset *set);
  * counterpart in the reference; results do not depend on it. */
 int cg_adapterset_jit_status(const cg_adapterset *set);
 /* The generated translation unit (for inspection).  Returns its length; copies at most cap - 1 characters. */
-int64_t cg_adapterset_jit_source(const cg_adapterset *set, int32_t plane_words, int32_t has_qual, char *buf, int64_t cap);
+int64_t cg_adapterset_jit_source(const cg_adapterset *set, int32_t plane_words, int32_t has_qual, int32_t stats,
+                                 char *buf, int64_t cap);
 int cg_adapterset_slots(const cg_adapterset *set); /* 1, or 2 if any group is LINKED */
 /* Aligner.effective_length / PrefixComparer.effective_length (_align.pyx:188,268-271,626-630) */
 int cg_adapterset_effective_length(const cg_adapterset *set, int32_t adapter, int32_t *out);
@@ -254,10 +255,11 @@ int cg_process_batch_device(cg_ctx *ctx, const cg_adapterset *set, const uint8_t
                             int32_t max_read_len, const cg_params *params, cg_match *d_matches,
                             int32_t *d_qtrim);
 /* The same plus the statistics of these reads ADDED to d_stats (int64[cg_stats_size(n_adapters, stats_max_len,
- * stats_kmax)], device memory; what cg_stats_accumulate_device computes from the records).  With
- * CUTADAPT_B200_FUSED_STATS=1 and a set of one plain adapter the split pipeline counts the reads its first stage
- * settles while they are in shared memory and the rest from its task list, so the records are not read back;
- * otherwise the statistics kernel runs after the pass.
+ * stats_kmax)], device memory; what cg_stats_accumulate_device computes from the records, bit for bit).  For a set
+ * of one plain adapter, one round, no quality trimming and stats_max_len <= 4096 the split pipeline counts the reads
+ * its first stage settles while they are in shared memory (a variant of that kernel compiled with the statistics
+ * code) and the rest from its task list, so the records are not read back; otherwise the statistics kernel runs after
+ * the pass.
  * With quality trimming d_qtrim is required. */
 int cg_process_batch_device_stats(cg_ctx *ctx, const cg_adapterset *set, const uint8_t *d_seq, const uint8_t *d_qual,
                                   const int64_t *d_offsets, int64_t n_reads, int32_t max_read_len, const cg_params *params,
