@@ -1960,7 +1960,8 @@ static int fastq_stage_stats(cg_ctx *c, FastqSlot &f, FqStage &g, int kmax, cuda
 
 // After the finish kernel: written lengths, poly-A lengths, reverse_complemented per adapter; then the vector goes to
 // the host (the output stage waits for it).
-static int fastq_stage_stats_tail(cg_ctx *c, FastqSlot &f, const FqStage &g, cudaStream_t st)
+static int fastq_stage_stats_tail(cg_ctx *c, FastqSlot &f, const FqStage &g, cudaStream_t st,
+                                  const int32_t *d_route = nullptr)
 {
     if (!g.acc || g.n == 0) return CG_OK;
     const int n_ad = g.acc->n_adapters;
@@ -1968,7 +1969,7 @@ static int fastq_stage_stats_tail(cg_ctx *c, FastqSlot &f, const FqStage &g, cud
     const long long tail = cg_stats_total(n_ad, g.st_len, g.st_kmax);
     CU(cg_launch_fastq_stats_tail(g.n, f.d_interval.p, f.d_outlen.p, g.st_poly_a ? f.d_polya.p : nullptr, g.d_matches,
                                   g.times, g.slots, g.d_is_rc, n_ad, g.st_len, v + CG_STATS_SCALARS, v + tail + n_ad,
-                                  v + tail, st));
+                                  v + tail, st, d_route));
     c->launches += 1;
     const size_t total = (size_t)fqstats_total(n_ad, g.st_len, g.st_kmax);
     CU(cudaMemcpyAsync(f.h_fqstats.p, v, total * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
@@ -2075,25 +2076,49 @@ static int fastq_stage_route(cg_ctx *c, FastqSlot &f1, FastqSlot *f2, long long 
     return CG_OK;
 }
 
+// Filter outputs (cg_fastq_collect_split*): a read or pair that the too-short, too-long or untrimmed filter removes goes
+// to destination 1, 2 or 3 when `redirect` has that filter's CG_REDIRECT_* bit; the finish kernel fills d_route, the
+// output is partitioned by it like a demultiplexed one and written in each destination's format.
+struct FqSplit {
+    int redirect = 0;                // CG_REDIRECT_* bits
+    int fasta_dests = 0;             // bit d: destination d is written as FASTA
+    int32_t *d_route = nullptr;      // device, per record: destination, -1 = dropped
+    static constexpr int n_dest = 4;
+};
+
+// The checks of cg_fastq_collect_split(_paired) on the parameters of a mate
+static int split_check(const FqSplit &sp, const cg_fastq_params *fp, const char *who)
+{
+    if (sp.redirect & ~7) return fail(CG_EINVAL, std::string(who) + ": redirect takes CG_REDIRECT_* bits only");
+    if ((sp.fasta_dests >> 1) & ~7) return fail(CG_EINVAL, std::string(who) + ": fasta_outputs takes CG_REDIRECT_* bits only");
+    if ((sp.redirect & CG_REDIRECT_UNTRIMMED) && fp->discard_trimmed)
+        return fail(CG_EINVAL, std::string(who) + ": the untrimmed output cannot be combined with discard_trimmed");
+    if (fp->format == CG_FORMAT_FASTA && (sp.redirect & ~(sp.fasta_dests >> 1)))
+        return fail(CG_EINVAL, std::string(who) + ": FASTA input can only be written as FASTA (set every redirect bit in "
+                                                   "fasta_outputs)");
+    return CG_OK;
+}
+
 // sizes -> offsets -> formatted records -> host; counters.  segments (host, n_dest + 1 values): where each destination
 // starts in `out`.
 static int fastq_stage_output(cg_ctx *c, FastqSlot &f, const FqStage &g, cudaStream_t st, uint8_t *out,
                               int64_t out_capacity, cg_fastq_result *res, const FqDemux *dm = nullptr,
-                              int64_t *segments = nullptr)
+                              int64_t *segments = nullptr, const FqSplit *sp = nullptr)
 {
     const long long n = g.n;
     int rc;
     long long total = 0;
     int fq_err[2];
-    if (dm) {
-        const int n_dest = dm->n_dest();
+    if (dm || sp) {
+        const int n_dest = dm ? dm->n_dest() : FqSplit::n_dest;
+        const int32_t *d_dest = dm ? dm->d_dest : sp->d_route;
         const long long tiles = cg_demux_tiles(n), cells = tiles * n_dest;
         if ((rc = f.d_dmbytes.ensure((size_t)cells)) != CG_OK) return rc;
         if ((rc = f.d_dmbase.ensure((size_t)cells + 1)) != CG_OK) return rc;
         if ((rc = f.d_scan.ensure((size_t)cg_scan_tiles(cells) + 1)) != CG_OK) return rc;
-        CU(cg_launch_fastq_demux(0, f.d_outlen.p, dm->d_dest, n, n_dest, f.d_dmbytes.p, nullptr, nullptr, st));
+        CU(cg_launch_fastq_demux(0, f.d_outlen.p, d_dest, n, n_dest, f.d_dmbytes.p, nullptr, nullptr, st));
         CU(cg_launch_scan_i32(f.d_dmbytes.p, cells, f.d_scan.p, f.d_dmbase.p, st));
-        CU(cg_launch_fastq_demux(1, f.d_outlen.p, dm->d_dest, n, n_dest, nullptr, f.d_dmbase.p, f.d_outoff.p, st));
+        CU(cg_launch_fastq_demux(1, f.d_outlen.p, d_dest, n, n_dest, nullptr, f.d_dmbase.p, f.d_outoff.p, st));
         c->launches += 5;
         // segment d starts at base[d][tile 0]; the last entry is the total
         CU(cudaMemcpy2DAsync(segments, sizeof(int64_t), f.d_dmbase.p, (size_t)tiles * sizeof(int64_t), sizeof(int64_t),
@@ -2124,9 +2149,23 @@ static int fastq_stage_output(cg_ctx *c, FastqSlot &f, const FqStage &g, cudaStr
     if (total > 0) {
         if (!out) return fail(CG_EINVAL, "cg_fastq_collect: out is NULL");
         if ((rc = f.d_out.ensure((size_t)total + 64)) != CG_OK) return rc;
-        CU(cg_launch_fastq_write(f.d_in.p, f.d_rec.p, f.d_interval.p, f.d_outoff.p, f.d_outlen.p, n, f.d_out.p, g.action,
-                                 f.d_keep.p, f.d_mask.p, g.rc_suffix, st, g.fasta_out() ? 1 : 0));
-        c->launches += 1;
+        if (sp) {
+            // one writer per format that has bytes to write, each skipping the other format's destinations
+            for (int fa = 0; fa < 2; ++fa) {
+                bool present = false;
+                for (int d = 0; d < FqSplit::n_dest; ++d)
+                    present |= ((sp->fasta_dests >> d) & 1) == fa && segments[d + 1] > segments[d];
+                if (!present) continue;
+                CU(cg_launch_fastq_write(f.d_in.p, f.d_rec.p, f.d_interval.p, f.d_outoff.p, f.d_outlen.p, n, f.d_out.p,
+                                         g.action, f.d_keep.p, f.d_mask.p, g.rc_suffix, st, fa, sp->d_route,
+                                         sp->fasta_dests));
+                c->launches += 1;
+            }
+        } else {
+            CU(cg_launch_fastq_write(f.d_in.p, f.d_rec.p, f.d_interval.p, f.d_outoff.p, f.d_outlen.p, n, f.d_out.p, g.action,
+                                     f.d_keep.p, f.d_mask.p, g.rc_suffix, st, g.fasta_out() ? 1 : 0));
+            c->launches += 1;
+        }
         if (is_pinned(out)) {
             CU(cudaMemcpyAsync(out, f.d_out.p, (size_t)total, cudaMemcpyDeviceToHost, st));
             CU(cudaStreamSynchronize(st));
@@ -2191,7 +2230,7 @@ static int fastq_stage_info(cg_ctx *c, FastqSlot &f, const FqStage &g, const cg_
 
 static int fastq_collect_impl(cg_ctx *c, int32_t slot, const cg_adapterset *s, const cg_fastq_params *fp,
                               uint8_t *out, int64_t out_capacity, cg_fastq_result *res, FqDemux *dm, int64_t *segments,
-                              const FqInfo *info = nullptr)
+                              const FqInfo *info = nullptr, FqSplit *sp = nullptr)
 {
     if (!c || !fp || !res || slot < 0 || slot >= CG_FQ_SLOTS) return fail(CG_EINVAL, "cg_fastq_collect: bad argument");
     if (s && s->ctx != c) return fail(CG_EINVAL, "adapter set belongs to another context");
@@ -2200,19 +2239,28 @@ static int fastq_collect_impl(cg_ctx *c, int32_t slot, const cg_adapterset *s, c
     CU(cudaSetDevice(c->device));
     f.busy = false;
     memset(res, 0, sizeof *res);
+    int rc;
+    if (sp && (rc = split_check(*sp, fp, "cg_fastq_collect_split")) != CG_OK) return rc;
     FqStage g;
-    int rc = fqstats_lookup(c, fp->stats, s ? s->host.n_adapters : 0, &g.acc);
+    rc = fqstats_lookup(c, fp->stats, s ? s->host.n_adapters : 0, &g.acc);
     if (rc != CG_OK) return rc;
     rc = fastq_stage_evaluate(c, f, s, fp, 1, f.stream, g);
     if (rc != CG_OK || g.n == 0) return rc;
     if (info && (rc = fastq_stage_info(c, f, g, fp, *info, f.stream)) != CG_OK) return rc;
     if (dm && (rc = fastq_stage_route(c, f, nullptr, g.n, *dm, f.stream)) != CG_OK) return rc;
-    CU(cg_launch_fastq_finish(g.n, f.d_rec.p, f.d_interval.p, f.d_mask.p, fastq_enabled_filters(fp), f.d_outlen.p,
+    int enabled = fastq_enabled_filters(fp);
+    if (sp) {
+        if ((rc = f.d_dest.ensure((size_t)g.n)) != CG_OK) return rc;
+        sp->d_route = f.d_dest.p;
+        enabled = fq_route_enabled(enabled, sp->redirect);
+    }
+    CU(cg_launch_fastq_finish(g.n, f.d_rec.p, f.d_interval.p, f.d_mask.p, enabled, f.d_outlen.p,
                               f.d_counters + 1, nullptr, nullptr, nullptr, 0, nullptr, nullptr, 0, 0, g.rc_suffix,
-                              dm ? dm->d_dest : nullptr, dm ? dm->d_dest_keep : nullptr, f.stream, g.fasta_out() ? 1 : 0));
+                              dm ? dm->d_dest : nullptr, dm ? dm->d_dest_keep : nullptr, f.stream, g.fasta_out() ? 1 : 0,
+                              sp ? sp->redirect : 0, sp ? sp->fasta_dests : 0, sp ? sp->d_route : nullptr));
     c->launches += 1;
-    if ((rc = fastq_stage_stats_tail(c, f, g, f.stream)) != CG_OK) return rc;
-    if ((rc = fastq_stage_output(c, f, g, f.stream, out, out_capacity, res, dm, segments)) != CG_OK) return rc;
+    if ((rc = fastq_stage_stats_tail(c, f, g, f.stream, sp ? sp->d_route : nullptr)) != CG_OK) return rc;
+    if ((rc = fastq_stage_output(c, f, g, f.stream, out, out_capacity, res, dm, segments, sp)) != CG_OK) return rc;
     if ((rc = check_err_flag(c)) != CG_OK) return rc;
     fastq_stats_commit(f, g, fp, *res);
     return CG_OK;
@@ -2222,6 +2270,24 @@ extern "C" int cg_fastq_collect(cg_ctx *c, int32_t slot, const cg_adapterset *s,
                                 uint8_t *out, int64_t out_capacity, cg_fastq_result *res)
 {
     return fastq_collect_impl(c, slot, s, fp, out, out_capacity, res, nullptr, nullptr);
+}
+
+// bit d of the destinations written as FASTA: 0 the main output (params.format), 1-3 the bits of fasta_outputs
+static int split_fasta_dests(const cg_fastq_params *fp, int32_t fasta_outputs)
+{
+    return (fp && fp->format != CG_FORMAT_FASTQ ? 1 : 0) | (fasta_outputs << 1);
+}
+
+extern "C" int cg_fastq_collect_split(cg_ctx *c, int32_t slot, const cg_adapterset *s, const cg_fastq_params *fp,
+                                      int32_t redirect, int32_t fasta_outputs, uint8_t *out, int64_t out_capacity,
+                                      cg_fastq_result *res, int64_t *segments)
+{
+    if (!segments) return fail(CG_EINVAL, "cg_fastq_collect_split: bad argument");
+    for (int d = 0; d <= FqSplit::n_dest; ++d) segments[d] = 0;
+    FqSplit sp;
+    sp.redirect = redirect;
+    sp.fasta_dests = split_fasta_dests(fp, fasta_outputs);
+    return fastq_collect_impl(c, slot, s, fp, out, out_capacity, res, nullptr, segments, nullptr, &sp);
 }
 
 extern "C" int cg_fastq_collect_info(cg_ctx *c, int32_t slot, const cg_adapterset *s, const cg_fastq_params *fp,
@@ -2351,7 +2417,8 @@ static int fastq_collect_paired_impl(cg_ctx *c, int32_t slot1, int32_t slot2, co
                                      const cg_adapterset *s2, const FqPairAdapters *pa, const cg_fastq_params *fp1,
                                      const cg_fastq_params *fp2, int32_t pair_filter_mode, uint8_t *out1,
                                      int64_t out_capacity1, uint8_t *out2, int64_t out_capacity2, cg_fastq_result *res1,
-                                     cg_fastq_result *res2, FqDemux *dm, int64_t *segments1, int64_t *segments2)
+                                     cg_fastq_result *res2, FqDemux *dm, int64_t *segments1, int64_t *segments2,
+                                     FqSplit *sp = nullptr)
 {
     if (!c || !fp1 || !fp2 || !res1 || !res2 || slot1 < 0 || slot1 >= CG_FQ_SLOTS || slot2 < 0 || slot2 >= CG_FQ_SLOTS ||
         slot1 == slot2 || pair_filter_mode < 0 || pair_filter_mode > 2)
@@ -2375,6 +2442,11 @@ static int fastq_collect_paired_impl(cg_ctx *c, int32_t slot1, int32_t slot2, co
         cudaStreamSynchronize(f2.stream);
         return fail(CG_EINVAL, "cg_fastq_collect_paired: the two mates need different statistics handles");
     }
+    if (sp && ((rc = split_check(*sp, fp1, "cg_fastq_collect_paired_split")) != CG_OK ||
+               (rc = split_check(*sp, fp2, "cg_fastq_collect_paired_split")) != CG_OK)) {
+        cudaStreamSynchronize(f2.stream);
+        return rc;
+    }
     if ((rc = fqstats_lookup(c, fp1->stats, pa ? pa->n_pairs : (s1 ? s1->host.n_adapters : 0), &g1.acc)) != CG_OK ||
         (rc = fqstats_lookup(c, fp2->stats, pa ? pa->n_pairs : (s2 ? s2->host.n_adapters : 0), &g2.acc)) != CG_OK) {
         cudaStreamSynchronize(f2.stream);
@@ -2395,15 +2467,25 @@ static int fastq_collect_paired_impl(cg_ctx *c, int32_t slot1, int32_t slot2, co
     if (dm && (rc = fastq_stage_route(c, f1, &f2, g1.n, *dm, st)) != CG_OK) return rc;
     // --discard-untrimmed with adapters on one mate only tests "both" (cli.py:859-893)
     const int mode_untrimmed = (!pa && (!s1 || !s2)) ? 1 : pair_filter_mode;
-    CU(cg_launch_fastq_finish(g1.n, f1.d_rec.p, f1.d_interval.p, f1.d_mask.p, fastq_enabled_filters(fp1), f1.d_outlen.p,
-                              f1.d_counters + 1, f2.d_rec.p, f2.d_interval.p, f2.d_mask.p, fastq_enabled_filters(fp2),
+    int enabled1 = fastq_enabled_filters(fp1), enabled2 = fastq_enabled_filters(fp2);
+    if (sp) {
+        // both mates share one destination per pair (the first mate's slot holds it)
+        if ((rc = f1.d_dest.ensure((size_t)g1.n)) != CG_OK) return rc;
+        sp->d_route = f1.d_dest.p;
+        enabled1 = fq_route_enabled(enabled1, sp->redirect);
+        enabled2 = fq_route_enabled(enabled2, sp->redirect);
+    }
+    CU(cg_launch_fastq_finish(g1.n, f1.d_rec.p, f1.d_interval.p, f1.d_mask.p, enabled1, f1.d_outlen.p,
+                              f1.d_counters + 1, f2.d_rec.p, f2.d_interval.p, f2.d_mask.p, enabled2,
                               f2.d_outlen.p, f2.d_counters + 1, pair_filter_mode, mode_untrimmed, 0,
-                              dm ? dm->d_dest : nullptr, dm ? dm->d_dest_keep : nullptr, st, g1.fasta_out() ? 1 : 0));
+                              dm ? dm->d_dest : nullptr, dm ? dm->d_dest_keep : nullptr, st, g1.fasta_out() ? 1 : 0,
+                              sp ? sp->redirect : 0, sp ? sp->fasta_dests : 0, sp ? sp->d_route : nullptr));
     c->launches += 1;
-    if ((rc = fastq_stage_stats_tail(c, f1, g1, st)) != CG_OK) return rc;
-    if ((rc = fastq_stage_stats_tail(c, f2, g2, st)) != CG_OK) return rc;
-    if ((rc = fastq_stage_output(c, f1, g1, st, out1, out_capacity1, res1, dm, segments1)) != CG_OK) return rc;
-    if ((rc = fastq_stage_output(c, f2, g2, st, out2, out_capacity2, res2, dm, segments2)) != CG_OK) return rc;
+    const int32_t *route = sp ? sp->d_route : nullptr;
+    if ((rc = fastq_stage_stats_tail(c, f1, g1, st, route)) != CG_OK) return rc;
+    if ((rc = fastq_stage_stats_tail(c, f2, g2, st, route)) != CG_OK) return rc;
+    if ((rc = fastq_stage_output(c, f1, g1, st, out1, out_capacity1, res1, dm, segments1, sp)) != CG_OK) return rc;
+    if ((rc = fastq_stage_output(c, f2, g2, st, out2, out_capacity2, res2, dm, segments2, sp)) != CG_OK) return rc;
     if ((rc = check_err_flag(c)) != CG_OK) return rc;
     fastq_stats_commit(f1, g1, fp1, *res1);
     fastq_stats_commit(f2, g2, fp2, *res2);
@@ -2417,6 +2499,22 @@ extern "C" int cg_fastq_collect_paired(cg_ctx *c, int32_t slot1, int32_t slot2, 
 {
     return fastq_collect_paired_impl(c, slot1, slot2, s1, s2, nullptr, fp1, fp2, pair_filter_mode, out1, out_capacity1, out2,
                                      out_capacity2, res1, res2, nullptr, nullptr, nullptr);
+}
+
+extern "C" int cg_fastq_collect_paired_split(cg_ctx *c, int32_t slot1, int32_t slot2, const cg_adapterset *s1,
+                                             const cg_adapterset *s2, const cg_fastq_params *fp1, const cg_fastq_params *fp2,
+                                             int32_t pair_filter_mode, int32_t redirect, int32_t fasta_outputs,
+                                             uint8_t *out1, int64_t out_capacity1, uint8_t *out2, int64_t out_capacity2,
+                                             cg_fastq_result *res1, cg_fastq_result *res2, int64_t *segments1,
+                                             int64_t *segments2)
+{
+    if (!segments1 || !segments2) return fail(CG_EINVAL, "cg_fastq_collect_paired_split: bad argument");
+    for (int d = 0; d <= FqSplit::n_dest; ++d) segments1[d] = segments2[d] = 0;
+    FqSplit sp;
+    sp.redirect = redirect;
+    sp.fasta_dests = split_fasta_dests(fp1, fasta_outputs);
+    return fastq_collect_paired_impl(c, slot1, slot2, s1, s2, nullptr, fp1, fp2, pair_filter_mode, out1, out_capacity1, out2,
+                                     out_capacity2, res1, res2, nullptr, segments1, segments2, &sp);
 }
 
 extern "C" int cg_fastq_collect_pair_adapters(cg_ctx *c, int32_t slot1, int32_t slot2, const cg_adapterset *const *sets1,

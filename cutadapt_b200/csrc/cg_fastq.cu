@@ -466,13 +466,16 @@ __device__ __constant__ int kFilterCounter[7] = {4, 5, 8, 9, 10, 7, 7};
 // --discard-untrimmed to "both" when only one mate has adapters).  The first filter that fires gets the count.
 // out_len = size of the formatted record ("@" name "\n" sequence "\n+\n" qualities "\n", or with fasta_out
 // ">" name "\n" sequence "\n") or 0.
+// route != nullptr (filter outputs): route[r] = fq_route_core's destination; a record a filter with an output removes
+// is sized too, in the format of its destination (bit d of fasta_dests: destination d is FASTA).  The filter counters
+// stay as they are; n_written and bp_out count the main output only.
 __global__ void fq_finish_kernel(long long n_records, const CgFastqRecord *rec1, const int32_t *interval1,
                                  const int32_t *mask1, int enabled1, int32_t *out_len1, unsigned long long *counters1,
                                  const CgFastqRecord *rec2, const int32_t *interval2, const int32_t *mask2, int enabled2,
                                  int32_t *out_len2, unsigned long long *counters2, int mode, int mode_untrimmed,
-                                 int rc_suffix, const int32_t *dest, const uint8_t *dest_keep, int fasta_out)
+                                 int rc_suffix, const int32_t *dest, const uint8_t *dest_keep, int fasta_out,
+                                 int redirect, int fasta_dests, int32_t *route)
 {
-    const int per_base = fasta_out ? 1 : 2, fixed = fasta_out ? 3 : 6;
     const long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     int fired = -1;
     unsigned long long bp1 = 0, bp2 = 0;
@@ -481,14 +484,22 @@ __global__ void fq_finish_kernel(long long n_records, const CgFastqRecord *rec1,
         fired = fq_finish_core(mask1[r], mask2 ? mask2[r] : 0, mask2 != nullptr, enabled1, enabled2, mode, mode_untrimmed);
         // a demultiplexer without a writer for this destination drops the pair without counting it (steps.py:574-577)
         if (fired < 0 && dest_keep && !dest_keep[dest[r]]) fired = 7;
+        int to = fired < 0 ? 0 : -1;
+        bool fa = fasta_out != 0;
+        if (route) {
+            to = fq_route_core(fired, redirect);
+            route[r] = to;
+            fa = to >= 0 && ((fasta_dests >> to) & 1);
+        }
+        const int per_base = fa ? 1 : 2, fixed = fa ? 3 : 6;
         const int left1 = interval1[2 * r + 1] - interval1[2 * r];
         // a reverse-complemented read gets " rc" appended to its name (modifiers.py:295-296)
         const int extra1 = (rc_suffix && (mask1[r] & CG_FQ_MASK_RC)) ? 3 : 0;
-        out_len1[r] = fired < 0 ? rec1[r].hdr_len + extra1 + per_base * left1 + fixed : 0;
+        out_len1[r] = to >= 0 ? rec1[r].hdr_len + extra1 + per_base * left1 + fixed : 0;
         if (mask2) {
             const int left2 = interval2[2 * r + 1] - interval2[2 * r];
             const int extra2 = (rc_suffix && (mask2[r] & CG_FQ_MASK_RC)) ? 3 : 0;
-            out_len2[r] = fired < 0 ? rec2[r].hdr_len + extra2 + per_base * left2 + fixed : 0;
+            out_len2[r] = to >= 0 ? rec2[r].hdr_len + extra2 + per_base * left2 + fixed : 0;
             bp2 = fired < 0 ? left2 : 0;
         }
         written = fired < 0;
@@ -520,11 +531,12 @@ __global__ void fq_finish_kernel(long long n_records, const CgFastqRecord *rec1,
 //   rc[a]       matches on reads that were replaced by their reverse complement (modifiers.py:301-306), counted
 //               for the adapter of the first record of the match (the front part of a linked match)
 // The two histograms are privatised per CTA in shared memory when SMEM (2 x (max_len + 1) counters fit).
+// route != nullptr (filter outputs): only records of the main output (route 0) are written records.
 template <bool SMEM>
 __global__ void fq_stats_tail_kernel(long long n_records, const int32_t *interval, const int32_t *out_len,
                                      const int32_t *poly_a_len, const cg_match_rec *matches, int times, int slots,
                                      const uint8_t *is_rc, int n_adapters, int max_len, unsigned long long *lengths,
-                                     unsigned long long *poly_a, unsigned long long *rc)
+                                     unsigned long long *poly_a, unsigned long long *rc, const int32_t *route)
 {
     extern __shared__ unsigned int s_tail[];
     const int bins = max_len + 1;
@@ -534,7 +546,7 @@ __global__ void fq_stats_tail_kernel(long long n_records, const int32_t *interva
     }
     const long long nthreads = (long long)gridDim.x * blockDim.x;
     for (long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x; r < n_records; r += nthreads) {
-        if (out_len[r] != 0) {
+        if (out_len[r] != 0 && (!route || route[r] == 0)) {
             int w = interval[2 * r + 1] - interval[2 * r];
             w = w < 0 ? 0 : (w > max_len ? max_len : w);
             if (SMEM) atomicAdd(&s_tail[w], 1u); else atomicAdd(&lengths[w], 1ull);
@@ -562,17 +574,21 @@ __global__ void fq_stats_tail_kernel(long long n_records, const int32_t *interva
     }
 }
 
-// the trimmed records, one warp per record; FASTA_OUT: ">name\nsequence\n", the sequence on one line
+// the trimmed records, one warp per record; FASTA_OUT: ">name\nsequence\n", the sequence on one line.
+// route != nullptr (filter outputs): only the records whose destination d has bit d of fasta_dests == FASTA_OUT (the
+// other format's records are left to the other instantiation)
 template <bool FASTA_OUT>
 __global__ void __launch_bounds__(256) fq_write_kernel(const uint8_t *buf, const CgFastqRecord *rec, const int32_t *interval,
                                                         const int64_t *out_off, const int32_t *out_len,
                                                         long long n_records, uint8_t *out, int action,
-                                                        const int32_t *keep_interval, const int32_t *mask, int rc_suffix)
+                                                        const int32_t *keep_interval, const int32_t *mask, int rc_suffix,
+                                                        const int32_t *route, int fasta_dests)
 {
     const int lane = threadIdx.x & 31;
     const long long warps = ((long long)gridDim.x * blockDim.x) >> 5;
     for (long long r = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5; r < n_records; r += warps) {
         if (out_len[r] == 0) continue;         // filtered
+        if (route && (((fasta_dests >> route[r]) & 1) != (FASTA_OUT ? 1 : 0))) continue;
         const long long o = out_off[r];
         const CgFastqRecord m = rec[r];
         const int start = interval[2 * r], left = interval[2 * r + 1] - start;
@@ -1042,7 +1058,8 @@ cudaError_t cg_launch_fastq_evaluate(const uint8_t *d_buf, const CgFastqRecord *
 cudaError_t cg_launch_fastq_stats_tail(long long n_records, const int32_t *d_interval, const int32_t *d_out_len,
                                        const int32_t *d_poly_a_len, const cg_match_rec *d_matches, int times, int slots,
                                        const uint8_t *d_is_rc, int n_adapters, int max_len, unsigned long long *d_lengths,
-                                       unsigned long long *d_poly_a, unsigned long long *d_rc, cudaStream_t st)
+                                       unsigned long long *d_poly_a, unsigned long long *d_rc, cudaStream_t st,
+                                       const int32_t *d_route)
 {
     if (n_records <= 0) return cudaSuccess;
     const int block = 256;
@@ -1053,11 +1070,11 @@ cudaError_t cg_launch_fastq_stats_tail(long long n_records, const int32_t *d_int
     if (smem <= 48 * 1024 && n_records / grid < (1LL << 31))
         fq_stats_tail_kernel<true><<<(unsigned)grid, block, smem, st>>>(n_records, d_interval, d_out_len, d_poly_a_len,
                                                                        d_matches, times, slots, d_is_rc, n_adapters, max_len,
-                                                                       d_lengths, d_poly_a, d_rc);
+                                                                       d_lengths, d_poly_a, d_rc, d_route);
     else
         fq_stats_tail_kernel<false><<<(unsigned)grid, block, 0, st>>>(n_records, d_interval, d_out_len, d_poly_a_len,
                                                                      d_matches, times, slots, d_is_rc, n_adapters, max_len,
-                                                                     d_lengths, d_poly_a, d_rc);
+                                                                     d_lengths, d_poly_a, d_rc, d_route);
     return cudaGetLastError();
 }
 
@@ -1066,31 +1083,33 @@ cudaError_t cg_launch_fastq_finish(long long n_records, const CgFastqRecord *d_r
                                    unsigned long long *d_counters1, const CgFastqRecord *d_rec2,
                                    const int32_t *d_interval2, const int32_t *d_mask2, int enabled2, int32_t *d_out_len2,
                                    unsigned long long *d_counters2, int mode, int mode_untrimmed, int rc_suffix,
-                                   const int32_t *d_dest, const uint8_t *d_dest_keep, cudaStream_t st, int fasta_out)
+                                   const int32_t *d_dest, const uint8_t *d_dest_keep, cudaStream_t st, int fasta_out,
+                                   int redirect, int fasta_dests, int32_t *d_route)
 {
     if (n_records <= 0) return cudaSuccess;
     fq_finish_kernel<<<(unsigned)((n_records + 255) / 256), 256, 0, st>>>(n_records, d_rec1, d_interval1, d_mask1, enabled1,
                                                                          d_out_len1, d_counters1, d_rec2, d_interval2,
                                                                          d_mask2, enabled2, d_out_len2, d_counters2, mode,
                                                                          mode_untrimmed, rc_suffix, d_dest, d_dest_keep,
-                                                                         fasta_out);
+                                                                         fasta_out, redirect, fasta_dests, d_route);
     return cudaGetLastError();
 }
 
 cudaError_t cg_launch_fastq_write(const uint8_t *d_buf, const CgFastqRecord *d_rec, const int32_t *d_interval,
                                   const int64_t *d_out_off, const int32_t *d_out_len, long long n_records,
                                   uint8_t *d_out, int action, const int32_t *d_keep_interval, const int32_t *d_mask,
-                                  int rc_suffix, cudaStream_t st, int fasta_out)
+                                  int rc_suffix, cudaStream_t st, int fasta_out, const int32_t *d_route, int fasta_dests)
 {
     if (n_records <= 0) return cudaSuccess;
     long long grid = (n_records + 7) / 8;
     grid = cg_grid_cap(grid, 16);
     if (fasta_out)
         fq_write_kernel<true><<<(unsigned)grid, 256, 0, st>>>(d_buf, d_rec, d_interval, d_out_off, d_out_len, n_records, d_out,
-                                                              action, d_keep_interval, d_mask, rc_suffix);
+                                                              action, d_keep_interval, d_mask, rc_suffix, d_route, fasta_dests);
     else
         fq_write_kernel<false><<<(unsigned)grid, 256, 0, st>>>(d_buf, d_rec, d_interval, d_out_off, d_out_len, n_records, d_out,
-                                                               action, d_keep_interval, d_mask, rc_suffix);
+                                                               action, d_keep_interval, d_mask, rc_suffix, d_route,
+                                                               fasta_dests);
     return cudaGetLastError();
 }
 

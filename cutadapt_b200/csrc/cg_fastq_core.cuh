@@ -328,3 +328,19 @@ CG_HD int fq_finish_core(int m1, int m2, bool pair, int enabled1, int enabled2, 
     }
     return -1;
 }
+
+// Filter outputs (cg_fastq_collect_split): where a read or pair goes once fq_finish_core named the filter that fired
+// (-1: none).  0 the main output, 1 --too-short-output, 2 --too-long-output, 3 --untrimmed-output, -1 dropped.  A
+// filter with an output writes what it removes (SingleEndFilter / PairedEndFilter with a writer, steps.py:70-180),
+// every other filter drops it.  redirect: CG_REDIRECT_* bits (1 too-short, 2 too-long, 4 untrimmed).
+// fq_route_enabled: the enabled filters of a mate given to fq_finish_core -- an untrimmed output is the IsUntrimmed
+// filter with a writer, so it switches that filter (bit 6) on.
+CG_HD int fq_route_enabled(int enabled, int redirect) { return enabled | ((redirect & 4) ? 64 : 0); }
+CG_HD int fq_route_core(int fired, int redirect)
+{
+    if (fired < 0) return 0;
+    if (fired == 0 && (redirect & 1)) return 1;
+    if (fired == 1 && (redirect & 2)) return 2;
+    if (fired == 6 && (redirect & 4)) return 3;
+    return -1;
+}

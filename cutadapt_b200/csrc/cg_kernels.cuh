@@ -134,22 +134,29 @@ cudaError_t cg_launch_fastq_evaluate(const uint8_t *d_buf, const CgFastqRecord *
                                      int32_t *d_poly_a_len = nullptr);   // optional: bases PolyATrimmer removed, per read
 // statistics of the FASTQ path beyond the match records (after the finish kernel): written lengths of the records with
 // d_out_len != 0, the poly-A histogram (d_poly_a_len may be null), reverse_complemented per adapter (per match of the
-// records with d_is_rc set; d_is_rc may be null); every histogram has max_len + 1 bins
+// records with d_is_rc set; d_is_rc may be null); every histogram has max_len + 1 bins.  d_route (filter outputs, may
+// be null): only records routed to the main output (0) count as written.
 cudaError_t cg_launch_fastq_stats_tail(long long n_records, const int32_t *d_interval, const int32_t *d_out_len,
                                        const int32_t *d_poly_a_len, const cg_match_rec *d_matches, int times, int slots,
                                        const uint8_t *d_is_rc, int n_adapters, int max_len, unsigned long long *d_lengths,
-                                       unsigned long long *d_poly_a, unsigned long long *d_rc, cudaStream_t st);
-// verdict per read (second mate = nullptr) or pair -> sizes of the output records, filter counters
+                                       unsigned long long *d_poly_a, unsigned long long *d_rc, cudaStream_t st,
+                                       const int32_t *d_route = nullptr);
+// verdict per read (second mate = nullptr) or pair -> sizes of the output records, filter counters.  d_route (filter
+// outputs, may be null): every record's destination (fq_route_core of `redirect`, -1 = dropped); a redirected record is
+// sized in its destination's format (bit d of fasta_dests: destination d is FASTA; fasta_out is then unused).
 cudaError_t cg_launch_fastq_finish(long long n_records, const CgFastqRecord *d_rec1, const int32_t *d_interval1,
                                    const int32_t *d_mask1, int enabled1, int32_t *d_out_len1,
                                    unsigned long long *d_counters1, const CgFastqRecord *d_rec2,
                                    const int32_t *d_interval2, const int32_t *d_mask2, int enabled2, int32_t *d_out_len2,
                                    unsigned long long *d_counters2, int mode, int mode_untrimmed, int rc_suffix,
-                                   const int32_t *d_dest, const uint8_t *d_dest_keep, cudaStream_t st, int fasta_out = 0);
+                                   const int32_t *d_dest, const uint8_t *d_dest_keep, cudaStream_t st, int fasta_out = 0,
+                                   int redirect = 0, int fasta_dests = 0, int32_t *d_route = nullptr);
+// d_route (may be null): write only the records whose destination's bit in fasta_dests equals fasta_out
 cudaError_t cg_launch_fastq_write(const uint8_t *d_buf, const CgFastqRecord *d_rec, const int32_t *d_interval,
                                   const int64_t *d_out_off, const int32_t *d_out_len, long long n_records,
                                   uint8_t *d_out, int action, const int32_t *d_keep_interval, const int32_t *d_mask,
-                                  int rc_suffix, cudaStream_t st, int fasta_out = 0);
+                                  int rc_suffix, cudaStream_t st, int fasta_out = 0, const int32_t *d_route = nullptr,
+                                  int fasta_dests = 0);
 // demultiplexing: cg_launch_fastq_dest gives every record its destination (adapter of the most recent match of R1, or
 // of both mates: d1 * (n_named2 + 1) + d2; reads without a match: the last value of the dimension); phase 0 fills
 // d_bytes[n_dest][tiles] (output bytes per destination and tile of 256 records); after an exclusive scan of that

@@ -858,6 +858,34 @@ def _fastq_params(times=1, quality_cutoff=None, quality_base=33, nextseq_cutoff=
     return fp
 
 
+REDIRECT_OUTPUTS = ("too_short", "too_long", "untrimmed")     # destinations 1, 2, 3 of cg_fastq_collect_split
+
+
+def _redirect_bits(redirect, redirect_formats, params) -> Tuple[int, int]:
+    """(redirect, fasta_outputs) bits of cg_fastq_collect_split from output names and {name: "fasta" / "fastq"} (default:
+    the main output's format).  FASTA input can only be written as FASTA."""
+    redirect = tuple(redirect or ())
+    formats = dict(redirect_formats or {})
+    for name in list(redirect) + list(formats):
+        if name not in REDIRECT_OUTPUTS:
+            raise ValueError(f"unknown filter output {name!r} (one of {', '.join(REDIRECT_OUTPUTS)})")
+    main = "fastq" if params.format == _lib.CG_FORMAT_FASTQ else "fasta"
+    bits = fasta = 0
+    for i, name in enumerate(REDIRECT_OUTPUTS):
+        fmt = formats.get(name, main)
+        if fmt not in ("fastq", "fasta"):
+            raise ValueError(f"format of the {name} output must be 'fastq' or 'fasta', not {fmt!r}")
+        if name in redirect:
+            if fmt == "fastq" and params.format == _lib.CG_FORMAT_FASTA:
+                raise ValueError(f"FASTA input cannot be written as FASTQ (the {name} output)")
+            bits |= 1 << i
+        if fmt == "fasta":
+            fasta |= 1 << i
+    if bits & _lib.CG_REDIRECT_UNTRIMMED and params.discard_trimmed:
+        raise ValueError("the untrimmed output cannot be combined with discard_trimmed")
+    return bits, fasta
+
+
 def _device_set(adapters, ctx):
     if adapters is not None and not isinstance(adapters, Matchable):
         adapters = MultipleAdapters(list(adapters)) if len(adapters) else None
@@ -910,10 +938,16 @@ class FastqTrimmer:
     collect_statistics  also collect what the report needs beyond the counters (cg_fastq_stats_*): per-adapter
                         statistics, the poly-A and written-length histograms; ``statistics_vector()``,
                         ``adapter_statistics()``, ``poly_a_trimmed_lengths``, ``written_lengths``
+    redirect            filter outputs: names out of REDIRECT_OUTPUTS ("too_short", "too_long", "untrimmed") --
+                        --too-short-output / --too-long-output / --untrimmed-output.  The reads these filters remove
+                        are written to their own output, trimmed like the main output (``process_chunk_split``);
+                        "untrimmed" switches the untrimmed filter on and counts its reads in ``discarded``
+    redirect_formats    {output name: "fastq" or "fasta"}; an output not named has the main output's format
 
     ``process_chunk(bytes) -> bytes``; ``process_chunks(iterable)`` keeps one chunk in flight so that the
-    upload of chunk i+1 overlaps the download of chunk i.  ``statistics`` accumulates the counters of
-    ``cg_fastq_result`` over all chunks.  Chunks must consist of complete records (what
+    upload of chunk i+1 overlaps the download of chunk i.  With ``redirect``: ``process_chunk_split(bytes) ->
+    {"output": bytes, <redirected output>: bytes, ...}`` and ``process_chunks_split(iterable)``.  ``statistics``
+    accumulates the counters of ``cg_fastq_result`` over all chunks.  Chunks must consist of complete records (what
     ``dnaio.read_chunks`` yields; read_fastq_chunks / read_fasta_chunks).
     """
 
@@ -925,12 +959,15 @@ class FastqTrimmer:
                  length: Optional[int] = None, trim_n: bool = False, discard_casava: bool = False,
                  action: Optional[str] = "trim", revcomp: bool = False, rc_suffix: bool = True,
                  input_format: str = "fastq", output_format: Optional[str] = None,
-                 ctx: Optional[_lib.Context] = None, collect_statistics: bool = False):
-        self.ctx = ctx or _lib.default_context()
-        self.adapters, self._set = _device_set(adapters, self.ctx)
+                 ctx: Optional[_lib.Context] = None, collect_statistics: bool = False,
+                 redirect: Sequence[str] = (), redirect_formats: Optional[dict] = None):
         self.params = _fastq_params(times, quality_cutoff, quality_base, nextseq_cutoff, minimum_length, maximum_length,
                                     max_n, max_expected_errors, discard_trimmed, discard_untrimmed, cut, poly_a, length,
                                     trim_n, discard_casava, action, revcomp, rc_suffix, input_format, output_format)
+        self.redirect = tuple(dict.fromkeys(redirect or ()))
+        self._redirect, self._fasta_outputs = _redirect_bits(self.redirect, redirect_formats, self.params)
+        self.ctx = ctx or _lib.default_context()
+        self.adapters, self._set = _device_set(adapters, self.ctx)
         self._stats = None
         if collect_statistics:
             n = len(self.adapters._flatten()[0]) if self.adapters is not None else 0
@@ -980,8 +1017,53 @@ class FastqTrimmer:
             self.statistics[k] = self.statistics.get(k, 0) + v
         return out[: res.out_bytes].tobytes() if copy else out[: res.out_bytes]
 
+    def _no_redirect(self, what: str):
+        if self._redirect:
+            raise ValueError(f"filter outputs ({', '.join(self.redirect)}) cannot be combined with {what}; "
+                             "use process_chunk_split / process_chunks_split")
+
     def process_chunk(self, chunk) -> bytes:
+        self._no_redirect("process_chunk")
         return self._collect(self._submit(chunk))
+
+    def _collect_split(self, ticket, copy: bool = True) -> dict:
+        slot, n_bytes, chunk = ticket
+        out = self._out_buffer(slot, _output_capacity(n_bytes, self.params.format))
+        segments = np.zeros(5, dtype=np.int64)
+        while True:
+            res = _lib.cg_fastq_result()
+            rc = _lib.lib().cg_fastq_collect_split(
+                self.ctx.handle, slot, self._set.handle if self._set is not None else None, C.byref(self.params),
+                self._redirect, self._fasta_outputs, out.ctypes.data, out.size, C.byref(res), segments.ctypes.data)
+            # " rc" suffixes can exceed the bound; the call says how much it needs, run the chunk again
+            if rc != 0 and res.out_bytes > out.size:
+                slot, _, chunk = self._submit(chunk)
+                out = self._out_buffer(slot, res.out_bytes)
+                continue
+            _lib.check(rc)
+            break
+        for k, v in res.as_dict().items():
+            self.statistics[k] = self.statistics.get(k, 0) + v
+        names = ("output",) + REDIRECT_OUTPUTS
+        part = (lambda a, b: out[a:b].tobytes()) if copy else (lambda a, b: out[a:b])
+        return {name: part(segments[d], segments[d + 1]) for d, name in enumerate(names)
+                if d == 0 or name in self.redirect}
+
+    def process_chunk_split(self, chunk) -> dict:
+        """{"output": main output, and for every name in ``redirect``: the reads that filter removed} for one chunk,
+        every output in input order (``cg_fastq_collect_split``)."""
+        return self._collect_split(self._submit(chunk))
+
+    def process_chunks_split(self, chunks, copy: bool = True):
+        """process_chunk_split over an iterable with one chunk in flight (see process_chunks)."""
+        pending = None
+        for chunk in chunks:
+            ticket = self._submit(chunk)
+            if pending is not None:
+                yield self._collect_split(pending, copy)
+            pending = ticket
+        if pending is not None:
+            yield self._collect_split(pending, copy)
 
     def _demux_names(self):
         return _demux_names(self.adapters)
@@ -989,6 +1071,7 @@ class FastqTrimmer:
     def process_chunk_demux(self, chunk, unknown: str = "unknown") -> dict:
         """{adapter name: FASTQ bytes} + {unknown: reads without a match} -- what ``-o 'demux-{name}.fastq'`` writes
         for this chunk (every output in input order); ``cg_fastq_collect_demux``."""
+        self._no_redirect("demultiplexing")
         outputs, dest = self._demux_names()
         slot, n_bytes, _ = self._submit(chunk)
         out = self._out_buffer(slot, _output_capacity(n_bytes, self.params.format))
@@ -1016,6 +1099,7 @@ class FastqTrimmer:
         return b"".join(blobs), offsets
 
     def _process_chunk_rows(self, chunk, kind: int, blob: bytes, offsets: np.ndarray) -> Tuple[bytes, bytes]:
+        self._no_redirect(("info", "rest", "wildcard")[kind] + " file rows")
         if self.adapters is None:
             raise ValueError("these outputs need adapters")
         per_read = max(1, self.params.trim.times) * 2
@@ -1097,6 +1181,7 @@ class FastqTrimmer:
 
     def process_chunks(self, chunks, copy: bool = True):
         """copy=False yields uint8 array views into per-slot buffers: valid until the next-but-one result."""
+        self._no_redirect("process_chunks")
         pending = None
         for chunk in chunks:
             ticket = self._submit(chunk)
@@ -1118,7 +1203,10 @@ class PairedFastqTrimmer:
     mates (read_paired_fasta_chunks).  ``process_chunk(chunk1, chunk2) -> (bytes, bytes)``;
     ``statistics`` = (dict for R1, dict for R2).  ``collect_statistics``: as for FastqTrimmer, one accumulator per
     mate; ``statistics_vector()``, ``adapter_statistics()``, ``poly_a_trimmed_lengths`` and ``written_lengths`` give
-    one value per mate.
+    one value per mate.  ``redirect`` / ``redirect_formats``: as for FastqTrimmer, both mates of a removed pair go to
+    the filter's two outputs (--too-short-output / --too-short-paired-output, ...); with adapters on one mate only, a
+    pair is untrimmed when both mates are (cli.py:859-893).  ``process_chunk_split(chunk1, chunk2) -> {name: (bytes1,
+    bytes2)}`` and ``process_chunks_split(iterable of pairs)``.
     """
 
     MODES = {"any": 0, "both": 1, "first": 2}
@@ -1126,13 +1214,19 @@ class PairedFastqTrimmer:
     def __init__(self, adapters1=None, adapters2=None, options1: Optional[dict] = None,
                  options2: Optional[dict] = None, pair_filter: str = "any", pair_adapters: bool = False,
                  input_format: str = "fastq", output_format: Optional[str] = None,
-                 ctx: Optional[_lib.Context] = None, collect_statistics: bool = False):
+                 ctx: Optional[_lib.Context] = None, collect_statistics: bool = False,
+                 redirect: Sequence[str] = (), redirect_formats: Optional[dict] = None):
         if pair_filter not in self.MODES:
             raise ValueError("pair_filter must be 'any', 'both' or 'first'")
-        self.ctx = ctx or _lib.default_context()
         formats = dict(input_format=input_format, output_format=output_format)
         self.params1 = _fastq_params(**{**(options1 or {}), **formats})
         self.params2 = _fastq_params(**{**(options2 or {}), **formats})
+        self.redirect = tuple(dict.fromkeys(redirect or ()))
+        self._redirect, self._fasta_outputs = _redirect_bits(self.redirect, redirect_formats, self.params1)
+        _redirect_bits(self.redirect, redirect_formats, self.params2)
+        if self._redirect and pair_adapters:
+            raise ValueError("filter outputs cannot be combined with --pair-adapters")
+        self.ctx = ctx or _lib.default_context()
         self.mode = self.MODES[pair_filter]
         self.statistics = ({}, {})
         self._pairs = None
@@ -1212,7 +1306,46 @@ class PairedFastqTrimmer:
             for k, v in res.as_dict().items():
                 st[k] = st.get(k, 0) + v
 
+    def _no_redirect(self, what: str):
+        if self._redirect:
+            raise ValueError(f"filter outputs ({', '.join(self.redirect)}) cannot be combined with {what}; "
+                             "use process_chunk_split / process_chunks_split")
+
+    def _collect_split(self, tickets) -> dict:
+        (s1, b1), (s2, b2) = tickets
+        out1 = np.empty(_output_capacity(b1.size, self.params1.format), dtype=np.uint8)
+        out2 = np.empty(_output_capacity(b2.size, self.params2.format), dtype=np.uint8)
+        r1, r2 = _lib.cg_fastq_result(), _lib.cg_fastq_result()
+        seg1, seg2 = np.zeros(5, dtype=np.int64), np.zeros(5, dtype=np.int64)
+        _lib.check(_lib.lib().cg_fastq_collect_paired_split(
+            self.ctx.handle, s1, s2, self._set1.handle if self._set1 is not None else None,
+            self._set2.handle if self._set2 is not None else None, C.byref(self.params1), C.byref(self.params2),
+            self.mode, self._redirect, self._fasta_outputs, out1.ctypes.data, out1.size, out2.ctypes.data, out2.size,
+            C.byref(r1), C.byref(r2), seg1.ctypes.data, seg2.ctypes.data))
+        self._account(r1, r2)
+        names = ("output",) + REDIRECT_OUTPUTS
+        return {name: (out1[seg1[d]:seg1[d + 1]].tobytes(), out2[seg2[d]:seg2[d + 1]].tobytes())
+                for d, name in enumerate(names) if d == 0 or name in self.redirect}
+
+    def process_chunk_split(self, chunk1, chunk2) -> dict:
+        """{"output": (R1, R2) of the main outputs, and for every name in ``redirect``: (R1, R2) of the pairs that filter
+        removed} for one pair of chunks (``cg_fastq_collect_paired_split``)."""
+        return self._collect_split((self._submit(chunk1), self._submit(chunk2)))
+
+    def process_chunks_split(self, pairs):
+        """process_chunk_split over an iterable of (chunk1, chunk2) with one pair in flight: the upload of pair i+1
+        overlaps the work on pair i."""
+        pending = None
+        for chunk1, chunk2 in pairs:
+            tickets = (self._submit(chunk1), self._submit(chunk2))
+            if pending is not None:
+                yield self._collect_split(pending)
+            pending = tickets
+        if pending is not None:
+            yield self._collect_split(pending)
+
     def process_chunk(self, chunk1, chunk2) -> Tuple[bytes, bytes]:
+        self._no_redirect("process_chunk")
         (s1, b1), (s2, b2) = self._submit(chunk1), self._submit(chunk2)
         out1 = np.empty(_output_capacity(b1.size, self.params1.format), dtype=np.uint8)
         out2 = np.empty(_output_capacity(b2.size, self.params2.format), dtype=np.uint8)
@@ -1243,6 +1376,7 @@ class PairedFastqTrimmer:
         """
         if self._pairs is not None:
             raise ValueError("demultiplexing with --pair-adapters is not supported")
+        self._no_redirect("demultiplexing")
         names1, dest1 = _demux_names(self.adapters1)
         n1 = len(names1)
         if combinatorial:

@@ -445,6 +445,33 @@ int cg_fastq_collect_paired_demux(cg_ctx *ctx, int32_t slot1, int32_t slot2, con
                                   int64_t out_capacity1, uint8_t *out2, int64_t out_capacity2, cg_fastq_result *res1,
                                   cg_fastq_result *res2, int64_t *segments1, int64_t *segments2);
 
+/* Filter outputs: --too-short-output, --too-long-output, --untrimmed-output and their paired forms (SingleEndFilter /
+ * PairedEndFilter with a writer, steps.py:70-180).  A read (or pair) that one of these filters removes is written to
+ * that filter's output instead of being dropped: trimmed and modified exactly as the main output would have it.  The
+ * first filter in chain order that fires decides, as in cg_fastq_collect; filters without an output still drop.
+ * Destinations: 0 main, 1 too-short, 2 too-long, 3 untrimmed.  `out` holds them back to back, each in input order:
+ * output d is out[segments[d] .. segments[d + 1]) (5 values; outputs not redirected are empty).
+ *   redirect       CG_REDIRECT_* bits.  CG_REDIRECT_UNTRIMMED switches the untrimmed filter on for both mates (with
+ *                  adapters on one mate only, a pair is untrimmed when both mates are, cli.py:859-893); combined
+ *                  with discard_trimmed it is CG_EINVAL.  redirect == 0 gives what cg_fastq_collect(_paired) gives.
+ *   fasta_outputs  the same bits: a set bit writes that output as FASTA (">name\nsequence\n"), a clear one as FASTQ;
+ *                  the main output follows params.format.  With CG_FORMAT_FASTA input every redirect bit must be set.
+ * Counters: the filter counters count every removed read as before (the untrimmed output in `discarded`); n_written,
+ * bp_out and the written-length histogram of params.stats count the main output only.  The output bound and the
+ * "buffer too small -> out_bytes" contract are those of cg_fastq_collect (every record is written at most once). */
+#define CG_REDIRECT_TOO_SHORT 1
+#define CG_REDIRECT_TOO_LONG 2
+#define CG_REDIRECT_UNTRIMMED 4
+int cg_fastq_collect_split(cg_ctx *ctx, int32_t slot, const cg_adapterset *set, const cg_fastq_params *params,
+                           int32_t redirect, int32_t fasta_outputs, uint8_t *out, int64_t out_capacity,
+                           cg_fastq_result *res, int64_t *segments);
+/* Paired-end: cg_fastq_collect_paired's arguments; both mates of a pair go to the same destination. */
+int cg_fastq_collect_paired_split(cg_ctx *ctx, int32_t slot1, int32_t slot2, const cg_adapterset *set1,
+                                  const cg_adapterset *set2, const cg_fastq_params *params1, const cg_fastq_params *params2,
+                                  int32_t pair_filter_mode, int32_t redirect, int32_t fasta_outputs, uint8_t *out1,
+                                  int64_t out_capacity1, uint8_t *out2, int64_t out_capacity2, cg_fastq_result *res1,
+                                  cg_fastq_result *res2, int64_t *segments1, int64_t *segments2);
+
 /* ---- trim statistics (the payload of the end-of-run all-reduce, report.py:81-126) --------
  * Device-side reduction of a batch's match records into a fixed-layout int64 vector that carries everything the
  * reference's Statistics.__iadd__ adds up (report.py:81-126), so that one all-reduce merges the ranks:

@@ -1,6 +1,7 @@
 """End-to-end throughput of the FASTQ entry point (not a bench line; see DESIGN.md sections 4.6, 4.7).
 
   python tools/measure_fastq.py [n_reads] [chunk_megabytes] [fastq | fasta | fasta60 | barcodes] [--statistics]
+                                [--redirect]
 
 Builds n_reads synthetic FASTQ records of BASELINE configs[1]'s shape (150 bp, Phred+33 qualities, names
 "@SIM2:000000123") in pinned host memory, cuts the buffer into chunks of whole records and streams them
@@ -10,6 +11,8 @@ FASTA (">SIM2:000000123" and the sequence on one line / wrapped at 60 columns) t
 (input_format="fasta", -a AGATCGGAAGAGC -m 20: FASTA has no qualities to trim).  "barcodes": the FASTQ reads with
 the 96 anchored 5' barcodes of config 5 (-g ^BARCODE..., IndexedPrefixAdapters) instead of the 3' adapter.
 --statistics: the trimmer also collects the report's statistics (collect_statistics=True; cg_fastq_stats_*).
+--redirect: the filters keep what they remove (--too-short-output --untrimmed-output: process_chunks_split,
+cg_fastq_collect_split); the output bytes are those of all three outputs.
 """
 import json
 import sys
@@ -76,7 +79,8 @@ def build_fasta(n, wrap=None, pinned=True):
 
 def main():
     collect = "--statistics" in sys.argv
-    argv = [a for a in sys.argv if a != "--statistics"]
+    redirect = ("too_short", "untrimmed") if "--redirect" in sys.argv else ()
+    argv = [a for a in sys.argv if a not in ("--statistics", "--redirect")]
     n = int(argv[1]) if len(argv) > 1 else 4_000_000
     chunk_mb = int(argv[2]) if len(argv) > 2 else 64
     variant = argv[3] if len(argv) > 3 else "fastq"
@@ -87,8 +91,9 @@ def main():
     per_chunk = max(1, (chunk_mb << 20) // rec_len)
     chunks = [data[i * rec_len:min(n, i + per_chunk) * rec_len] for i in range(0, n, per_chunk)]
     adapters = [PA.BackAdapter("AGATCGGAAGAGC", max_errors=0.1)]
+    split = dict(redirect=redirect) if redirect else {}
     if variant == "fastq":
-        t = FastqTrimmer(adapters, quality_cutoff=(0, 20), minimum_length=20, collect_statistics=collect)
+        t = FastqTrimmer(adapters, quality_cutoff=(0, 20), minimum_length=20, collect_statistics=collect, **split)
         what = "FASTQ bytes in -> trimmed FASTQ bytes out (-a AGATCGGAAGAGC -q 20 -m 20), host to host"
     elif variant == "barcodes":
         from cutadapt_b200.configs import config5_barcodes
@@ -96,22 +101,29 @@ def main():
         barcodes = [PA.PrefixAdapter(b, max_errors=0.1, min_overlap=3, indels=True, name=f"bc{i}")
                     for i, b in enumerate(config5_barcodes())]
         t = FastqTrimmer(PA.MultipleAdapters([PA.IndexedPrefixAdapters(barcodes)]), quality_cutoff=(0, 20),
-                         minimum_length=20, collect_statistics=collect)
+                         minimum_length=20, collect_statistics=collect, **split)
         what = "FASTQ bytes in -> trimmed FASTQ bytes out (96 barcodes -g ^BC -q 20 -m 20), host to host"
     else:
-        t = FastqTrimmer(adapters, minimum_length=20, input_format="fasta", collect_statistics=collect)
+        t = FastqTrimmer(adapters, minimum_length=20, input_format="fasta", collect_statistics=collect, **split)
         what = f"FASTA ({variant}) bytes in -> trimmed FASTA bytes out (-a AGATCGGAAGAGC -m 20), host to host"
-    out_bytes = sum(len(o) for o in t.process_chunks(chunks[:9], copy=False))   # warm-up: every slot's buffers, pool
+    if redirect:
+        what += ", --too-short-output --untrimmed-output"
+
+        def run(cs):
+            return sum(len(o) for parts in t.process_chunks_split(cs, copy=False) for o in parts.values())
+    else:
+        def run(cs):
+            return sum(len(o) for o in t.process_chunks(cs, copy=False))
+    run(chunks[:9])                    # warm-up: every slot's buffers, pool
     t.statistics.clear()
     t0 = time.perf_counter()
-    out_bytes = 0
-    for o in t.process_chunks(chunks, copy=False):
-        out_bytes += len(o)
+    out_bytes = run(chunks)
     wall = time.perf_counter() - t0
     st = t.statistics
     print(json.dumps({
         "what": what,
-        "reads": n, "chunk_mb": chunk_mb, "collect_statistics": collect, "chunks": len(chunks), "reads_per_s": n / wall,
+        "reads": n, "chunk_mb": chunk_mb, "collect_statistics": collect, "redirect": list(redirect), "chunks": len(chunks),
+        "reads_per_s": n / wall,
         "in_GB_per_s": data.size / wall / 1e9, "out_GB_per_s": out_bytes / wall / 1e9,
         "in_bytes": int(data.size), "out_bytes": out_bytes, "wall_s": wall,
         "statistics": {k: int(v) for k, v in st.items()},

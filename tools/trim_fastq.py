@@ -9,10 +9,13 @@ on real files.
   python tools/trim_fastq.py -a ADAPT1 -A ADAPT2 -q 20 -m 20 -o out.1.fastq -p out.2.fastq in.1.fastq in.2.fastq
   python tools/trim_fastq.py -g bc1=^ACGTACGTAC -g bc2=^TTGCATTGCA -o 'demux-{name}.fastq' in.fastq     (demultiplex)
   python tools/trim_fastq.py -a AGATCGGAAGAGC -m 20 -o out.fasta in.fasta           (FASTA; also FASTQ -> FASTA)
+  python tools/trim_fastq.py -a AGATCGGAAGAGC -m 20 --too-short-output short.fastq --untrimmed-output untrimmed.fasta \
+      -o out.fastq in.fastq                                                            (filter outputs)
 
 The input format comes from the first byte of the (first) input, as cutadapt's files.detect_file_format does: '>' or
 '#' is FASTA, anything else (an empty file included) FASTQ.  The output is FASTA when the input is, when -o ends in
-.fasta / .fa, or with --fasta.  --json FILE also writes what the report shows per adapter (removed length x errors,
+.fasta / .fa, or with --fasta; every filter output (--too-short-output, --too-long-output, --untrimmed-output and the
+paired forms) gets its format from its own name the same way.  --json FILE also writes what the report shows per adapter (removed length x errors,
 bases preceding the adapter, reverse-complemented count), the poly-A and written-length histograms and the counters,
 collected on the device (collect_statistics=True); the stderr line stays as it is.
 """
@@ -65,6 +68,38 @@ def report_json(counters, adapter_statistics, poly_a, written):
             "written_lengths": {str(k): v for k, v in sorted(written.items())}}
 
 
+FILTER_OUTPUTS = (("too_short", "too-short"), ("too_long", "too-long"), ("untrimmed", "untrimmed"))
+
+
+def check_filter_outputs(ap, args, paired, demultiplex):
+    """The command-line errors of the reference around the filter outputs (cli.py:588-592, 600-622, 713-733, 798-808):
+    ap.error() exits with status 2."""
+    if not paired and args.untrimmed_paired_output:
+        ap.error("Option --untrimmed-paired-output can only be used when trimming paired-end reads.")
+    if paired:
+        for dest, name in FILTER_OUTPUTS:
+            if bool(getattr(args, dest + "_output")) != bool(getattr(args, dest + "_paired_output")):
+                ap.error("When trimming paired-end data, you must use either none or both of the"
+                         f" --{name}-output/--{name}-paired-output options.")
+    for length, dest, name, flag, what in ((args.minimum_length, "too_short", "too-short", "-m/--minimum-length", "minimum"),
+                                           (args.maximum_length, "too_long", "too-long", "-M/--maximum-length", "maximum")):
+        if length is None and (getattr(args, dest + "_output") or getattr(args, dest + "_paired_output")):
+            ap.error(f"When --{name}-output or --{name}-paired-output are used, a {what} length must be provided with "
+                     f"{flag}")
+        if not paired and getattr(args, dest + "_paired_output"):
+            ap.error("--too-short/long-paired-output cannot be used with single-end data")
+    if int(args.discard_trimmed) + int(args.discard_untrimmed) + int(bool(args.untrimmed_output)) > 1:
+        ap.error("Only one of the --discard-trimmed, --discard-untrimmed and --untrimmed-output options can be used at "
+                 "the same time.")
+    if demultiplex and (args.too_short_output or args.too_long_output):
+        ap.error("--too-short-output and --too-long-output cannot be combined with demultiplexing ({name} in -o)")
+
+
+def file_format(path, input_format, fasta):
+    """Format of an output file: FASTA for FASTA input, with --fasta, or for a .fasta / .fa name."""
+    return "fasta" if input_format == "fasta" or fasta or path.endswith((".fasta", ".fa")) else "fastq"
+
+
 def main():
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     for flag, dest in (("-a", "back"), ("-g", "front"), ("-b", "anywhere"), ("-A", "back2"), ("-G", "front2"),
@@ -77,7 +112,7 @@ def main():
     ap.add_argument("--quality-base", type=int, default=33)
     ap.add_argument("--nextseq-trim", type=int, default=None)
     ap.add_argument("-u", "--cut", type=int, action="append", default=[])
-    ap.add_argument("-m", "--minimum-length", type=int, default=0)
+    ap.add_argument("-m", "--minimum-length", type=int, default=None)
     ap.add_argument("-M", "--maximum-length", type=int, default=None)
     ap.add_argument("--max-n", type=float, default=None)
     ap.add_argument("--max-ee", type=float, default=None)
@@ -94,8 +129,14 @@ def main():
     ap.add_argument("-o", "--output", required=True, help="output FASTQ; with {name}: one file per adapter name")
     ap.add_argument("-p", "--paired-output")
     ap.add_argument("--json", default=None, metavar="FILE", help="write the report's statistics as JSON")
+    for dest, name in FILTER_OUTPUTS:
+        ap.add_argument(f"--{name}-output", dest=dest + "_output", metavar="FILE",
+                        help=f"write the reads the {name} filter removes to FILE instead of dropping them")
+        ap.add_argument(f"--{name}-paired-output", dest=dest + "_paired_output", metavar="FILE",
+                        help=f"the second mates of the pairs --{name}-output gets")
     ap.add_argument("inputs", nargs="+")
     args = ap.parse_args()
+    check_filter_outputs(ap, args, len(args.inputs) == 2, "{name}" in args.output)
     input_format = detect_format(args.inputs[0])
     fasta_out = input_format == "fasta" or args.fasta or args.output.endswith((".fasta", ".fa"))
     output_format = "fasta" if fasta_out and input_format == "fastq" else None
@@ -115,6 +156,11 @@ def main():
                   discard_untrimmed=args.discard_untrimmed, cut=args.cut, poly_a=args.poly_a, length=args.length,
                   trim_n=args.trim_n, discard_casava=args.discard_casava, action=args.action)
     formats = dict(input_format=input_format, output_format=output_format, collect_statistics=args.json is not None)
+    # filter outputs (the untrimmed output of a demultiplexer is its "unknown" output)
+    redirect = [d for d, _ in FILTER_OUTPUTS if getattr(args, d + "_output") and "{name}" not in args.output]
+    split = dict(redirect=redirect,
+                 redirect_formats={d: file_format(getattr(args, d + "_output"), input_format, args.fasta)
+                                   for d in redirect}) if redirect else {}
     ads1 = (make_adapters(args.back, "back", args.error_rate, args.overlap)
             + make_adapters(args.front, "front", args.error_rate, args.overlap)
             + make_adapters(args.anywhere, "anywhere", args.error_rate, args.overlap))
@@ -127,13 +173,25 @@ def main():
             ap.error("paired-end input needs -p")
         if detect_format(args.inputs[1]) != input_format:
             ap.error("both inputs must have the same format")
-        t = PairedFastqTrimmer(ads1, ads2, common, common, args.pair_filter, **formats)
+        t = PairedFastqTrimmer(ads1, ads2, common, common, args.pair_filter, **formats, **split)
         with open(args.inputs[0], "rb") as f1, open(args.inputs[1], "rb") as f2, \
                 open(args.output, "wb") as o1, open(args.paired_output, "wb") as o2:
-            for c1, c2 in paired_reader(f1, f2, args.buffer_size):
-                r1, r2 = t.process_chunk(c1, c2)
-                o1.write(r1)
-                o2.write(r2)
+            if redirect:
+                files = {d: (open(getattr(args, d + "_output"), "wb"), open(getattr(args, d + "_paired_output"), "wb"))
+                         for d in redirect}
+                files["output"] = (o1, o2)
+                for parts in t.process_chunks_split(paired_reader(f1, f2, args.buffer_size)):
+                    for name, (r1, r2) in parts.items():
+                        files[name][0].write(r1)
+                        files[name][1].write(r2)
+                for d in redirect:
+                    files[d][0].close()
+                    files[d][1].close()
+            else:
+                for c1, c2 in paired_reader(f1, f2, args.buffer_size):
+                    r1, r2 = t.process_chunk(c1, c2)
+                    o1.write(r1)
+                    o2.write(r2)
         stats = {"read1": t.statistics[0], "read2": t.statistics[1]}
     elif "{name}" in args.output:
         t = FastqTrimmer(ads1, **common, **formats)
@@ -144,10 +202,24 @@ def main():
                     if name == "unknown" and args.discard_untrimmed:
                         continue
                     if name not in files:
-                        files[name] = open(args.output.replace("{name}", name), "wb")
+                        # Demultiplexer(untrimmed_output=...): reads without a match go to --untrimmed-output
+                        path = args.untrimmed_output if name == "unknown" and args.untrimmed_output else \
+                            args.output.replace("{name}", name)
+                        files[name] = open(path, "wb")
                     files[name].write(data)
         for fh in files.values():
             fh.close()
+        stats = t.statistics
+    elif redirect:
+        t = FastqTrimmer(ads1, **common, **formats, **split)
+        with open(args.inputs[0], "rb") as f:
+            files = {d: open(getattr(args, d + "_output"), "wb") for d in redirect}
+            files["output"] = open(args.output, "wb")
+            for parts in t.process_chunks_split(reader(f, args.buffer_size), copy=False):
+                for name, data in parts.items():
+                    files[name].write(data)
+            for fh in files.values():
+                fh.close()
         stats = t.statistics
     else:
         t = FastqTrimmer(ads1, **common, **formats)
