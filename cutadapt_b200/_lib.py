@@ -40,6 +40,7 @@ CG_FORMAT_FASTQ_TO_FASTA = 2     # FASTQ in, FASTA out
 CG_REDIRECT_TOO_SHORT = 1        # cg_fastq_collect_split: --too-short-output (destination 1)
 CG_REDIRECT_TOO_LONG = 2         # --too-long-output (destination 2)
 CG_REDIRECT_UNTRIMMED = 4        # --untrimmed-output (destination 3)
+CG_INTERLEAVE_MAIN = 8           # cg_fastq_collect_paired_interleaved: the main output is interleaved
 
 
 class cg_kmer_entry(C.Structure):
@@ -204,6 +205,10 @@ def _declare(lib) -> None:
     lib.cg_fastq_collect_paired_split.argtypes = [vp, i32, i32, vp, vp, C.POINTER(cg_fastq_params),
                                                   C.POINTER(cg_fastq_params), i32, i32, i32, vp, i64, vp, i64,
                                                   C.POINTER(cg_fastq_result), C.POINTER(cg_fastq_result), vp, vp]
+    lib.cg_fastq_submit_interleaved.argtypes = [vp, vp, i64, i32, C.POINTER(i32), C.POINTER(i32)]
+    lib.cg_fastq_collect_paired_interleaved.argtypes = [vp, i32, i32, vp, vp, C.POINTER(cg_fastq_params),
+                                                        C.POINTER(cg_fastq_params), i32, i32, i32, i32, vp, i64, vp, i64,
+                                                        C.POINTER(cg_fastq_result), C.POINTER(cg_fastq_result), vp, vp]
     lib.cg_fastq_stats_create.argtypes = [vp, i32, C.POINTER(i32)]
     lib.cg_fastq_stats_read.argtypes = [vp, i32, C.POINTER(i32), C.POINTER(i32), vp, i64, C.POINTER(i64), C.c_int]
     lib.cg_fastq_stats_destroy.argtypes = [vp, i32]

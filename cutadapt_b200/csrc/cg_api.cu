@@ -128,6 +128,11 @@ struct FastqSlot {
     DevBuf<unsigned long long> d_fqstats;       // statistics on: the chunk's statistics vector (added on success)
     DevBuf<int32_t> d_polya;                    // statistics with --poly-a: bases PolyATrimmer removed, per record
     PinBuf<unsigned long long> h_fqstats;
+    DevBuf<int32_t> d_fold;                     // interleaved outputs: the sizes the partition runs on
+    DevBuf<unsigned long long> d_ilverr;        // interleaved input: first problem of the split, record << 32 | code
+    // interleaved input (cg_fastq_submit_interleaved): 0 = a chunk of its own, 1 / 2 = mate 1 / 2 of the chunk uploaded to
+    // mate 1's slot, split when the pair is collected; ilv_peer = the other mate's slot, ilv_format = input format
+    int ilv = 0, ilv_peer = -1, ilv_format = 0;
     unsigned long long *d_counters = nullptr;   // [0] newline total, [1..] CG_FQ_COUNTERS
     int *d_err = nullptr;                       // [0] code, [1] record
     PinBuf<uint8_t> h_in, h_out;
@@ -1612,7 +1617,8 @@ static void parallel_copy(cg_ctx *c, void *dst, const void *src, size_t n)
     });
 }
 
-static int fastq_format_error(const int err[2])
+// mate (FastqSlot::ilv): the record number of a mate of an interleaved chunk is given as the chunk's (2r or 2r + 1)
+static int fastq_format_error(const int err[2], int mate = 0)
 {
     if (err[0] == CG_FA_ERR_BEFORE_HEADER || err[0] == CG_FA_ERR_LATE_COMMENT)
         return fail(CG_EINVAL, std::string("FASTA format error in line ") + std::to_string((long long)(unsigned)err[1] + 1) +
@@ -1622,18 +1628,15 @@ static int fastq_format_error(const int err[2])
     static const char *what[] = {"", "a record does not start with '@'", "the third line of a record does not start with '+'",
                                  "sequence and qualities differ in length", "invalid quality value",
                                  "sequence descriptions don't match (the second one must be empty or equal to the first)"};
-    return fail(CG_EINVAL, std::string("FASTQ format error in record ") + std::to_string(err[1]) + ": " + what[err[0] & 7]);
+    const long long r = mate ? 2LL * err[1] + (mate - 1) : (long long)err[1];
+    return fail(CG_EINVAL, std::string("FASTQ format error in record ") + std::to_string(r) +
+                               (mate ? " of the interleaved chunk: " : ": ") + what[err[0] & 7]);
 }
 
-extern "C" int cg_fastq_submit(cg_ctx *c, const uint8_t *fastq, int64_t n_bytes, int32_t *slot_out)
+// Streams, counters and error words of a slot, the host pool; the upload of the chunk and its newline count
+static int fastq_slot_upload(cg_ctx *c, FastqSlot &f, const uint8_t *fastq, int64_t n_bytes)
 {
-    if (!c || !slot_out || n_bytes < 0 || (n_bytes && !fastq)) return fail(CG_EINVAL, "cg_fastq_submit: bad argument");
-    if (n_bytes >= (1LL << 31)) return fail(CG_EINVAL, "cg_fastq_submit: a chunk must be smaller than 2 GiB");
-    CU(cudaSetDevice(c->device));
-    const int si = c->fq_next;
-    FastqSlot &f = c->fq[si];
-    if (f.busy) return fail(CG_EINVAL, "cg_fastq_submit: all slots are in flight, collect one first");
-    c->fq_next = (si + 1) % CG_FQ_SLOTS;
+    f.ilv = 0;
     if (!f.stream) CU(cudaStreamCreateWithFlags(&f.stream, cudaStreamNonBlocking));
     if (!f.d_counters) CU(cudaMalloc((void **)&f.d_counters, (1 + CG_FQ_COUNTERS) * sizeof(unsigned long long)));
     if (!f.d_err) CU(cudaMalloc((void **)&f.d_err, 2 * sizeof(int)));
@@ -1662,8 +1665,47 @@ extern "C" int cg_fastq_submit(cg_ctx *c, const uint8_t *fastq, int64_t n_bytes,
         c->launches += 2;
     }
     CU(cudaMemcpyAsync(f.h_counters.p, f.d_counters, sizeof(unsigned long long), cudaMemcpyDeviceToHost, f.stream));
+    return CG_OK;
+}
+
+extern "C" int cg_fastq_submit(cg_ctx *c, const uint8_t *fastq, int64_t n_bytes, int32_t *slot_out)
+{
+    if (!c || !slot_out || n_bytes < 0 || (n_bytes && !fastq)) return fail(CG_EINVAL, "cg_fastq_submit: bad argument");
+    if (n_bytes >= (1LL << 31)) return fail(CG_EINVAL, "cg_fastq_submit: a chunk must be smaller than 2 GiB");
+    CU(cudaSetDevice(c->device));
+    const int si = c->fq_next;
+    FastqSlot &f = c->fq[si];
+    if (f.busy) return fail(CG_EINVAL, "cg_fastq_submit: all slots are in flight, collect one first");
+    c->fq_next = (si + 1) % CG_FQ_SLOTS;
+    const int rc = fastq_slot_upload(c, f, fastq, n_bytes);
+    if (rc != CG_OK) return rc;
     f.busy = true;
     *slot_out = si;
+    return CG_OK;
+}
+
+extern "C" int cg_fastq_submit_interleaved(cg_ctx *c, const uint8_t *chunk, int64_t n_bytes, int32_t format, int32_t *slot1,
+                                           int32_t *slot2)
+{
+    if (!c || !slot1 || !slot2 || n_bytes < 0 || (n_bytes && !chunk) || format < CG_FORMAT_FASTQ ||
+        format > CG_FORMAT_FASTQ_TO_FASTA)
+        return fail(CG_EINVAL, "cg_fastq_submit_interleaved: bad argument");
+    if (n_bytes >= (1LL << 31)) return fail(CG_EINVAL, "cg_fastq_submit_interleaved: a chunk must be smaller than 2 GiB");
+    CU(cudaSetDevice(c->device));
+    const int s1 = c->fq_next, s2 = (s1 + 1) % CG_FQ_SLOTS;
+    FastqSlot &f1 = c->fq[s1], &f2 = c->fq[s2];
+    if (f1.busy || f2.busy)
+        return fail(CG_EINVAL, "cg_fastq_submit_interleaved: two free slots are needed, collect one first");
+    c->fq_next = (s2 + 1) % CG_FQ_SLOTS;
+    int rc;
+    if ((rc = fastq_slot_upload(c, f1, chunk, n_bytes)) != CG_OK) return rc;
+    if ((rc = fastq_slot_upload(c, f2, nullptr, 0)) != CG_OK) return rc;     // its chunk comes from the split
+    f1.ilv = 1; f1.ilv_peer = s2;
+    f2.ilv = 2; f2.ilv_peer = s1;
+    f1.ilv_format = f2.ilv_format = format == CG_FORMAT_FASTA ? CG_FORMAT_FASTA : CG_FORMAT_FASTQ;
+    f1.busy = f2.busy = true;
+    *slot1 = s1;
+    *slot2 = s2;
     return CG_OK;
 }
 
@@ -1736,6 +1778,131 @@ static int fasta_stage_normalise(cg_ctx *c, FastqSlot &f, const cg_fastq_params 
     std::swap(f.d_in, f.d_norm);                // every later kernel reads the normalised chunk
     f.n_bytes = n_norm;
     *n_records = n;
+    return CG_OK;
+}
+
+// The demultiplexer's stable byte partition: record r has d_len[r] bytes (0: none) for destination d_dest[r].  f.d_outoff
+// receives every record's offset; segments (host, n_dest + 1 values) where each destination starts and *total the sum,
+// both once the stream has got there.
+static int fastq_partition(cg_ctx *c, FastqSlot &f, long long n, int n_dest, const int32_t *d_len, const int32_t *d_dest,
+                           int64_t *segments, long long *total, cudaStream_t st)
+{
+    const long long tiles = cg_demux_tiles(n), cells = tiles * n_dest;
+    int rc;
+    if ((rc = f.d_dmbytes.ensure((size_t)cells)) != CG_OK) return rc;
+    if ((rc = f.d_dmbase.ensure((size_t)cells + 1)) != CG_OK) return rc;
+    if ((rc = f.d_scan.ensure((size_t)cg_scan_tiles(cells) + 1)) != CG_OK) return rc;
+    CU(cg_launch_fastq_demux(0, d_len, d_dest, n, n_dest, f.d_dmbytes.p, nullptr, nullptr, st));
+    CU(cg_launch_scan_i32(f.d_dmbytes.p, cells, f.d_scan.p, f.d_dmbase.p, st));
+    CU(cg_launch_fastq_demux(1, d_len, d_dest, n, n_dest, nullptr, f.d_dmbase.p, f.d_outoff.p, st));
+    c->launches += 5;
+    // segment d starts at base[d][tile 0]; the last entry is the total
+    CU(cudaMemcpy2DAsync(segments, sizeof(int64_t), f.d_dmbase.p, (size_t)tiles * sizeof(int64_t), sizeof(int64_t),
+                         (size_t)n_dest, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(segments + n_dest, f.d_dmbase.p + cells, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(total, f.d_dmbase.p + cells, sizeof *total, cudaMemcpyDeviceToHost, st));
+    return CG_OK;
+}
+
+// Interleaved input (cg_fastq_submit_interleaved): the chunk uploaded to f1 becomes two mate chunks, f1 and f2, as if
+// each had been submitted.  FASTQ: records are 4 lines of the line index; FASTA: the chunk is normalised first (format
+// errors name lines of the chunk), its records are ">name\n" + sequence.  Per record its span, mate (r & 1) and name
+// (ilv_records_kernel, which also checks the FASTQ format), the mate-name check per pair (ilv_pairs_kernel), the
+// demultiplexer's partition of the record sizes by mate, one copy kernel into the two slots; then every slot's newline
+// count, as cg_fastq_submit leaves it.  Runs on f1's stream; the scratch buffers are f1's per-record buffers, which the
+// collect sizes anew.
+static int fastq_split_interleaved(cg_ctx *c, FastqSlot &f1, FastqSlot &f2, cudaStream_t st)
+{
+    CU(cudaStreamSynchronize(f2.stream));
+    CU(cudaStreamSynchronize(st));              // upload + newline count of the chunk
+    const bool fasta = f1.ilv_format == CG_FORMAT_FASTA;
+    FqStage g;
+    g.n_nl = (long long)f1.h_counters.p[0];
+    long long n_lines = g.n_nl;                 // the last line may come without its newline
+    if (f1.n_bytes > 0) {
+        uint8_t last = 0;
+        CU(cudaMemcpyAsync(&last, f1.d_in.p + f1.n_bytes - 1, 1, cudaMemcpyDeviceToHost, st));
+        CU(cudaStreamSynchronize(st));
+        if (last != '\n') n_lines += 1;
+    }
+    int rc;
+    long long n = 0;
+    if (!fasta) {
+        if (n_lines % 4 != 0)
+            return fail(CG_EINVAL, "FASTQ chunk does not consist of complete 4-line records (" + std::to_string(n_lines) +
+                                       " lines)");
+        n = n_lines / 4;
+        if ((rc = f1.d_nl.ensure((size_t)g.n_nl + 1)) != CG_OK) return rc;
+        CU(cg_launch_fastq_index(f1.d_in.p, f1.n_bytes, f1.d_tiles.p, nullptr, f1.d_nl.p, 1, st));
+        c->launches += 1;
+    } else if (n_lines > 0) {
+        cg_fastq_params plain;
+        memset(&plain, 0, sizeof plain);
+        if ((rc = fasta_stage_normalise(c, f1, &plain, n_lines, st, g, &n)) != CG_OK) return rc;
+    }
+    if (n % 2 != 0)
+        return fail(CG_EINVAL, "Interleaved input file incomplete: the chunk holds an odd number of records (" +
+                                   std::to_string(n) + "), record " + std::to_string(n - 1) + " has no mate");
+    int64_t seg[3] = {0, 0, 0};                 // mate 1 starts, mate 2 starts, end
+    if (n > 0) {
+        if ((rc = f1.d_rec.ensure((size_t)n + 1)) != CG_OK) return rc;
+        if ((rc = f1.d_len.ensure((size_t)n)) != CG_OK) return rc;
+        if ((rc = f1.d_outlen.ensure((size_t)n)) != CG_OK) return rc;
+        if ((rc = f1.d_dest.ensure((size_t)n)) != CG_OK) return rc;
+        if ((rc = f1.d_outoff.ensure((size_t)n + 1)) != CG_OK) return rc;
+        if ((rc = f1.d_ilverr.ensure(1)) != CG_OK) return rc;
+        const unsigned long long none = ~0ull;
+        CU(cudaMemcpyAsync(f1.d_ilverr.p, &none, sizeof none, cudaMemcpyHostToDevice, st));
+        // d_len: where each record starts, d_outlen: its size, d_dest: its mate
+        CU(cg_launch_interleaved_split(0, f1.d_in.p, f1.n_bytes, fasta ? nullptr : f1.d_nl.p, g.n_nl, n, f1.d_rec.p,
+                                       f1.d_len.p, f1.d_outlen.p, f1.d_dest.p, f1.d_ilverr.p, nullptr, 0, nullptr, nullptr,
+                                       fasta ? 1 : 0, st));
+        c->launches += 2;
+        long long total = 0;
+        if ((rc = fastq_partition(c, f1, n, 2, f1.d_outlen.p, f1.d_dest.p, seg, &total, st)) != CG_OK) return rc;
+        unsigned long long bad = none;
+        CU(cudaMemcpyAsync(&bad, f1.d_ilverr.p, sizeof bad, cudaMemcpyDeviceToHost, st));
+        CU(cudaStreamSynchronize(st));
+        if (bad != none) {
+            const long long r = (long long)(bad >> 32);
+            const int code = (int)(bad & 0xFFFFFFFFu);
+            if (code != CG_FQ_ERR_PAIR) {
+                const int e[2] = {code, (int)r};
+                return fastq_format_error(e);
+            }
+            CgFastqRecord h[2];
+            CU(cudaMemcpy(h, f1.d_rec.p + r - 1, sizeof h, cudaMemcpyDeviceToHost));
+            std::string names[2];
+            for (int k = 0; k < 2; ++k) {
+                names[k].resize((size_t)std::max(h[k].hdr_len, 0));
+                if (h[k].hdr_len > 0)
+                    CU(cudaMemcpy(&names[k][0], f1.d_in.p + h[k].hdr_start, (size_t)h[k].hdr_len, cudaMemcpyDeviceToHost));
+            }
+            return fail(CG_EINVAL, "Reads are improperly paired: records " + std::to_string(r - 1) + " and " +
+                                       std::to_string(r) + " of the interleaved chunk, read name '" + names[0] +
+                                       "' does not match '" + names[1] + "'");
+        }
+        std::swap(f1.d_in, f1.d_norm);          // the chunk becomes the source, d_in receives mate 1
+        if ((rc = f1.d_in.ensure((size_t)seg[1] + 64)) != CG_OK) return rc;
+        if ((rc = f2.d_in.ensure((size_t)(seg[2] - seg[1]) + 64)) != CG_OK) return rc;
+        CU(cg_launch_interleaved_split(1, f1.d_norm.p, 0, nullptr, 0, n, nullptr, f1.d_len.p, f1.d_outlen.p, nullptr,
+                                       nullptr, f1.d_outoff.p, seg[1], f1.d_in.p, f2.d_in.p, fasta ? 1 : 0, st));
+        c->launches += 1;
+    }
+    f1.n_bytes = seg[1];
+    f2.n_bytes = seg[2] - seg[1];
+    const int err_init[2] = {0, 0x7FFFFFFF};
+    for (FastqSlot *f : {&f1, &f2}) {
+        if ((rc = f->d_tiles.ensure((size_t)cg_fastq_tiles(f->n_bytes) + 1)) != CG_OK) return rc;
+        CU(cudaMemsetAsync(f->d_counters, 0, (1 + CG_FQ_COUNTERS) * sizeof(unsigned long long), st));
+        CU(cudaMemcpyAsync(f->d_err, err_init, sizeof err_init, cudaMemcpyHostToDevice, st));
+        if (f->n_bytes) {
+            CU(cg_launch_fastq_index(f->d_in.p, f->n_bytes, f->d_tiles.p, f->d_counters, nullptr, 0, st));
+            c->launches += 2;
+        }
+        CU(cudaMemcpyAsync(f->h_counters.p, f->d_counters, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+    }
+    CU(cudaStreamSynchronize(st));
     return CG_OK;
 }
 
@@ -1848,7 +2015,7 @@ static int fastq_stage_pack(cg_ctx *c, FastqSlot &f, cudaStream_t st, FqStage &g
     CU(cudaMemcpyAsync(&g.max_len, c->d_err + 1, sizeof(int), cudaMemcpyDeviceToHost, st));
     CU(cudaMemcpyAsync(fq_err, f.d_err, sizeof fq_err, cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
-    if (fq_err[0]) return fastq_format_error(fq_err);
+    if (fq_err[0]) return fastq_format_error(fq_err, f.ilv);
     return CG_OK;
 }
 
@@ -2083,6 +2250,8 @@ struct FqSplit {
     int redirect = 0;                // CG_REDIRECT_* bits
     int fasta_dests = 0;             // bit d: destination d is written as FASTA
     int32_t *d_route = nullptr;      // device, per record: destination, -1 = dropped
+    bool interleaved = false;        // cg_fastq_collect_paired_interleaved ...
+    int ilv_dests = 0;               // ... bit d: destination d is written interleaved
     static constexpr int n_dest = 4;
 };
 
@@ -2099,6 +2268,67 @@ static int split_check(const FqSplit &sp, const cg_fastq_params *fp, const char 
     return CG_OK;
 }
 
+// The counters of a mate into its result, once the stream has got there; reports format errors.
+static int fastq_stage_result(FastqSlot &f, const FqStage &g, cudaStream_t st, cg_fastq_result *res)
+{
+    int fq_err[2];
+    CU(cudaMemcpyAsync(fq_err, f.d_err, sizeof fq_err, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(f.h_counters.p, f.d_counters, (1 + CG_FQ_COUNTERS) * sizeof(unsigned long long),
+                       cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    if (fq_err[0]) return fastq_format_error(fq_err, f.ilv);
+    const unsigned long long *k = f.h_counters.p + 1;
+    res->n_records = g.n;
+    res->n_written = (int64_t)k[0]; res->bp_in = (int64_t)k[1]; res->bp_out = (int64_t)k[2];
+    res->with_adapters = (int64_t)k[3]; res->too_short = (int64_t)k[4]; res->too_long = (int64_t)k[5];
+    res->quality_trimmed_bp = (int64_t)k[6]; res->discarded = (int64_t)k[7]; res->too_many_n = (int64_t)k[8];
+    res->too_many_expected_errors = (int64_t)k[9];
+    res->casava_filtered = (int64_t)k[10];
+    res->reverse_complemented = (int64_t)k[11];
+    return CG_OK;
+}
+
+// The formatted records of a mate at f.d_outoff in d_out.  sp: one writer per format that has bytes to write (segments:
+// the destinations, host), each skipping the other format's destinations.
+static int fastq_write_records(cg_ctx *c, FastqSlot &f, const FqStage &g, uint8_t *d_out, const FqSplit *sp,
+                               const int64_t *segments, cudaStream_t st)
+{
+    if (!sp) {
+        CU(cg_launch_fastq_write(f.d_in.p, f.d_rec.p, f.d_interval.p, f.d_outoff.p, f.d_outlen.p, g.n, d_out, g.action,
+                                 f.d_keep.p, f.d_mask.p, g.rc_suffix, st, g.fasta_out() ? 1 : 0));
+        c->launches += 1;
+        return CG_OK;
+    }
+    for (int fa = 0; fa < 2; ++fa) {
+        bool present = false;
+        for (int d = 0; d < FqSplit::n_dest; ++d)
+            present |= ((sp->fasta_dests >> d) & 1) == fa && segments[d + 1] > segments[d];
+        if (!present) continue;
+        CU(cg_launch_fastq_write(f.d_in.p, f.d_rec.p, f.d_interval.p, f.d_outoff.p, f.d_outlen.p, g.n, d_out, g.action,
+                                 f.d_keep.p, f.d_mask.p, g.rc_suffix, st, fa, sp->d_route, sp->fasta_dests));
+        c->launches += 1;
+    }
+    return CG_OK;
+}
+
+// bytes of d_src to the caller's `out` (through the slot's pinned bounce buffer unless `out` is pinned)
+static int fastq_copy_out(cg_ctx *c, FastqSlot &f, uint8_t *out, const uint8_t *d_src, long long bytes, cudaStream_t st)
+{
+    if (bytes <= 0) return CG_OK;
+    if (is_pinned(out)) {
+        CU(cudaMemcpyAsync(out, d_src, (size_t)bytes, cudaMemcpyDeviceToHost, st));
+        CU(cudaStreamSynchronize(st));
+    } else {
+        const int rc = f.h_out.ensure((size_t)bytes);
+        if (rc != CG_OK) return rc;
+        CU(cudaMemcpyAsync(f.h_out.p, d_src, (size_t)bytes, cudaMemcpyDeviceToHost, st));
+        CU(cudaStreamSynchronize(st));
+        parallel_copy(c, out, f.h_out.p, (size_t)bytes);
+    }
+    c->d2h_bytes += bytes;
+    return CG_OK;
+}
+
 // sizes -> offsets -> formatted records -> host; counters.  segments (host, n_dest + 1 values): where each destination
 // starts in `out`.
 static int fastq_stage_output(cg_ctx *c, FastqSlot &f, const FqStage &g, cudaStream_t st, uint8_t *out,
@@ -2108,76 +2338,65 @@ static int fastq_stage_output(cg_ctx *c, FastqSlot &f, const FqStage &g, cudaStr
     const long long n = g.n;
     int rc;
     long long total = 0;
-    int fq_err[2];
     if (dm || sp) {
-        const int n_dest = dm ? dm->n_dest() : FqSplit::n_dest;
-        const int32_t *d_dest = dm ? dm->d_dest : sp->d_route;
-        const long long tiles = cg_demux_tiles(n), cells = tiles * n_dest;
-        if ((rc = f.d_dmbytes.ensure((size_t)cells)) != CG_OK) return rc;
-        if ((rc = f.d_dmbase.ensure((size_t)cells + 1)) != CG_OK) return rc;
-        if ((rc = f.d_scan.ensure((size_t)cg_scan_tiles(cells) + 1)) != CG_OK) return rc;
-        CU(cg_launch_fastq_demux(0, f.d_outlen.p, d_dest, n, n_dest, f.d_dmbytes.p, nullptr, nullptr, st));
-        CU(cg_launch_scan_i32(f.d_dmbytes.p, cells, f.d_scan.p, f.d_dmbase.p, st));
-        CU(cg_launch_fastq_demux(1, f.d_outlen.p, d_dest, n, n_dest, nullptr, f.d_dmbase.p, f.d_outoff.p, st));
-        c->launches += 5;
-        // segment d starts at base[d][tile 0]; the last entry is the total
-        CU(cudaMemcpy2DAsync(segments, sizeof(int64_t), f.d_dmbase.p, (size_t)tiles * sizeof(int64_t), sizeof(int64_t),
-                             (size_t)n_dest, cudaMemcpyDeviceToHost, st));
-        CU(cudaMemcpyAsync(segments + n_dest, f.d_dmbase.p + cells, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
-        CU(cudaMemcpyAsync(&total, f.d_dmbase.p + cells, sizeof total, cudaMemcpyDeviceToHost, st));
+        rc = fastq_partition(c, f, n, dm ? dm->n_dest() : FqSplit::n_dest, f.d_outlen.p, dm ? dm->d_dest : sp->d_route,
+                             segments, &total, st);
+        if (rc != CG_OK) return rc;
     } else {
         CU(cg_launch_scan_i32(f.d_outlen.p, n, f.d_scan.p, f.d_outoff.p, st));
         c->launches += 3;
         CU(cudaMemcpyAsync(&total, f.d_outoff.p + n, sizeof total, cudaMemcpyDeviceToHost, st));
     }
-    CU(cudaMemcpyAsync(fq_err, f.d_err, sizeof fq_err, cudaMemcpyDeviceToHost, st));
-    CU(cudaMemcpyAsync(f.h_counters.p, f.d_counters, (1 + CG_FQ_COUNTERS) * sizeof(unsigned long long),
-                       cudaMemcpyDeviceToHost, st));
-    CU(cudaStreamSynchronize(st));
-    if (fq_err[0]) return fastq_format_error(fq_err);
-    const unsigned long long *k = f.h_counters.p + 1;
-    res->n_records = n;
-    res->n_written = (int64_t)k[0]; res->bp_in = (int64_t)k[1]; res->bp_out = (int64_t)k[2];
-    res->with_adapters = (int64_t)k[3]; res->too_short = (int64_t)k[4]; res->too_long = (int64_t)k[5];
-    res->quality_trimmed_bp = (int64_t)k[6]; res->discarded = (int64_t)k[7]; res->too_many_n = (int64_t)k[8];
-    res->too_many_expected_errors = (int64_t)k[9];
-    res->casava_filtered = (int64_t)k[10];
-    res->reverse_complemented = (int64_t)k[11];
+    if ((rc = fastq_stage_result(f, g, st, res)) != CG_OK) return rc;
     res->out_bytes = total;
     if (total > out_capacity)
         return fail(CG_EINVAL, "cg_fastq_collect: output buffer too small (" + std::to_string(total) + " bytes needed)");
     if (total > 0) {
         if (!out) return fail(CG_EINVAL, "cg_fastq_collect: out is NULL");
         if ((rc = f.d_out.ensure((size_t)total + 64)) != CG_OK) return rc;
-        if (sp) {
-            // one writer per format that has bytes to write, each skipping the other format's destinations
-            for (int fa = 0; fa < 2; ++fa) {
-                bool present = false;
-                for (int d = 0; d < FqSplit::n_dest; ++d)
-                    present |= ((sp->fasta_dests >> d) & 1) == fa && segments[d + 1] > segments[d];
-                if (!present) continue;
-                CU(cg_launch_fastq_write(f.d_in.p, f.d_rec.p, f.d_interval.p, f.d_outoff.p, f.d_outlen.p, n, f.d_out.p,
-                                         g.action, f.d_keep.p, f.d_mask.p, g.rc_suffix, st, fa, sp->d_route,
-                                         sp->fasta_dests));
-                c->launches += 1;
-            }
-        } else {
-            CU(cg_launch_fastq_write(f.d_in.p, f.d_rec.p, f.d_interval.p, f.d_outoff.p, f.d_outlen.p, n, f.d_out.p, g.action,
-                                     f.d_keep.p, f.d_mask.p, g.rc_suffix, st, g.fasta_out() ? 1 : 0));
-            c->launches += 1;
-        }
-        if (is_pinned(out)) {
-            CU(cudaMemcpyAsync(out, f.d_out.p, (size_t)total, cudaMemcpyDeviceToHost, st));
-            CU(cudaStreamSynchronize(st));
-        } else {
-            if ((rc = f.h_out.ensure((size_t)total)) != CG_OK) return rc;
-            CU(cudaMemcpyAsync(f.h_out.p, f.d_out.p, (size_t)total, cudaMemcpyDeviceToHost, st));
-            CU(cudaStreamSynchronize(st));
-            parallel_copy(c, out, f.h_out.p, (size_t)total);
-        }
-        c->d2h_bytes += total;
+        if ((rc = fastq_write_records(c, f, g, f.d_out.p, sp, segments, st)) != CG_OK) return rc;
+        if ((rc = fastq_copy_out(c, f, out, f.d_out.p, total, st)) != CG_OK) return rc;
     }
     return CG_OK;
+}
+
+// Interleaved outputs (cg_fastq_collect_paired_interleaved): bit d of sp.ilv_dests = destination d gets both mates in
+// out1, R1 then R2 per pair.  The pair's sizes are folded into mate 1 for the partition, mate 2 then follows its mate 1
+// (off1 + len1); both mates go through the writer into one device buffer, mate 1's region (total1 bytes) then mate 2's,
+// which two copies return.
+static int fastq_stage_output_interleaved(cg_ctx *c, FastqSlot &f1, const FqStage &g1, FastqSlot &f2, const FqStage &g2,
+                                          cudaStream_t st, uint8_t *out1, int64_t out_capacity1, uint8_t *out2,
+                                          int64_t out_capacity2, cg_fastq_result *res1, cg_fastq_result *res2,
+                                          int64_t *segments1, int64_t *segments2, const FqSplit &sp)
+{
+    const long long n = g1.n;
+    int rc;
+    if ((rc = f1.d_fold.ensure((size_t)n)) != CG_OK) return rc;
+    if ((rc = f2.d_fold.ensure((size_t)n)) != CG_OK) return rc;
+    CU(cg_launch_fastq_interleave(0, n, sp.d_route, sp.ilv_dests, f1.d_outlen.p, f2.d_outlen.p, f1.d_fold.p, f2.d_fold.p,
+                                  nullptr, nullptr, nullptr, st));
+    c->launches += 1;
+    long long total1 = 0, total2 = 0;
+    if ((rc = fastq_partition(c, f1, n, FqSplit::n_dest, f1.d_fold.p, sp.d_route, segments1, &total1, st)) != CG_OK) return rc;
+    if ((rc = fastq_partition(c, f2, n, FqSplit::n_dest, f2.d_fold.p, sp.d_route, segments2, &total2, st)) != CG_OK) return rc;
+    CU(cg_launch_fastq_interleave(1, n, sp.d_route, sp.ilv_dests, f1.d_outlen.p, f2.d_outlen.p, nullptr, nullptr,
+                                  f1.d_outoff.p, f2.d_outoff.p, f1.d_dmbase.p + cg_demux_tiles(n) * FqSplit::n_dest, st));
+    c->launches += 1;
+    if ((rc = fastq_stage_result(f1, g1, st, res1)) != CG_OK) return rc;
+    if ((rc = fastq_stage_result(f2, g2, st, res2)) != CG_OK) return rc;
+    res1->out_bytes = total1;
+    res2->out_bytes = total2;
+    if (total1 > out_capacity1 || total2 > out_capacity2)
+        return fail(CG_EINVAL, "cg_fastq_collect_paired_interleaved: output buffer too small (" + std::to_string(total1) +
+                                   " and " + std::to_string(total2) + " bytes needed)");
+    if ((total1 && !out1) || (total2 && !out2)) return fail(CG_EINVAL, "cg_fastq_collect_paired_interleaved: out is NULL");
+    if (total1 + total2 == 0) return CG_OK;
+    if ((rc = f1.d_out.ensure((size_t)(total1 + total2) + 64)) != CG_OK) return rc;
+    // a pair has bytes in a destination for both mates or for neither: segments1 says which formats mate 2 needs too
+    if ((rc = fastq_write_records(c, f1, g1, f1.d_out.p, &sp, segments1, st)) != CG_OK) return rc;
+    if ((rc = fastq_write_records(c, f2, g2, f1.d_out.p, &sp, segments1, st)) != CG_OK) return rc;
+    if ((rc = fastq_copy_out(c, f1, out1, f1.d_out.p, total1, st)) != CG_OK) return rc;
+    return fastq_copy_out(c, f2, out2, f1.d_out.p + total1, total2, st);
 }
 
 // --info-file rows of a chunk, an extra output of a collect
@@ -2236,6 +2455,7 @@ static int fastq_collect_impl(cg_ctx *c, int32_t slot, const cg_adapterset *s, c
     if (s && s->ctx != c) return fail(CG_EINVAL, "adapter set belongs to another context");
     FastqSlot &f = c->fq[slot];
     if (!f.busy) return fail(CG_EINVAL, "cg_fastq_collect: nothing was submitted to this slot");
+    if (f.ilv) return fail(CG_EINVAL, "cg_fastq_collect: the slot holds a mate of an interleaved chunk, collect it as a pair");
     CU(cudaSetDevice(c->device));
     f.busy = false;
     memset(res, 0, sizeof *res);
@@ -2428,6 +2648,9 @@ static int fastq_collect_paired_impl(cg_ctx *c, int32_t slot1, int32_t slot2, co
         return fail(CG_EINVAL, "--revcomp on pairs (PairedReverseComplementer) is not available on the device path");
     FastqSlot &f1 = c->fq[slot1], &f2 = c->fq[slot2];
     if (!f1.busy || !f2.busy) return fail(CG_EINVAL, "cg_fastq_collect_paired: nothing was submitted to a slot");
+    if ((f1.ilv || f2.ilv) && (f1.ilv != 1 || f2.ilv != 2 || f1.ilv_peer != slot2 || f2.ilv_peer != slot1))
+        return fail(CG_EINVAL, "cg_fastq_collect_paired: the two slots were not submitted together (an interleaved chunk's "
+                               "slots go in the order cg_fastq_submit_interleaved gave them)");
     CU(cudaSetDevice(c->device));
     f1.busy = f2.busy = false;
     if (fp1->format != fp2->format) return fail(CG_EINVAL, "cg_fastq_collect_paired: both mates must have the same format");
@@ -2437,6 +2660,14 @@ static int fastq_collect_paired_impl(cg_ctx *c, int32_t slot1, int32_t slot2, co
     cudaStream_t st = f1.stream;
     FqStage g1, g2;
     int rc;
+    if (f1.ilv) {
+        if ((fp1->format == CG_FORMAT_FASTA) != (f1.ilv_format == CG_FORMAT_FASTA)) {
+            cudaStreamSynchronize(f2.stream);
+            return fail(CG_EINVAL, "cg_fastq_collect_paired: the input format of the parameters is not the one the "
+                                   "interleaved chunk was submitted with");
+        }
+        if ((rc = fastq_split_interleaved(c, f1, f2, st)) != CG_OK) return rc;
+    }
     // one statistics accumulator per mate, as the reference keeps per-mate statistics (report.py:162-208)
     if (fp1->stats != 0 && fp1->stats == fp2->stats) {
         cudaStreamSynchronize(f2.stream);
@@ -2484,8 +2715,14 @@ static int fastq_collect_paired_impl(cg_ctx *c, int32_t slot1, int32_t slot2, co
     const int32_t *route = sp ? sp->d_route : nullptr;
     if ((rc = fastq_stage_stats_tail(c, f1, g1, st, route)) != CG_OK) return rc;
     if ((rc = fastq_stage_stats_tail(c, f2, g2, st, route)) != CG_OK) return rc;
-    if ((rc = fastq_stage_output(c, f1, g1, st, out1, out_capacity1, res1, dm, segments1, sp)) != CG_OK) return rc;
-    if ((rc = fastq_stage_output(c, f2, g2, st, out2, out_capacity2, res2, dm, segments2, sp)) != CG_OK) return rc;
+    if (sp && sp->interleaved) {
+        rc = fastq_stage_output_interleaved(c, f1, g1, f2, g2, st, out1, out_capacity1, out2, out_capacity2, res1, res2,
+                                            segments1, segments2, *sp);
+        if (rc != CG_OK) return rc;
+    } else {
+        if ((rc = fastq_stage_output(c, f1, g1, st, out1, out_capacity1, res1, dm, segments1, sp)) != CG_OK) return rc;
+        if ((rc = fastq_stage_output(c, f2, g2, st, out2, out_capacity2, res2, dm, segments2, sp)) != CG_OK) return rc;
+    }
     if ((rc = check_err_flag(c)) != CG_OK) return rc;
     fastq_stats_commit(f1, g1, fp1, *res1);
     fastq_stats_commit(f2, g2, fp2, *res2);
@@ -2513,6 +2750,28 @@ extern "C" int cg_fastq_collect_paired_split(cg_ctx *c, int32_t slot1, int32_t s
     FqSplit sp;
     sp.redirect = redirect;
     sp.fasta_dests = split_fasta_dests(fp1, fasta_outputs);
+    return fastq_collect_paired_impl(c, slot1, slot2, s1, s2, nullptr, fp1, fp2, pair_filter_mode, out1, out_capacity1, out2,
+                                     out_capacity2, res1, res2, nullptr, segments1, segments2, &sp);
+}
+
+extern "C" int cg_fastq_collect_paired_interleaved(cg_ctx *c, int32_t slot1, int32_t slot2, const cg_adapterset *s1,
+                                                   const cg_adapterset *s2, const cg_fastq_params *fp1,
+                                                   const cg_fastq_params *fp2, int32_t pair_filter_mode, int32_t redirect,
+                                                   int32_t fasta_outputs, int32_t interleaved_outputs, uint8_t *out1,
+                                                   int64_t out_capacity1, uint8_t *out2, int64_t out_capacity2,
+                                                   cg_fastq_result *res1, cg_fastq_result *res2, int64_t *segments1,
+                                                   int64_t *segments2)
+{
+    if (!segments1 || !segments2) return fail(CG_EINVAL, "cg_fastq_collect_paired_interleaved: bad argument");
+    if (interleaved_outputs & ~(CG_INTERLEAVE_MAIN | 7))
+        return fail(CG_EINVAL, "cg_fastq_collect_paired_interleaved: interleaved_outputs takes CG_INTERLEAVE_MAIN and "
+                               "CG_REDIRECT_* bits only");
+    for (int d = 0; d <= FqSplit::n_dest; ++d) segments1[d] = segments2[d] = 0;
+    FqSplit sp;
+    sp.redirect = redirect;
+    sp.fasta_dests = split_fasta_dests(fp1, fasta_outputs);
+    sp.interleaved = true;
+    sp.ilv_dests = ((interleaved_outputs & CG_INTERLEAVE_MAIN) ? 1 : 0) | ((interleaved_outputs & 7) << 1);
     return fastq_collect_paired_impl(c, slot1, slot2, s1, s2, nullptr, fp1, fp2, pair_filter_mode, out1, out_capacity1, out2,
                                      out_capacity2, res1, res2, nullptr, segments1, segments2, &sp);
 }

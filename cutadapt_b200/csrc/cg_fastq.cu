@@ -922,6 +922,86 @@ __global__ void fq_pair_select_kernel(long long n, int pair, const cg_match_rec 
     }
 }
 
+// ---- interleaved input (cg_fastq_submit_interleaved): record 2p of the chunk is record p of mate 1, record 2p + 1
+// record p of mate 2.  One thread per record: where the record lies in the chunk (start, size), its mate (dest = r & 1)
+// and its name (rec).  FASTQ (nl_pos != nullptr): lines 4r .. 4r+3 with their newlines, the format checked by
+// fq_record_core; FASTA: the record table of the normalised chunk, ">name\n" + sequence, to which the copy appends
+// the '\n' the normalised buffer leaves out.  err: the first problem as one 64-bit word, record << 32 | code.
+__global__ void ilv_records_kernel(const uint8_t *buf, long long n, const uint32_t *nl_pos, long long n_nl,
+                                   long long n_records, CgFastqRecord *rec, int32_t *start, int32_t *size, int32_t *dest,
+                                   unsigned long long *err)
+{
+    const long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= n_records) return;
+    long long s, e;
+    if (nl_pos) {
+        CgFastqRecord o;
+        int len;
+        const int bad = fq_record_core(buf, n, nl_pos, n_nl, r, 0, 0, &o, &len);
+        if (bad) atomicMin(err, ((unsigned long long)r << 32) | (unsigned)bad);
+        rec[r] = o;
+        s = r == 0 ? 0 : (long long)nl_pos[4 * r - 1] + 1;
+        e = 4 * r + 3 < n_nl ? (long long)nl_pos[4 * r + 3] + 1 : n;
+    } else {
+        s = (long long)rec[r].hdr_start - 1;
+        e = (r + 1 < n_records ? (long long)rec[r + 1].hdr_start - 1 : n) + 1;
+    }
+    start[r] = (int32_t)s;
+    size[r] = (int32_t)(e - s);
+    dest[r] = (int32_t)(r & 1);
+}
+
+// one thread per pair: the mates' names must match (fq_mates_match); a mismatch is reported at the pair's second record,
+// after any format error of that record (code CG_FQ_ERR_PAIR sorts behind the format codes)
+__global__ void ilv_pairs_kernel(const uint8_t *buf, const CgFastqRecord *rec, long long n_pairs, unsigned long long *err)
+{
+    const long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= n_pairs) return;
+    const CgFastqRecord a = rec[2 * p], b = rec[2 * p + 1];
+    if (!fq_mates_match(buf + a.hdr_start, a.hdr_len, buf + b.hdr_start, b.hdr_len))
+        atomicMin(err, ((unsigned long long)(2 * p + 1) << 32) | (unsigned)CG_FQ_ERR_PAIR);
+}
+
+// one warp per record: the record's bytes to its offset in its mate's chunk (mate 2's offsets start at seg1)
+__global__ void __launch_bounds__(256) ilv_copy_kernel(const uint8_t *src, const int32_t *start, const int32_t *size,
+                                                        const int64_t *off, long long n_records, long long seg1,
+                                                        uint8_t *dst1, uint8_t *dst2, int fasta)
+{
+    const int lane = threadIdx.x & 31;
+    const long long warps = ((long long)gridDim.x * blockDim.x) >> 5;
+    for (long long r = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5; r < n_records; r += warps) {
+        uint8_t *d = (r & 1) ? dst2 + (off[r] - seg1) : dst1 + off[r];
+        const uint8_t *s = src + start[r];
+        const int len = size[r] - (fasta ? 1 : 0);
+        for (int j = lane; j < len; j += 32) d[j] = s[j];
+        if (fasta && lane == 0) d[len] = '\n';
+    }
+}
+
+// ---- interleaved outputs (cg_fastq_collect_paired_interleaved): bit d of ilv = destination d is interleaved.  Its
+// pairs are sized as one record of mate 1 (both mates' bytes) and none of mate 2 for the partition ...
+__global__ void fq_ilv_fold_kernel(long long n, const int32_t *route, int ilv, const int32_t *len1, const int32_t *len2,
+                                   int32_t *fold1, int32_t *fold2)
+{
+    const long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= n) return;
+    const int d = route[r];
+    const bool in = d >= 0 && ((ilv >> d) & 1);
+    fold1[r] = in ? len1[r] + len2[r] : len1[r];
+    fold2[r] = in ? 0 : len2[r];
+}
+
+// ... after which mate 2 of such a pair follows its mate 1 (off1 + len1); every other record of mate 2 moves behind
+// mate 1's region (*total1 bytes), so that both mates are written into one buffer
+__global__ void fq_ilv_offsets_kernel(long long n, const int32_t *route, int ilv, const int64_t *off1, const int32_t *len1,
+                                      const int32_t *len2, int64_t *off2, const int64_t *total1)
+{
+    const long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= n || len2[r] <= 0) return;
+    const int d = route[r];
+    off2[r] = ((ilv >> d) & 1) ? off1[r] + len1[r] : off2[r] + *total1;
+}
+
 }  // namespace
 
 // ------------------------------------------------------------------------------------------
@@ -1145,6 +1225,40 @@ cudaError_t cg_launch_fastq_pair_select(long long n_records, int pair, const cg_
     if (n_records <= 0) return cudaSuccess;
     fq_pair_select_kernel<<<(unsigned)((n_records + 255) / 256), 256, 0, st>>>(n_records, pair, d_cur1, slots1, d_cur2, slots2,
                                                                               d_best1, d_best2, slots, d_best_key);
+    return cudaGetLastError();
+}
+
+cudaError_t cg_launch_interleaved_split(int phase, const uint8_t *d_buf, long long n_bytes, const uint32_t *d_nl_pos,
+                                        long long n_newlines, long long n_records, CgFastqRecord *d_rec, int32_t *d_start,
+                                        int32_t *d_size, int32_t *d_dest, unsigned long long *d_err, const int64_t *d_off,
+                                        long long seg1, uint8_t *d_out1, uint8_t *d_out2, int fasta, cudaStream_t st)
+{
+    if (n_records <= 0) return cudaSuccess;
+    if (phase == 0) {
+        ilv_records_kernel<<<(unsigned)((n_records + 255) / 256), 256, 0, st>>>(d_buf, n_bytes, d_nl_pos, n_newlines, n_records,
+                                                                               d_rec, d_start, d_size, d_dest, d_err);
+        const long long pairs = n_records / 2;
+        if (pairs > 0)
+            ilv_pairs_kernel<<<(unsigned)((pairs + 255) / 256), 256, 0, st>>>(d_buf, d_rec, pairs, d_err);
+    } else {
+        long long grid = (n_records + 7) / 8;
+        grid = cg_grid_cap(grid, 16);
+        ilv_copy_kernel<<<(unsigned)grid, 256, 0, st>>>(d_buf, d_start, d_size, d_off, n_records, seg1, d_out1, d_out2,
+                                                         fasta);
+    }
+    return cudaGetLastError();
+}
+
+cudaError_t cg_launch_fastq_interleave(int phase, long long n_records, const int32_t *d_route, int ilv,
+                                       const int32_t *d_len1, const int32_t *d_len2, int32_t *d_fold1, int32_t *d_fold2,
+                                       const int64_t *d_off1, int64_t *d_off2, const int64_t *d_total1, cudaStream_t st)
+{
+    if (n_records <= 0) return cudaSuccess;
+    const unsigned grid = (unsigned)((n_records + 255) / 256);
+    if (phase == 0)
+        fq_ilv_fold_kernel<<<grid, 256, 0, st>>>(n_records, d_route, ilv, d_len1, d_len2, d_fold1, d_fold2);
+    else
+        fq_ilv_offsets_kernel<<<grid, 256, 0, st>>>(n_records, d_route, ilv, d_off1, d_len1, d_len2, d_off2, d_total1);
     return cudaGetLastError();
 }
 

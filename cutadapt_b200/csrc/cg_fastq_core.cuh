@@ -329,6 +329,24 @@ CG_HD int fq_finish_core(int m1, int m2, bool pair, int enabled1, int enabled2, 
     return -1;
 }
 
+// Do two headers (without '@' / '>') name the two mates of one pair?  The rule of dnaio's paired readers
+// (doc/reference.rst:925-950): compare the IDs, each header up to its first space or tab; a final '1', '2' or '3' of the
+// IDs is ignored, so "read1/1 some text" matches "read1/2 other text", but "my_read/1;1" does not match "my_read/2;1".
+// This is the strict reading: the last character is dropped only when it is 1, 2 or 3 in BOTH IDs ("r1" and "r"
+// differ).  No stored answer of the reference pins that case.
+#define CG_FQ_ERR_PAIR 8      // interleaved input: the two records of a pair are not mates
+CG_HD bool fq_mates_match(const uint8_t *h1, int len1, const uint8_t *h2, int len2)
+{
+    int i1 = 0, i2 = 0;
+    while (i1 < len1 && h1[i1] != ' ' && h1[i1] != '\t') ++i1;
+    while (i2 < len2 && h2[i2] != ' ' && h2[i2] != '\t') ++i2;
+    if (i1 > 0 && i2 > 0 && (uint8_t)(h1[i1 - 1] - '1') < 3 && (uint8_t)(h2[i2 - 1] - '1') < 3) { --i1; --i2; }
+    if (i1 != i2) return false;
+    for (int j = 0; j < i1; ++j)
+        if (h1[j] != h2[j]) return false;
+    return true;
+}
+
 // Filter outputs (cg_fastq_collect_split): where a read or pair goes once fq_finish_core named the filter that fired
 // (-1: none).  0 the main output, 1 --too-short-output, 2 --too-long-output, 3 --untrimmed-output, -1 dropped.  A
 // filter with an output writes what it removes (SingleEndFilter / PairedEndFilter with a writer, steps.py:70-180),

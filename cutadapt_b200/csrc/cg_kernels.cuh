@@ -175,6 +175,21 @@ cudaError_t cg_launch_fastq_info(int phase, const uint8_t *d_buf, const CgFastqR
                                  uint8_t *d_out, cudaStream_t st, int kind = 0, const int32_t *d_qtrim = nullptr,
                                  const int32_t *d_seq_len = nullptr,    // kind 1 / 2: --rest-file / --wildcard-file rows
                                  int has_qual = 1);                     // 0: FASTA input, empty quality columns
+// interleaved input: phase 0 = per record of the chunk its span (d_start, d_size), mate (d_dest = r & 1) and name
+// (d_rec; FASTQ: from the line index d_nl_pos, format checked; FASTA, d_nl_pos == nullptr: d_rec is the normalised
+// chunk's record table), then the mate-name check per pair; d_err: first problem, record << 32 | code.  After the
+// demultiplexer's partition of d_size by d_dest (d_off), phase 1 copies every record into d_out1 / d_out2 (mate 2's
+// offsets start at seg1; fasta: a '\n' is appended to every record).
+cudaError_t cg_launch_interleaved_split(int phase, const uint8_t *d_buf, long long n_bytes, const uint32_t *d_nl_pos,
+                                        long long n_newlines, long long n_records, CgFastqRecord *d_rec, int32_t *d_start,
+                                        int32_t *d_size, int32_t *d_dest, unsigned long long *d_err, const int64_t *d_off,
+                                        long long seg1, uint8_t *d_out1, uint8_t *d_out2, int fasta, cudaStream_t st);
+// interleaved outputs (bit d of ilv: destination d of d_route): phase 0 folds the sizes of such pairs into mate 1
+// (d_fold1 / d_fold2, what the partition runs on); phase 1, after the partitions, gives mate 2 of such a pair the offset
+// off1 + len1 and moves every other record of mate 2 behind mate 1's region (*d_total1 bytes)
+cudaError_t cg_launch_fastq_interleave(int phase, long long n_records, const int32_t *d_route, int ilv,
+                                       const int32_t *d_len1, const int32_t *d_len2, int32_t *d_fold1, int32_t *d_fold2,
+                                       const int64_t *d_off1, int64_t *d_off2, const int64_t *d_total1, cudaStream_t st);
 // --pair-adapters: fold the records of adapter pair `pair` into the best pair per read (modifiers.py:480-503)
 cudaError_t cg_launch_fastq_pair_select(long long n_records, int pair, const cg_match_rec *d_cur1, int slots1,
                                         const cg_match_rec *d_cur2, int slots2, cg_match_rec *d_best1, cg_match_rec *d_best2,

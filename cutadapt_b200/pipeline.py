@@ -652,12 +652,13 @@ class BatchTrimmer:
         return [stats[id(o)] for o in owners]
 
 
-def _fastq_head(buf, end: int) -> int:
+def _fastq_head(buf, end: int, lines: int = 4) -> int:
     """Length of the longest prefix of buf[:end] that consists of complete 4-line records (the buffer starts at a
-    record; same counting rule as dnaio's chunk reader, which the reference uses at runners.py:116-126)."""
+    record; same counting rule as dnaio's chunk reader, which the reference uses at runners.py:116-126).  lines=8:
+    complete pairs of interleaved records."""
     linebreaks = buf.count(b"\n", 0, end)
     right = end
-    for _ in range(linebreaks % 4 + 1):
+    for _ in range(linebreaks % lines + 1):
         right = buf.rfind(b"\n", 0, right)
         if right < 0:
             return 0
@@ -678,6 +679,12 @@ def read_fastq_chunks(f, buffer_size: int = 4 * 1024 * 1024):
     workers (runners.py:116-126) and what ``FastqTrimmer.process_chunk(s)`` takes.  The last chunk may lack the
     final newline.  A record larger than the buffer makes the buffer grow.
     """
+    return _read_chunks(f, buffer_size, _fastq_head)
+
+
+def _read_chunks(f, buffer_size: int, head_of):
+    """Chunks of buf[:head_of(buf, end)] from a binary file object; the buffer grows when it holds no complete chunk,
+    whatever is left at the end of the file is the last chunk."""
     buf = bytearray(buffer_size)
     start = 0
     while True:
@@ -687,7 +694,7 @@ def read_fastq_chunks(f, buffer_size: int = 4 * 1024 * 1024):
         if not n:
             break
         end = start + n
-        head = _fastq_head(buf, end)
+        head = head_of(buf, end)
         if head:
             yield bytes(buf[:head])
             buf[0:end - head] = buf[head:end]
@@ -696,6 +703,16 @@ def read_fastq_chunks(f, buffer_size: int = 4 * 1024 * 1024):
             start = end
     if start:
         yield bytes(buf[:start])
+
+
+def read_interleaved_fastq_chunks(f, buffer_size: int = 4 * 1024 * 1024):
+    """
+    Chunks of whole pairs of an interleaved FASTQ file (R1 and R2 of each pair one after the other, ``--interleaved``):
+    every chunk ends after a multiple of 8 lines, for ``PairedFastqTrimmer``'s chunk methods with ``chunk2=None``.  A
+    record larger than the buffer makes the buffer grow.  An odd number of records at the end of the file stays in the
+    last chunk, which the device then rejects ("Interleaved input file incomplete").
+    """
+    return _read_chunks(f, buffer_size, lambda buf, end: _fastq_head(buf, end, 8))
 
 
 def read_paired_fastq_chunks(f1, f2, buffer_size: int = 4 * 1024 * 1024):
@@ -753,24 +770,19 @@ def read_fasta_chunks(f, buffer_size: int = 4 * 1024 * 1024):
     ends in front of a line that starts with '>'; the first chunk carries any '#' lines in front of the first record.
     A record larger than the buffer makes the buffer grow.
     """
-    buf = bytearray(buffer_size)
-    start = 0
-    while True:
-        if start == len(buf):
-            buf.extend(bytes(len(buf)))
-        n = f.readinto(memoryview(buf)[start:])
-        if not n:
-            break
-        end = start + n
-        head = _fasta_head(buf, end)
-        if head:
-            yield bytes(buf[:head])
-            buf[0:end - head] = buf[head:end]
-            start = end - head
-        else:
-            start = end
-    if start:
-        yield bytes(buf[:start])
+    return _read_chunks(f, buffer_size, _fasta_head)
+
+
+def _fasta_pairs_head(buf, end: int) -> int:
+    """The longest prefix of complete FASTA records that holds an even number of them (0 without a complete pair)."""
+    records = _fasta_headers(buf, _fasta_head(buf, end))
+    return _fasta_cut(buf, end, records - records % 2) if records >= 2 else 0
+
+
+def read_interleaved_fasta_chunks(f, buffer_size: int = 4 * 1024 * 1024):
+    """Chunks of whole pairs of an interleaved FASTA file: every chunk ends in front of every second header (see
+    read_interleaved_fastq_chunks)."""
+    return _read_chunks(f, buffer_size, _fasta_pairs_head)
 
 
 def read_paired_fasta_chunks(f1, f2, buffer_size: int = 4 * 1024 * 1024):
@@ -859,6 +871,11 @@ def _fastq_params(times=1, quality_cutoff=None, quality_base=33, nextseq_cutoff=
 
 
 REDIRECT_OUTPUTS = ("too_short", "too_long", "untrimmed")     # destinations 1, 2, 3 of cg_fastq_collect_split
+
+
+# the outputs cg_fastq_collect_paired_interleaved can interleave, and their bits
+INTERLEAVE_BITS = {"output": _lib.CG_INTERLEAVE_MAIN, "too_short": _lib.CG_REDIRECT_TOO_SHORT,
+                   "too_long": _lib.CG_REDIRECT_TOO_LONG, "untrimmed": _lib.CG_REDIRECT_UNTRIMMED}
 
 
 def _redirect_bits(redirect, redirect_formats, params) -> Tuple[int, int]:
@@ -1207,6 +1224,14 @@ class PairedFastqTrimmer:
     the filter's two outputs (--too-short-output / --too-short-paired-output, ...); with adapters on one mate only, a
     pair is untrimmed when both mates are (cli.py:859-893).  ``process_chunk_split(chunk1, chunk2) -> {name: (bytes1,
     bytes2)}`` and ``process_chunks_split(iterable of pairs)``.
+
+    Interleaved data (``--interleaved``): every chunk method takes ``chunk2=None`` to mean that ``chunk1`` holds R1 and
+    R2 of each pair one after the other (read_interleaved_fastq_chunks / read_interleaved_fasta_chunks); the device
+    splits it (``cg_fastq_submit_interleaved``) and rejects an odd record count or mates whose names do not match.
+    ``process_chunks_split`` takes single chunks in place of pairs.  ``interleaved_outputs``: names out of
+    ``("output",) + REDIRECT_OUTPUTS`` whose output is written interleaved, R1 then R2 of each pair, returned as
+    ``(bytes, b"")`` (the reference interleaves an output whose paired path is missing).  Not with ``pair_adapters``
+    or demultiplexing.
     """
 
     MODES = {"any": 0, "both": 1, "first": 2}
@@ -1215,7 +1240,8 @@ class PairedFastqTrimmer:
                  options2: Optional[dict] = None, pair_filter: str = "any", pair_adapters: bool = False,
                  input_format: str = "fastq", output_format: Optional[str] = None,
                  ctx: Optional[_lib.Context] = None, collect_statistics: bool = False,
-                 redirect: Sequence[str] = (), redirect_formats: Optional[dict] = None):
+                 redirect: Sequence[str] = (), redirect_formats: Optional[dict] = None,
+                 interleaved_outputs: Sequence[str] = ()):
         if pair_filter not in self.MODES:
             raise ValueError("pair_filter must be 'any', 'both' or 'first'")
         formats = dict(input_format=input_format, output_format=output_format)
@@ -1226,6 +1252,14 @@ class PairedFastqTrimmer:
         _redirect_bits(self.redirect, redirect_formats, self.params2)
         if self._redirect and pair_adapters:
             raise ValueError("filter outputs cannot be combined with --pair-adapters")
+        self.interleaved_outputs = tuple(dict.fromkeys(interleaved_outputs or ()))
+        self._interleave = 0
+        for name in self.interleaved_outputs:
+            if name not in INTERLEAVE_BITS:
+                raise ValueError(f"unknown output {name!r} to interleave (one of {', '.join(INTERLEAVE_BITS)})")
+            self._interleave |= INTERLEAVE_BITS[name]
+        if self._interleave and pair_adapters:
+            raise ValueError("interleaved outputs cannot be combined with --pair-adapters")
         self.ctx = ctx or _lib.default_context()
         self.mode = self.MODES[pair_filter]
         self.statistics = ({}, {})
@@ -1301,6 +1335,26 @@ class PairedFastqTrimmer:
                                               C.byref(slot)))
         return slot.value, buf
 
+    def _submit_pair(self, chunk1, chunk2):
+        """((slot1, chunk), (slot2, chunk)): two chunks, or one interleaved chunk (chunk2 None) split on the device."""
+        if chunk2 is not None:
+            return self._submit(chunk1), self._submit(chunk2)
+        buf = np.frombuffer(chunk1, dtype=np.uint8) if not isinstance(chunk1, np.ndarray) else chunk1
+        s1, s2 = C.c_int32(-1), C.c_int32(-1)
+        _lib.check(_lib.lib().cg_fastq_submit_interleaved(self.ctx.handle, buf.ctypes.data if buf.size else None,
+                                                          buf.size, self.params1.format, C.byref(s1), C.byref(s2)))
+        return (s1.value, buf), (s2.value, buf)
+
+    def _out_buffers(self, tickets):
+        """Output buffers of a pair: out1 also holds R2 of the interleaved outputs."""
+        (_, b1), (_, b2) = tickets
+        n1, n2 = _output_capacity(b1.size, self.params1.format), _output_capacity(b2.size, self.params2.format)
+        return np.empty(n1 + (n2 if self._interleave else 0), dtype=np.uint8), np.empty(n2, dtype=np.uint8)
+
+    def _no_interleave(self, what: str):
+        if self._interleave:
+            raise ValueError(f"interleaved outputs ({', '.join(self.interleaved_outputs)}) cannot be combined with {what}")
+
     def _account(self, r1, r2):
         for st, res in zip(self.statistics, (r1, r2)):
             for k, v in res.as_dict().items():
@@ -1313,42 +1367,54 @@ class PairedFastqTrimmer:
 
     def _collect_split(self, tickets) -> dict:
         (s1, b1), (s2, b2) = tickets
-        out1 = np.empty(_output_capacity(b1.size, self.params1.format), dtype=np.uint8)
-        out2 = np.empty(_output_capacity(b2.size, self.params2.format), dtype=np.uint8)
+        out1, out2 = self._out_buffers(tickets)
         r1, r2 = _lib.cg_fastq_result(), _lib.cg_fastq_result()
         seg1, seg2 = np.zeros(5, dtype=np.int64), np.zeros(5, dtype=np.int64)
-        _lib.check(_lib.lib().cg_fastq_collect_paired_split(
-            self.ctx.handle, s1, s2, self._set1.handle if self._set1 is not None else None,
-            self._set2.handle if self._set2 is not None else None, C.byref(self.params1), C.byref(self.params2),
-            self.mode, self._redirect, self._fasta_outputs, out1.ctypes.data, out1.size, out2.ctypes.data, out2.size,
-            C.byref(r1), C.byref(r2), seg1.ctypes.data, seg2.ctypes.data))
+        sets = (self._set1.handle if self._set1 is not None else None,
+                self._set2.handle if self._set2 is not None else None)
+        if self._interleave:
+            _lib.check(_lib.lib().cg_fastq_collect_paired_interleaved(
+                self.ctx.handle, s1, s2, *sets, C.byref(self.params1), C.byref(self.params2), self.mode,
+                self._redirect, self._fasta_outputs, self._interleave, out1.ctypes.data, out1.size, out2.ctypes.data,
+                out2.size, C.byref(r1), C.byref(r2), seg1.ctypes.data, seg2.ctypes.data))
+        else:
+            _lib.check(_lib.lib().cg_fastq_collect_paired_split(
+                self.ctx.handle, s1, s2, *sets, C.byref(self.params1), C.byref(self.params2), self.mode,
+                self._redirect, self._fasta_outputs, out1.ctypes.data, out1.size, out2.ctypes.data, out2.size,
+                C.byref(r1), C.byref(r2), seg1.ctypes.data, seg2.ctypes.data))
         self._account(r1, r2)
         names = ("output",) + REDIRECT_OUTPUTS
         return {name: (out1[seg1[d]:seg1[d + 1]].tobytes(), out2[seg2[d]:seg2[d + 1]].tobytes())
                 for d, name in enumerate(names) if d == 0 or name in self.redirect}
 
-    def process_chunk_split(self, chunk1, chunk2) -> dict:
+    def process_chunk_split(self, chunk1, chunk2=None) -> dict:
         """{"output": (R1, R2) of the main outputs, and for every name in ``redirect``: (R1, R2) of the pairs that filter
-        removed} for one pair of chunks (``cg_fastq_collect_paired_split``)."""
-        return self._collect_split((self._submit(chunk1), self._submit(chunk2)))
+        removed} for one pair of chunks, or one interleaved chunk (chunk2 None); an interleaved output is (R1 and R2,
+        b"") (``cg_fastq_collect_paired_split`` / ``cg_fastq_collect_paired_interleaved``)."""
+        return self._collect_split(self._submit_pair(chunk1, chunk2))
 
     def process_chunks_split(self, pairs):
-        """process_chunk_split over an iterable of (chunk1, chunk2) with one pair in flight: the upload of pair i+1
-        overlaps the work on pair i."""
+        """process_chunk_split over an iterable of (chunk1, chunk2), or of interleaved chunks, with one pair in flight:
+        the upload of pair i+1 overlaps the work on pair i."""
         pending = None
-        for chunk1, chunk2 in pairs:
-            tickets = (self._submit(chunk1), self._submit(chunk2))
+        for item in pairs:
+            chunk1, chunk2 = item if isinstance(item, (tuple, list)) else (item, None)
+            tickets = self._submit_pair(chunk1, chunk2)
             if pending is not None:
                 yield self._collect_split(pending)
             pending = tickets
         if pending is not None:
             yield self._collect_split(pending)
 
-    def process_chunk(self, chunk1, chunk2) -> Tuple[bytes, bytes]:
+    def process_chunk(self, chunk1, chunk2=None) -> Tuple[bytes, bytes]:
+        """(R1, R2) of one pair of chunks or of one interleaved chunk (chunk2 None); with "output" in
+        ``interleaved_outputs``: (R1 and R2 interleaved, b"")."""
         self._no_redirect("process_chunk")
-        (s1, b1), (s2, b2) = self._submit(chunk1), self._submit(chunk2)
-        out1 = np.empty(_output_capacity(b1.size, self.params1.format), dtype=np.uint8)
-        out2 = np.empty(_output_capacity(b2.size, self.params2.format), dtype=np.uint8)
+        if self._interleave:
+            return self._collect_split(self._submit_pair(chunk1, chunk2))["output"]
+        tickets = self._submit_pair(chunk1, chunk2)
+        (s1, b1), (s2, b2) = tickets
+        out1, out2 = self._out_buffers(tickets)
         r1, r2 = _lib.cg_fastq_result(), _lib.cg_fastq_result()
         if self._pairs is not None:
             _lib.check(_lib.lib().cg_fastq_collect_pair_adapters(
@@ -1363,7 +1429,7 @@ class PairedFastqTrimmer:
         self._account(r1, r2)
         return out1[: r1.out_bytes].tobytes(), out2[: r2.out_bytes].tobytes()
 
-    def process_chunk_demux(self, chunk1, chunk2, combinatorial: bool = False, discard_untrimmed: bool = False,
+    def process_chunk_demux(self, chunk1, chunk2=None, combinatorial: bool = False, discard_untrimmed: bool = False,
                             unknown: str = "unknown") -> dict:
         """
         Demultiplexed pairs of one chunk on the device (``cg_fastq_collect_paired_demux``).
@@ -1372,11 +1438,12 @@ class PairedFastqTrimmer:
         ``unknown``: (R1 bytes, R2 bytes)}; with ``discard_untrimmed`` the ``unknown`` output is not produced.
         combinatorial=True: ``CombinatorialDemultiplexer`` (steps.py:506-581) -- keys are (name1, name2) with None for a
         mate without a match; with ``discard_untrimmed`` only pairs with matches on both mates are kept.  Pairs
-        without an output are dropped without being counted, as in the reference.
+        without an output are dropped without being counted, as in the reference.  chunk2 None: chunk1 is interleaved.
         """
         if self._pairs is not None:
             raise ValueError("demultiplexing with --pair-adapters is not supported")
         self._no_redirect("demultiplexing")
+        self._no_interleave("demultiplexing")
         names1, dest1 = _demux_names(self.adapters1)
         n1 = len(names1)
         if combinatorial:
@@ -1388,9 +1455,9 @@ class PairedFastqTrimmer:
             dest2, n2 = None, 0
             keys = names1 + [unknown]
             keep = np.array([1] * n1 + [0 if discard_untrimmed else 1], dtype=np.uint8)
-        (s1, b1), (s2, b2) = self._submit(chunk1), self._submit(chunk2)
-        out1 = np.empty(_output_capacity(b1.size, self.params1.format), dtype=np.uint8)
-        out2 = np.empty(_output_capacity(b2.size, self.params2.format), dtype=np.uint8)
+        tickets = self._submit_pair(chunk1, chunk2)
+        (s1, b1), (s2, b2) = tickets
+        out1, out2 = self._out_buffers(tickets)
         r1, r2 = _lib.cg_fastq_result(), _lib.cg_fastq_result()
         seg1 = np.zeros(len(keys) + 1, dtype=np.int64)
         seg2 = np.zeros(len(keys) + 1, dtype=np.int64)

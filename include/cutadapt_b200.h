@@ -472,6 +472,40 @@ int cg_fastq_collect_paired_split(cg_ctx *ctx, int32_t slot1, int32_t slot2, con
                                   int64_t out_capacity1, uint8_t *out2, int64_t out_capacity2, cg_fastq_result *res1,
                                   cg_fastq_result *res2, int64_t *segments1, int64_t *segments2);
 
+/* Interleaved paired-end input (--interleaved with one input; what `fastq-dump --split-spot` writes): R1 and R2 of each
+ * pair follow each other in one chunk.  The chunk is uploaded once and split on the device into two slots that look
+ * exactly like two submitted mate chunks: record 2p of the chunk is record p of mate 1 (*slot1), record 2p + 1 record p
+ * of mate 2 (*slot2).  Every paired collect (cg_fastq_collect_paired, _paired_split, _paired_demux, _pair_adapters,
+ * _paired_interleaved) then takes (*slot1, *slot2) in that order; any other use of these slots is CG_EINVAL.  format is
+ * the input format as cg_fastq_params.format gives it: CG_FORMAT_FASTQ or CG_FORMAT_FASTQ_TO_FASTA for FASTQ,
+ * CG_FORMAT_FASTA for FASTA (a chunk of whole records); the collect's params must have the same input format.  The split runs when the pair is
+ * collected; these are then CG_EINVAL, the message naming what was found:
+ *   - an odd number of records (the last one has no mate: "Interleaved input file incomplete");
+ *   - mate names that do not match ("Reads are improperly paired"; the rule of dnaio's readers, doc/reference.rst:
+ *     925-950: the IDs up to the first space or tab, a final 1, 2 or 3 of both ignored), naming the first such pair by
+ *     its record numbers in the chunk;
+ *   - a FASTQ format error, naming the record number in the chunk (2p or 2p + 1); FASTA format errors name the line of
+ *     the chunk.
+ * The split takes two of the four slots, like a two-file pair, so one pair can stay in flight while the next uploads. */
+int cg_fastq_submit_interleaved(cg_ctx *ctx, const uint8_t *chunk, int64_t n_bytes, int32_t format, int32_t *slot1,
+                                int32_t *slot2);
+
+/* Interleaved outputs: cg_fastq_collect_paired_split plus interleaved_outputs, the destinations written interleaved
+ * (CG_INTERLEAVE_MAIN for the main output, the CG_REDIRECT_* bits for the too-short, too-long and untrimmed outputs; the
+ * reference interleaves each output whose paired path is missing, cli.py:650-661, 913-921).  An interleaved destination
+ * d holds both mates in out1's segment d, R1 then R2 of each pair in input order, and out2's segment d is empty.
+ * interleaved_outputs == 0 gives what cg_fastq_collect_paired_split gives, byte for byte.  The bound and the "buffer too
+ * small -> out_bytes" contract hold per buffer (out1 must hold both mates of every interleaved destination; out_bytes of
+ * res1 counts them); fasta_outputs applies per destination.  Counters, n_written, bp_out and the statistics vectors are
+ * those of the two-file call.  Works on two submitted mate chunks and on an interleaved submission alike. */
+#define CG_INTERLEAVE_MAIN 8
+int cg_fastq_collect_paired_interleaved(cg_ctx *ctx, int32_t slot1, int32_t slot2, const cg_adapterset *set1,
+                                        const cg_adapterset *set2, const cg_fastq_params *params1,
+                                        const cg_fastq_params *params2, int32_t pair_filter_mode, int32_t redirect,
+                                        int32_t fasta_outputs, int32_t interleaved_outputs, uint8_t *out1,
+                                        int64_t out_capacity1, uint8_t *out2, int64_t out_capacity2, cg_fastq_result *res1,
+                                        cg_fastq_result *res2, int64_t *segments1, int64_t *segments2);
+
 /* ---- trim statistics (the payload of the end-of-run all-reduce, report.py:81-126) --------
  * Device-side reduction of a batch's match records into a fixed-layout int64 vector that carries everything the
  * reference's Statistics.__iadd__ adds up (report.py:81-126), so that one all-reduce merges the ranks:

@@ -1,7 +1,7 @@
 """End-to-end throughput of the FASTQ entry point (not a bench line; see DESIGN.md sections 4.6, 4.7).
 
-  python tools/measure_fastq.py [n_reads] [chunk_megabytes] [fastq | fasta | fasta60 | barcodes] [--statistics]
-                                [--redirect]
+  python tools/measure_fastq.py [n_reads] [chunk_megabytes] [fastq | fasta | fasta60 | barcodes | paired | interleaved]
+                                [--statistics] [--redirect]
 
 Builds n_reads synthetic FASTQ records of BASELINE configs[1]'s shape (150 bp, Phred+33 qualities, names
 "@SIM2:000000123") in pinned host memory, cuts the buffer into chunks of whole records and streams them
@@ -13,6 +13,10 @@ the 96 anchored 5' barcodes of config 5 (-g ^BARCODE..., IndexedPrefixAdapters) 
 --statistics: the trimmer also collects the report's statistics (collect_statistics=True; cg_fastq_stats_*).
 --redirect: the filters keep what they remove (--too-short-output --untrimmed-output: process_chunks_split,
 cg_fastq_collect_split); the output bytes are those of all three outputs.
+"paired" / "interleaved": the same n_reads records as n_reads / 2 pairs (-a / -A AGATCGGAAGAGC -q 20 -m 20 on both
+mates; the mates of a pair share their name): "paired" streams them as two mate chunks per step
+(PairedFastqTrimmer.process_chunks_split, two uploads, two outputs), "interleaved" as one interleaved chunk in and out
+(cg_fastq_submit_interleaved, interleaved_outputs=("output",)); each step holds the same pairs, chunk_megabytes in all.
 """
 import json
 import sys
@@ -23,18 +27,19 @@ import torch
 
 sys.path.insert(0, __file__.rsplit("/", 2)[0])
 import cutadapt_b200.adapters as PA  # noqa: E402
-from cutadapt_b200.pipeline import FastqTrimmer  # noqa: E402
+from cutadapt_b200.pipeline import FastqTrimmer, PairedFastqTrimmer  # noqa: E402
 from cutadapt_b200.synth import make_read_tensor  # noqa: E402
 
 
-def build_fastq(n, pinned=True):
+def build_fastq(n, pinned=True, pair_names=False):
+    """n records; pair_names: records 2p and 2p + 1 are named after pair p (the two mates of an interleaved file)."""
     seq, qual = make_read_tensor(n, config=2, device="cuda", with_qualities=True)
     name_len = 6 + 9
     rec_len = 1 + name_len + 1 + 150 + 3 + 150 + 1
     rec = torch.empty((n, rec_len), dtype=torch.uint8, device="cuda")
     rec[:, 0] = ord("@")
     rec[:, 1:6] = torch.tensor(list(b"SIM2:"), dtype=torch.uint8, device="cuda")
-    idx = torch.arange(n, device="cuda")
+    idx = torch.arange(n, device="cuda") // (2 if pair_names else 1)
     for d in range(10):
         rec[:, 6 + 9 - d] = (48 + (idx // 10 ** d) % 10).to(torch.uint8)
     o = 1 + name_len
@@ -84,15 +89,31 @@ def main():
     n = int(argv[1]) if len(argv) > 1 else 4_000_000
     chunk_mb = int(argv[2]) if len(argv) > 2 else 64
     variant = argv[3] if len(argv) > 3 else "fastq"
-    if variant in ("fastq", "barcodes"):
+    if variant in ("paired", "interleaved"):
+        n -= n % 2
+        data, rec_len = build_fastq(n, pair_names=True)
+    elif variant in ("fastq", "barcodes"):
         data, rec_len = build_fastq(n)
     else:
         data, rec_len = build_fasta(n, wrap=60 if variant == "fasta60" else None)
     per_chunk = max(1, (chunk_mb << 20) // rec_len)
+    if variant in ("paired", "interleaved"):
+        per_chunk = max(2, per_chunk // 2 * 2)         # whole pairs
     chunks = [data[i * rec_len:min(n, i + per_chunk) * rec_len] for i in range(0, n, per_chunk)]
     adapters = [PA.BackAdapter("AGATCGGAAGAGC", max_errors=0.1)]
     split = dict(redirect=redirect) if redirect else {}
-    if variant == "fastq":
+    if variant in ("paired", "interleaved"):
+        opts = dict(quality_cutoff=(0, 20), minimum_length=20)
+        t = PairedFastqTrimmer(adapters, adapters, opts, opts, collect_statistics=collect, **split,
+                               interleaved_outputs=("output",) if variant == "interleaved" else ())
+        what = (f"paired FASTQ ({variant}) bytes in -> trimmed bytes out (-a/-A AGATCGGAAGAGC -q 20 -m 20), host to host")
+        if variant == "paired":
+            # the mates as two files: the same pairs, two chunks of chunk_megabytes per step
+            mates = [np.ascontiguousarray(data.reshape(n // 2, 2, rec_len)[:, k]).reshape(-1) for k in (0, 1)]
+            mates = [torch.from_numpy(m).pin_memory().numpy() for m in mates]
+            half = per_chunk // 2                           # the pairs of one interleaved chunk
+            chunks = [tuple(m[i * rec_len:min(n // 2, i + half) * rec_len] for m in mates) for i in range(0, n // 2, half)]
+    elif variant == "fastq":
         t = FastqTrimmer(adapters, quality_cutoff=(0, 20), minimum_length=20, collect_statistics=collect, **split)
         what = "FASTQ bytes in -> trimmed FASTQ bytes out (-a AGATCGGAAGAGC -q 20 -m 20), host to host"
     elif variant == "barcodes":
@@ -108,24 +129,29 @@ def main():
         what = f"FASTA ({variant}) bytes in -> trimmed FASTA bytes out (-a AGATCGGAAGAGC -m 20), host to host"
     if redirect:
         what += ", --too-short-output --untrimmed-output"
-
+    if variant in ("paired", "interleaved"):
+        def run(cs):
+            return sum(len(a) + len(b) for parts in t.process_chunks_split(cs) for a, b in parts.values())
+    elif redirect:
         def run(cs):
             return sum(len(o) for parts in t.process_chunks_split(cs, copy=False) for o in parts.values())
     else:
         def run(cs):
             return sum(len(o) for o in t.process_chunks(cs, copy=False))
     run(chunks[:9])                    # warm-up: every slot's buffers, pool
-    t.statistics.clear()
+    for st in (t.statistics if isinstance(t.statistics, tuple) else (t.statistics,)):
+        st.clear()
     t0 = time.perf_counter()
     out_bytes = run(chunks)
     wall = time.perf_counter() - t0
-    st = t.statistics
+    st = t.statistics[0] if isinstance(t.statistics, tuple) else t.statistics
     print(json.dumps({
         "what": what,
-        "reads": n, "chunk_mb": chunk_mb, "collect_statistics": collect, "redirect": list(redirect), "chunks": len(chunks),
+        "variant": variant, "reads": n, "chunk_mb": chunk_mb, "collect_statistics": collect, "redirect": list(redirect), "chunks": len(chunks),
         "reads_per_s": n / wall,
         "in_GB_per_s": data.size / wall / 1e9, "out_GB_per_s": out_bytes / wall / 1e9,
-        "in_bytes": int(data.size), "out_bytes": out_bytes, "wall_s": wall,
+        "in_bytes": int(data.size),
+        "gpu": torch.cuda.get_device_name(), "out_bytes": out_bytes, "wall_s": wall,
         "statistics": {k: int(v) for k, v in st.items()},
     }))
 

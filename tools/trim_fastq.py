@@ -11,6 +11,7 @@ on real files.
   python tools/trim_fastq.py -a AGATCGGAAGAGC -m 20 -o out.fasta in.fasta           (FASTA; also FASTQ -> FASTA)
   python tools/trim_fastq.py -a AGATCGGAAGAGC -m 20 --too-short-output short.fastq --untrimmed-output untrimmed.fasta \
       -o out.fastq in.fastq                                                            (filter outputs)
+  python tools/trim_fastq.py --interleaved -a ADAPT1 -A ADAPT2 -m 20:25 -o out.fastq in.interleaved.fastq
 
 The input format comes from the first byte of the (first) input, as cutadapt's files.detect_file_format does: '>' or
 '#' is FASTA, anything else (an empty file included) FASTQ.  The output is FASTA when the input is, when -o ends in
@@ -18,6 +19,10 @@ The input format comes from the first byte of the (first) input, as cutadapt's f
 paired forms) gets its format from its own name the same way.  --json FILE also writes what the report shows per adapter (removed length x errors,
 bases preceding the adapter, reverse-complemented count), the poly-A and written-length histograms and the counters,
 collected on the device (collect_statistics=True); the stderr line stays as it is.
+
+--interleaved, as in the reference: one input is interleaved input (R1 and R2 of each pair one after the other, split
+on the device), no -p means an interleaved main output, and a filter output without its --*-paired-output is written
+interleaved.  -m / -M take LEN[:LEN2], a length for each mate; an empty side means no filter on that mate.
 """
 import argparse
 import json
@@ -26,7 +31,8 @@ import sys
 sys.path.insert(0, __file__.rsplit("/", 2)[0])
 import cutadapt_b200.adapters as PA  # noqa: E402
 from cutadapt_b200.pipeline import (FastqTrimmer, PairedFastqTrimmer, read_fasta_chunks,  # noqa: E402
-                                    read_fastq_chunks, read_paired_fasta_chunks, read_paired_fastq_chunks)
+                                    read_fastq_chunks, read_interleaved_fasta_chunks, read_interleaved_fastq_chunks,
+                                    read_paired_fasta_chunks, read_paired_fastq_chunks)
 
 
 def detect_format(path):
@@ -68,15 +74,43 @@ def report_json(counters, adapter_statistics, poly_a, written):
             "written_lengths": {str(k): v for k, v in sorted(written.items())}}
 
 
+def parse_lengths(s):
+    """-m / -M: LEN or LEN1:LEN2 with one side possibly empty (cli.py:443-465, parse_lengths) -> tuple of int / None.
+    ValueError names what is wrong."""
+    fields = s.split(":")
+    if len(fields) not in (1, 2):
+        raise ValueError("Only at most one colon is allowed")
+    try:
+        values = tuple(int(f) if f != "" else None for f in fields)
+    except ValueError as e:
+        raise ValueError(f"Value not recognized: {e}")
+    if len(values) == 2 and values[0] is None and values[1] is None:
+        raise ValueError(f"Cannot parse '{s}': At least one length needs to be given")
+    return values
+
+
+def mate_lengths(ap, value, paired):
+    """(length of R1, length of R2) of a -m / -M value (None: no filter on that mate)."""
+    if value is None:
+        return None, None
+    try:
+        lengths = parse_lengths(value)
+    except ValueError as e:
+        ap.error(str(e))
+    if not paired and len(lengths) == 2:
+        ap.error("Two minimum or maximum lengths given for single-end data")
+    return (lengths[0], lengths[0]) if len(lengths) == 1 else lengths
+
+
 FILTER_OUTPUTS = (("too_short", "too-short"), ("too_long", "too-long"), ("untrimmed", "untrimmed"))
 
 
-def check_filter_outputs(ap, args, paired, demultiplex):
+def check_filter_outputs(ap, args, paired, demultiplex, interleaved=False):
     """The command-line errors of the reference around the filter outputs (cli.py:588-592, 600-622, 713-733, 798-808):
     ap.error() exits with status 2."""
     if not paired and args.untrimmed_paired_output:
         ap.error("Option --untrimmed-paired-output can only be used when trimming paired-end reads.")
-    if paired:
+    if paired and not interleaved:
         for dest, name in FILTER_OUTPUTS:
             if bool(getattr(args, dest + "_output")) != bool(getattr(args, dest + "_paired_output")):
                 ap.error("When trimming paired-end data, you must use either none or both of the"
@@ -112,8 +146,10 @@ def main():
     ap.add_argument("--quality-base", type=int, default=33)
     ap.add_argument("--nextseq-trim", type=int, default=None)
     ap.add_argument("-u", "--cut", type=int, action="append", default=[])
-    ap.add_argument("-m", "--minimum-length", type=int, default=None)
-    ap.add_argument("-M", "--maximum-length", type=int, default=None)
+    ap.add_argument("-m", "--minimum-length", default=None, metavar="LEN[:LEN2]")
+    ap.add_argument("-M", "--maximum-length", default=None, metavar="LEN[:LEN2]")
+    ap.add_argument("--interleaved", action="store_true",
+                    help="read and/or write interleaved paired-end reads (one input file, or no -p)")
     ap.add_argument("--max-n", type=float, default=None)
     ap.add_argument("--max-ee", type=float, default=None)
     ap.add_argument("--length", "-l", type=int, default=None)
@@ -136,7 +172,15 @@ def main():
                         help=f"the second mates of the pairs --{name}-output gets")
     ap.add_argument("inputs", nargs="+")
     args = ap.parse_args()
-    check_filter_outputs(ap, args, len(args.inputs) == 2, "{name}" in args.output)
+    if args.interleaved and len(args.inputs) == 2 and args.paired_output:
+        ap.error("--interleaved was given with two input files and two output files (-o and -p): use it for interleaved "
+                 "input (one input file) or interleaved output (no -p)")
+    if len(args.inputs) > 2:
+        ap.error("at most two input files")
+    paired = len(args.inputs) == 2 or args.interleaved
+    min1, min2 = mate_lengths(ap, args.minimum_length, paired)
+    max1, max2 = mate_lengths(ap, args.maximum_length, paired)
+    check_filter_outputs(ap, args, paired, "{name}" in args.output, args.interleaved)
     input_format = detect_format(args.inputs[0])
     fasta_out = input_format == "fasta" or args.fasta or args.output.endswith((".fasta", ".fa"))
     output_format = "fasta" if fasta_out and input_format == "fastq" else None
@@ -151,7 +195,7 @@ def main():
         parts = [int(x) for x in args.quality_cutoff.split(",")]
         qc = (0, parts[0]) if len(parts) == 1 else (parts[0], parts[1])
     common = dict(times=args.times, quality_cutoff=qc, quality_base=args.quality_base, nextseq_cutoff=args.nextseq_trim,
-                  minimum_length=args.minimum_length, maximum_length=args.maximum_length, max_n=args.max_n,
+                  minimum_length=min1, maximum_length=max1, max_n=args.max_n,
                   max_expected_errors=args.max_ee, discard_trimmed=args.discard_trimmed,
                   discard_untrimmed=args.discard_untrimmed, cut=args.cut, poly_a=args.poly_a, length=args.length,
                   trim_n=args.trim_n, discard_casava=args.discard_casava, action=args.action)
@@ -168,30 +212,38 @@ def main():
             + make_adapters(args.front2, "front", args.error_rate, args.overlap)
             + make_adapters(args.anywhere2, "anywhere", args.error_rate, args.overlap))
 
-    if len(args.inputs) == 2:
-        if not args.paired_output:
-            ap.error("paired-end input needs -p")
-        if detect_format(args.inputs[1]) != input_format:
+    if paired:
+        if not args.paired_output and not args.interleaved:
+            ap.error("paired-end input needs -p (or --interleaved for an interleaved output)")
+        if len(args.inputs) == 2 and detect_format(args.inputs[1]) != input_format:
             ap.error("both inputs must have the same format")
-        t = PairedFastqTrimmer(ads1, ads2, common, common, args.pair_filter, **formats, **split)
-        with open(args.inputs[0], "rb") as f1, open(args.inputs[1], "rb") as f2, \
-                open(args.output, "wb") as o1, open(args.paired_output, "wb") as o2:
-            if redirect:
-                files = {d: (open(getattr(args, d + "_output"), "wb"), open(getattr(args, d + "_paired_output"), "wb"))
-                         for d in redirect}
-                files["output"] = (o1, o2)
-                for parts in t.process_chunks_split(paired_reader(f1, f2, args.buffer_size)):
-                    for name, (r1, r2) in parts.items():
-                        files[name][0].write(r1)
-                        files[name][1].write(r2)
-                for d in redirect:
-                    files[d][0].close()
-                    files[d][1].close()
-            else:
-                for c1, c2 in paired_reader(f1, f2, args.buffer_size):
-                    r1, r2 = t.process_chunk(c1, c2)
-                    o1.write(r1)
-                    o2.write(r2)
+        options2 = dict(common, minimum_length=min2, maximum_length=max2)
+        # an output is interleaved when its paired path is missing (cli.py:650-661, 913-921)
+        interleaved = [d for d in ["output"] + redirect
+                       if not (args.paired_output if d == "output" else getattr(args, d + "_paired_output"))]
+        t = PairedFastqTrimmer(ads1, ads2, common, options2, args.pair_filter, **formats, **split,
+                               interleaved_outputs=interleaved)
+        if len(args.inputs) == 2:
+            f1, f2 = open(args.inputs[0], "rb"), open(args.inputs[1], "rb")
+            chunks = paired_reader(f1, f2, args.buffer_size)
+        else:
+            f1 = f2 = open(args.inputs[0], "rb")
+            chunks = (read_interleaved_fasta_chunks if input_format == "fasta" else read_interleaved_fastq_chunks)(
+                f1, args.buffer_size)
+        paths = {d: (getattr(args, d + "_output"), getattr(args, d + "_paired_output")) for d in redirect}
+        paths["output"] = (args.output, args.paired_output)
+        files = {d: tuple(open(p, "wb") if p else None for p in ps) for d, ps in paths.items()}
+        for parts in t.process_chunks_split(chunks):
+            for name, (r1, r2) in parts.items():
+                files[name][0].write(r1)
+                if files[name][1] is not None:
+                    files[name][1].write(r2)
+        for fhs in files.values():
+            for fh in fhs:
+                if fh is not None:
+                    fh.close()
+        f1.close()
+        f2.close()
         stats = {"read1": t.statistics[0], "read2": t.statistics[1]}
     elif "{name}" in args.output:
         t = FastqTrimmer(ads1, **common, **formats)
@@ -229,7 +281,7 @@ def main():
         stats = t.statistics
     print(json.dumps(stats), file=sys.stderr)
     if args.json is not None:
-        if len(args.inputs) == 2:
+        if paired:
             report = {f"read{k + 1}": report_json(t.statistics[k], t.adapter_statistics()[k], t.poly_a_trimmed_lengths[k],
                                                   t.written_lengths[k]) for k in (0, 1)}
         else:
