@@ -41,6 +41,9 @@ CG_REDIRECT_TOO_SHORT = 1        # cg_fastq_collect_split: --too-short-output (d
 CG_REDIRECT_TOO_LONG = 2         # --too-long-output (destination 2)
 CG_REDIRECT_UNTRIMMED = 4        # --untrimmed-output (destination 3)
 CG_INTERLEAVE_MAIN = 8           # cg_fastq_collect_paired_interleaved: the main output is interleaved
+CG_GZIP_MAIN = 8                 # cg_fastq_params.gzip_outputs: the main (every demultiplexed) output is gzip
+GZ_MEMBER = 65280                # plain bytes per gzip member of a gzip output ...
+GZ_OVERHEAD = 23                 # ... and the most a member adds to them
 
 
 class cg_kmer_entry(C.Structure):
@@ -131,7 +134,7 @@ class cg_fastq_params(C.Structure):
         ("revcomp", C.c_int32),
         ("format", C.c_int32),
         ("stats", C.c_int32),
-        ("reserved", C.c_int32),
+        ("gzip_outputs", C.c_int32),
     ]
 
 
@@ -139,10 +142,12 @@ class cg_fastq_result(C.Structure):
     _fields_ = [(name, C.c_int64) for name in (
         "n_records", "n_written", "bp_in", "bp_out", "out_bytes", "with_adapters", "quality_trimmed_bp",
         "too_short", "too_long", "too_many_n", "too_many_expected_errors", "discarded", "casava_filtered",
-        "reverse_complemented")] + [("reserved", C.c_int64 * 2)]
+        "reverse_complemented", "out_bytes_plain")] + [("reserved", C.c_int64 * 1)]
 
-    def as_dict(self) -> dict:
-        return {name: int(getattr(self, name)) for name, _ in self._fields_ if name != "reserved"}
+    def as_dict(self, plain_bytes: bool = False) -> dict:
+        """The counters; out_bytes_plain (the uncompressed size of gzip outputs) only with plain_bytes."""
+        return {name: int(getattr(self, name)) for name, _ in self._fields_
+                if name != "reserved" and (plain_bytes or name != "out_bytes_plain")}
 
 
 MATCH_DTYPE = np.dtype(

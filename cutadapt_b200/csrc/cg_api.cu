@@ -19,6 +19,7 @@
 #include "cg_hostpack.h"
 #include <array>
 
+#include "cg_gzip_core.cuh"
 #include "cg_kernels.cuh"
 #include "cg_jit.h"
 #include "cg_setbuild.h"
@@ -130,6 +131,10 @@ struct FastqSlot {
     PinBuf<unsigned long long> h_fqstats;
     DevBuf<int32_t> d_fold;                     // interleaved outputs: the sizes the partition runs on
     DevBuf<unsigned long long> d_ilverr;        // interleaved input: first problem of the split, record << 32 | code
+    DevBuf<CgGzPiece> d_gzpieces;               // gzip outputs: the pieces of the destinations ...
+    DevBuf<uint8_t> d_gzslots, d_gzout;         // ... each compressed into its slot, then packed
+    DevBuf<int32_t> d_gzsizes;
+    DevBuf<int64_t> d_gzoff;
     // interleaved input (cg_fastq_submit_interleaved): 0 = a chunk of its own, 1 / 2 = mate 1 / 2 of the chunk uploaded to
     // mate 1's slot, split when the pair is collected; ilv_peer = the other mate's slot, ilv_format = input format
     int ilv = 0, ilv_peer = -1, ilv_format = 0;
@@ -302,6 +307,7 @@ extern "C" int cg_ctx_destroy(cg_ctx *c)
         f.d_names.release(); f.d_infoout.release(); f.d_nameoff.release(); f.d_inforow.release(); f.d_infooff.release();
         f.d_norm.release(); f.d_faline.release(); f.d_faoff.release();
         f.d_fqstats.release(); f.d_polya.release(); f.h_fqstats.release();
+        f.d_gzpieces.release(); f.d_gzslots.release(); f.d_gzout.release(); f.d_gzsizes.release(); f.d_gzoff.release();
         f.h_in.release(); f.h_out.release(); f.h_counters.release();
         if (f.d_counters) cudaFree(f.d_counters);
         if (f.d_err) cudaFree(f.d_err);
@@ -2329,11 +2335,66 @@ static int fastq_copy_out(cg_ctx *c, FastqSlot &f, uint8_t *out, const uint8_t *
     return CG_OK;
 }
 
+// gzip outputs: the destinations of d_src at bounds[0 .. n_dest] (host), destination d compressed when gz[d], else copied.
+// Every destination is cut into pieces of GZ_MEMBER bytes from its start; gz_compress_kernel turns each gzip piece into a
+// member in its slot, the host places the pieces behind each other and gz_gather_kernel packs them into f.d_gzout.
+// bounds then hold where each destination lies there; *total is the packed size.
+static int fastq_gzip(cg_ctx *c, FastqSlot &f, const uint8_t *d_src, std::vector<int64_t> &bounds, const std::vector<char> &gz,
+                      long long *total, cudaStream_t st)
+{
+    const size_t n_dest = gz.size();
+    std::vector<CgGzPiece> pieces;
+    for (size_t d = 0; d < n_dest; ++d)
+        for (int64_t o = bounds[d]; o < bounds[d + 1]; o += GZ_MEMBER)
+            pieces.push_back(CgGzPiece{(long long)o, (int32_t)std::min<int64_t>(GZ_MEMBER, bounds[d + 1] - o), gz[d] ? 1 : 0});
+    const size_t np = pieces.size();
+    *total = 0;
+    if (np == 0) return CG_OK;
+    int rc;
+    if ((rc = f.d_gzpieces.ensure(np)) != CG_OK || (rc = f.d_gzsizes.ensure(np)) != CG_OK ||
+        (rc = f.d_gzoff.ensure(np)) != CG_OK || (rc = f.d_gzslots.ensure(np * GZ_SLOT)) != CG_OK)
+        return rc;
+    CU(cudaMemcpyAsync(f.d_gzpieces.p, pieces.data(), np * sizeof(CgGzPiece), cudaMemcpyHostToDevice, st));
+    CU(cg_launch_gzip_compress(d_src, f.d_gzpieces.p, (int)np, f.d_gzslots.p, f.d_gzsizes.p, st));
+    std::vector<int32_t> sizes(np);
+    CU(cudaMemcpyAsync(sizes.data(), f.d_gzsizes.p, np * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    std::vector<int64_t> off(np);
+    int64_t at = 0;
+    size_t k = 0;
+    for (size_t d = 0; d < n_dest; ++d) {
+        const int64_t n_pieces = (bounds[d + 1] - bounds[d] + GZ_MEMBER - 1) / GZ_MEMBER;
+        bounds[d] = at;
+        for (int64_t i = 0; i < n_pieces; ++i, ++k) { off[k] = at; at += sizes[k]; }
+    }
+    bounds[n_dest] = at;
+    if ((rc = f.d_gzout.ensure((size_t)at + 64)) != CG_OK) return rc;
+    CU(cudaMemcpyAsync(f.d_gzoff.p, off.data(), np * sizeof(int64_t), cudaMemcpyHostToDevice, st));
+    CU(cg_launch_gzip_gather(f.d_gzslots.p, f.d_gzsizes.p, f.d_gzoff.p, (int)np, f.d_gzout.p, st));
+    c->launches += 2;
+    *total = at;
+    return CG_OK;
+}
+
+// whether destination d of a collect is written as gzip: the main output (every output of a demultiplexing collect)
+// under CG_GZIP_MAIN, filter output d under CG_REDIRECT_* bit d - 1
+static bool gzip_dest(int gzip_outputs, bool demux, int d)
+{
+    return (demux || d == 0) ? (gzip_outputs & CG_GZIP_MAIN) != 0 : ((gzip_outputs >> (d - 1)) & 1) != 0;
+}
+
+static int gzip_check(const cg_fastq_params *fp, const char *who)
+{
+    if (fp->gzip_outputs & ~(CG_GZIP_MAIN | 7))
+        return fail(CG_EINVAL, std::string(who) + ": gzip_outputs takes CG_GZIP_MAIN and CG_REDIRECT_* bits only");
+    return CG_OK;
+}
+
 // sizes -> offsets -> formatted records -> host; counters.  segments (host, n_dest + 1 values): where each destination
 // starts in `out`.
 static int fastq_stage_output(cg_ctx *c, FastqSlot &f, const FqStage &g, cudaStream_t st, uint8_t *out,
                               int64_t out_capacity, cg_fastq_result *res, const FqDemux *dm = nullptr,
-                              int64_t *segments = nullptr, const FqSplit *sp = nullptr)
+                              int64_t *segments = nullptr, const FqSplit *sp = nullptr, int gzip_outputs = 0)
 {
     const long long n = g.n;
     int rc;
@@ -2348,7 +2409,24 @@ static int fastq_stage_output(cg_ctx *c, FastqSlot &f, const FqStage &g, cudaStr
         CU(cudaMemcpyAsync(&total, f.d_outoff.p + n, sizeof total, cudaMemcpyDeviceToHost, st));
     }
     if ((rc = fastq_stage_result(f, g, st, res)) != CG_OK) return rc;
-    res->out_bytes = total;
+    res->out_bytes = res->out_bytes_plain = total;
+    if (gzip_outputs && total > 0) {
+        const int n_dest = dm ? dm->n_dest() : sp ? FqSplit::n_dest : 1;
+        std::vector<int64_t> bounds{0, (int64_t)total};
+        if (segments) bounds.assign(segments, segments + n_dest + 1);
+        std::vector<char> gz((size_t)n_dest);
+        for (int d = 0; d < n_dest; ++d) gz[(size_t)d] = gzip_dest(gzip_outputs, dm != nullptr, d);
+        if ((rc = f.d_out.ensure((size_t)total + 64)) != CG_OK) return rc;
+        if ((rc = fastq_write_records(c, f, g, f.d_out.p, sp, segments, st)) != CG_OK) return rc;
+        long long packed = 0;
+        if ((rc = fastq_gzip(c, f, f.d_out.p, bounds, gz, &packed, st)) != CG_OK) return rc;
+        res->out_bytes = packed;
+        if (packed > out_capacity)
+            return fail(CG_EINVAL, "cg_fastq_collect: output buffer too small (" + std::to_string(packed) + " bytes needed)");
+        if (!out) return fail(CG_EINVAL, "cg_fastq_collect: out is NULL");
+        if (segments) std::copy(bounds.begin(), bounds.end(), segments);
+        return fastq_copy_out(c, f, out, f.d_gzout.p, packed, st);
+    }
     if (total > out_capacity)
         return fail(CG_EINVAL, "cg_fastq_collect: output buffer too small (" + std::to_string(total) + " bytes needed)");
     if (total > 0) {
@@ -2367,7 +2445,7 @@ static int fastq_stage_output(cg_ctx *c, FastqSlot &f, const FqStage &g, cudaStr
 static int fastq_stage_output_interleaved(cg_ctx *c, FastqSlot &f1, const FqStage &g1, FastqSlot &f2, const FqStage &g2,
                                           cudaStream_t st, uint8_t *out1, int64_t out_capacity1, uint8_t *out2,
                                           int64_t out_capacity2, cg_fastq_result *res1, cg_fastq_result *res2,
-                                          int64_t *segments1, int64_t *segments2, const FqSplit &sp)
+                                          int64_t *segments1, int64_t *segments2, const FqSplit &sp, int gzip1, int gzip2)
 {
     const long long n = g1.n;
     int rc;
@@ -2384,8 +2462,38 @@ static int fastq_stage_output_interleaved(cg_ctx *c, FastqSlot &f1, const FqStag
     c->launches += 1;
     if ((rc = fastq_stage_result(f1, g1, st, res1)) != CG_OK) return rc;
     if ((rc = fastq_stage_result(f2, g2, st, res2)) != CG_OK) return rc;
-    res1->out_bytes = total1;
-    res2->out_bytes = total2;
+    res1->out_bytes = res1->out_bytes_plain = total1;
+    res2->out_bytes = res2->out_bytes_plain = total2;
+    if ((gzip1 || gzip2) && total1 + total2 > 0) {
+        // out1's four destinations, then out2's, in the one buffer the writer fills
+        std::vector<int64_t> bounds(2 * FqSplit::n_dest + 1);
+        std::vector<char> gz(2 * FqSplit::n_dest);
+        for (int d = 0; d < FqSplit::n_dest; ++d) {
+            bounds[d] = segments1[d];
+            bounds[FqSplit::n_dest + d] = total1 + segments2[d];
+            gz[d] = gzip_dest(gzip1, false, d);
+            gz[FqSplit::n_dest + d] = gzip_dest(gzip2, false, d);
+        }
+        bounds[2 * FqSplit::n_dest] = total1 + total2;
+        if ((rc = f1.d_out.ensure((size_t)(total1 + total2) + 64)) != CG_OK) return rc;
+        if ((rc = fastq_write_records(c, f1, g1, f1.d_out.p, &sp, segments1, st)) != CG_OK) return rc;
+        if ((rc = fastq_write_records(c, f2, g2, f1.d_out.p, &sp, segments1, st)) != CG_OK) return rc;
+        long long packed = 0;
+        if ((rc = fastq_gzip(c, f1, f1.d_out.p, bounds, gz, &packed, st)) != CG_OK) return rc;
+        const int64_t packed1 = bounds[FqSplit::n_dest], packed2 = packed - packed1;
+        res1->out_bytes = packed1;
+        res2->out_bytes = packed2;
+        if (packed1 > out_capacity1 || packed2 > out_capacity2)
+            return fail(CG_EINVAL, "cg_fastq_collect_paired_interleaved: output buffer too small (" + std::to_string(packed1) +
+                                       " and " + std::to_string(packed2) + " bytes needed)");
+        if ((packed1 && !out1) || (packed2 && !out2)) return fail(CG_EINVAL, "cg_fastq_collect_paired_interleaved: out is NULL");
+        for (int d = 0; d <= FqSplit::n_dest; ++d) {
+            segments1[d] = bounds[d];
+            segments2[d] = bounds[FqSplit::n_dest + d] - packed1;
+        }
+        if ((rc = fastq_copy_out(c, f1, out1, f1.d_gzout.p, packed1, st)) != CG_OK) return rc;
+        return fastq_copy_out(c, f2, out2, f1.d_gzout.p + packed1, packed2, st);
+    }
     if (total1 > out_capacity1 || total2 > out_capacity2)
         return fail(CG_EINVAL, "cg_fastq_collect_paired_interleaved: output buffer too small (" + std::to_string(total1) +
                                    " and " + std::to_string(total2) + " bytes needed)");
@@ -2461,6 +2569,7 @@ static int fastq_collect_impl(cg_ctx *c, int32_t slot, const cg_adapterset *s, c
     memset(res, 0, sizeof *res);
     int rc;
     if (sp && (rc = split_check(*sp, fp, "cg_fastq_collect_split")) != CG_OK) return rc;
+    if ((rc = gzip_check(fp, "cg_fastq_collect")) != CG_OK) return rc;
     FqStage g;
     rc = fqstats_lookup(c, fp->stats, s ? s->host.n_adapters : 0, &g.acc);
     if (rc != CG_OK) return rc;
@@ -2480,7 +2589,8 @@ static int fastq_collect_impl(cg_ctx *c, int32_t slot, const cg_adapterset *s, c
                               sp ? sp->redirect : 0, sp ? sp->fasta_dests : 0, sp ? sp->d_route : nullptr));
     c->launches += 1;
     if ((rc = fastq_stage_stats_tail(c, f, g, f.stream, sp ? sp->d_route : nullptr)) != CG_OK) return rc;
-    if ((rc = fastq_stage_output(c, f, g, f.stream, out, out_capacity, res, dm, segments, sp)) != CG_OK) return rc;
+    if ((rc = fastq_stage_output(c, f, g, f.stream, out, out_capacity, res, dm, segments, sp, fp->gzip_outputs)) != CG_OK)
+        return rc;
     if ((rc = check_err_flag(c)) != CG_OK) return rc;
     fastq_stats_commit(f, g, fp, *res);
     return CG_OK;
@@ -2678,6 +2788,19 @@ static int fastq_collect_paired_impl(cg_ctx *c, int32_t slot1, int32_t slot2, co
         cudaStreamSynchronize(f2.stream);
         return rc;
     }
+    if ((rc = gzip_check(fp1, "cg_fastq_collect_paired")) != CG_OK || (rc = gzip_check(fp2, "cg_fastq_collect_paired")) != CG_OK) {
+        cudaStreamSynchronize(f2.stream);
+        return rc;
+    }
+    if (sp && sp->interleaved) {
+        // an interleaved destination holds both mates: both must agree on compressing it
+        const int ilv_bits = ((sp->ilv_dests & 1) ? CG_GZIP_MAIN : 0) | (sp->ilv_dests >> 1);
+        if ((fp1->gzip_outputs ^ fp2->gzip_outputs) & ilv_bits) {
+            cudaStreamSynchronize(f2.stream);
+            return fail(CG_EINVAL, "cg_fastq_collect_paired_interleaved: an interleaved output must have its gzip_outputs bit "
+                                   "set alike in both mates' parameters");
+        }
+    }
     if ((rc = fqstats_lookup(c, fp1->stats, pa ? pa->n_pairs : (s1 ? s1->host.n_adapters : 0), &g1.acc)) != CG_OK ||
         (rc = fqstats_lookup(c, fp2->stats, pa ? pa->n_pairs : (s2 ? s2->host.n_adapters : 0), &g2.acc)) != CG_OK) {
         cudaStreamSynchronize(f2.stream);
@@ -2717,11 +2840,13 @@ static int fastq_collect_paired_impl(cg_ctx *c, int32_t slot1, int32_t slot2, co
     if ((rc = fastq_stage_stats_tail(c, f2, g2, st, route)) != CG_OK) return rc;
     if (sp && sp->interleaved) {
         rc = fastq_stage_output_interleaved(c, f1, g1, f2, g2, st, out1, out_capacity1, out2, out_capacity2, res1, res2,
-                                            segments1, segments2, *sp);
+                                            segments1, segments2, *sp, fp1->gzip_outputs, fp2->gzip_outputs);
         if (rc != CG_OK) return rc;
     } else {
-        if ((rc = fastq_stage_output(c, f1, g1, st, out1, out_capacity1, res1, dm, segments1, sp)) != CG_OK) return rc;
-        if ((rc = fastq_stage_output(c, f2, g2, st, out2, out_capacity2, res2, dm, segments2, sp)) != CG_OK) return rc;
+        if ((rc = fastq_stage_output(c, f1, g1, st, out1, out_capacity1, res1, dm, segments1, sp, fp1->gzip_outputs)) != CG_OK)
+            return rc;
+        if ((rc = fastq_stage_output(c, f2, g2, st, out2, out_capacity2, res2, dm, segments2, sp, fp2->gzip_outputs)) != CG_OK)
+            return rc;
     }
     if ((rc = check_err_flag(c)) != CG_OK) return rc;
     fastq_stats_commit(f1, g1, fp1, *res1);

@@ -190,6 +190,18 @@ cudaError_t cg_launch_interleaved_split(int phase, const uint8_t *d_buf, long lo
 cudaError_t cg_launch_fastq_interleave(int phase, long long n_records, const int32_t *d_route, int ilv,
                                        const int32_t *d_len1, const int32_t *d_len2, int32_t *d_fold1, int32_t *d_fold2,
                                        const int64_t *d_off1, int64_t *d_off2, const int64_t *d_total1, cudaStream_t st);
+// gzip outputs (cg_gzip.cu): a piece of at most GZ_MEMBER bytes of a destination, at d_src + src; gz = 1 compresses it
+// into one member, gz = 0 copies it.  Piece k goes to d_slots + k * GZ_SLOT, its size to d_sizes[k]; the gather then
+// packs the pieces to d_out + d_dst_off[k].
+struct CgGzPiece {
+    long long src;
+    int32_t len;
+    int32_t gz;
+};
+cudaError_t cg_launch_gzip_compress(const uint8_t *d_src, const CgGzPiece *d_pieces, int n_pieces, uint8_t *d_slots,
+                                    int32_t *d_sizes, cudaStream_t st);
+cudaError_t cg_launch_gzip_gather(const uint8_t *d_slots, const int32_t *d_sizes, const int64_t *d_dst_off, int n_pieces,
+                                  uint8_t *d_out, cudaStream_t st);
 // --pair-adapters: fold the records of adapter pair `pair` into the best pair per read (modifiers.py:480-503)
 cudaError_t cg_launch_fastq_pair_select(long long n_records, int pair, const cg_match_rec *d_cur1, int slots1,
                                         const cg_match_rec *d_cur2, int slots2, cg_match_rec *d_best1, cg_match_rec *d_best2,

@@ -827,11 +827,13 @@ def _format_code(input_format: str, output_format: Optional[str]) -> int:
     return _FORMATS[(input_format, output_format)]
 
 
-def _output_capacity(n_bytes: int, fmt: int) -> int:
+def _output_capacity(n_bytes: int, fmt: int, gzip: bool = False, n_dest: int = 4) -> int:
     """Output bytes a chunk of n_bytes can need: trimming only shortens a record ("\\r\\n" -> "\\n" and "+name" -> "+"
     too), except for the newline a chunk without a final one gets and, in FASTA, the empty line of a record without
-    sequence (">a\\n" -> ">a\\n\\n", at most 1.5 x)."""
-    return (n_bytes + n_bytes // 2 if fmt == _lib.CG_FORMAT_FASTA else n_bytes) + 16
+    sequence (">a\\n" -> ">a\\n\\n", at most 1.5 x).  gzip outputs: a member adds at most 23 bytes to its 65 280, and
+    each of the n_dest outputs can end in a short member."""
+    plain = (n_bytes + n_bytes // 2 if fmt == _lib.CG_FORMAT_FASTA else n_bytes) + 16
+    return plain + (_lib.GZ_OVERHEAD * (plain // _lib.GZ_MEMBER + n_dest) if gzip else 0)
 
 
 def _fastq_params(times=1, quality_cutoff=None, quality_base=33, nextseq_cutoff=None, minimum_length=0,
@@ -876,6 +878,16 @@ REDIRECT_OUTPUTS = ("too_short", "too_long", "untrimmed")     # destinations 1, 
 # the outputs cg_fastq_collect_paired_interleaved can interleave, and their bits
 INTERLEAVE_BITS = {"output": _lib.CG_INTERLEAVE_MAIN, "too_short": _lib.CG_REDIRECT_TOO_SHORT,
                    "too_long": _lib.CG_REDIRECT_TOO_LONG, "untrimmed": _lib.CG_REDIRECT_UNTRIMMED}
+
+
+def _gzip_bits(names) -> int:
+    """cg_fastq_params.gzip_outputs of output names out of ("output",) + REDIRECT_OUTPUTS."""
+    bits = 0
+    for name in names or ():
+        if name not in INTERLEAVE_BITS:
+            raise ValueError(f"unknown output {name!r} to compress (one of {', '.join(INTERLEAVE_BITS)})")
+        bits |= _lib.CG_GZIP_MAIN if name == "output" else INTERLEAVE_BITS[name]
+    return bits
 
 
 def _redirect_bits(redirect, redirect_formats, params) -> Tuple[int, int]:
@@ -960,6 +972,10 @@ class FastqTrimmer:
                         are written to their own output, trimmed like the main output (``process_chunk_split``);
                         "untrimmed" switches the untrimmed filter on and counts its reads in ``discarded``
     redirect_formats    {output name: "fastq" or "fasta"}; an output not named has the main output's format
+    gzip_outputs        names out of ("output",) + REDIRECT_OUTPUTS written as gzip, compressed on the device: every
+                        method then returns gzip members (65 280 plain bytes each, see cg_fastq_params.gzip_outputs;
+                        "output" covers every demultiplexed output), which concatenate into one gzip file, and
+                        ``statistics`` gains ``out_bytes_plain``, the uncompressed size
 
     ``process_chunk(bytes) -> bytes``; ``process_chunks(iterable)`` keeps one chunk in flight so that the
     upload of chunk i+1 overlaps the download of chunk i.  With ``redirect``: ``process_chunk_split(bytes) ->
@@ -977,10 +993,13 @@ class FastqTrimmer:
                  action: Optional[str] = "trim", revcomp: bool = False, rc_suffix: bool = True,
                  input_format: str = "fastq", output_format: Optional[str] = None,
                  ctx: Optional[_lib.Context] = None, collect_statistics: bool = False,
-                 redirect: Sequence[str] = (), redirect_formats: Optional[dict] = None):
+                 redirect: Sequence[str] = (), redirect_formats: Optional[dict] = None,
+                 gzip_outputs: Sequence[str] = ()):
         self.params = _fastq_params(times, quality_cutoff, quality_base, nextseq_cutoff, minimum_length, maximum_length,
                                     max_n, max_expected_errors, discard_trimmed, discard_untrimmed, cut, poly_a, length,
                                     trim_n, discard_casava, action, revcomp, rc_suffix, input_format, output_format)
+        self.gzip_outputs = tuple(dict.fromkeys(gzip_outputs or ()))
+        self.params.gzip_outputs = _gzip_bits(self.gzip_outputs)
         self.redirect = tuple(dict.fromkeys(redirect or ()))
         self._redirect, self._fasta_outputs = _redirect_bits(self.redirect, redirect_formats, self.params)
         self.ctx = ctx or _lib.default_context()
@@ -1000,6 +1019,13 @@ class FastqTrimmer:
                                               C.byref(slot)))
         return slot.value, buf.size, buf    # buf is kept alive until collect
 
+    def _capacity(self, n_bytes: int, n_dest: int = 4) -> int:
+        return _output_capacity(n_bytes, self.params.format, self.params.gzip_outputs != 0, n_dest)
+
+    def _account(self, res) -> None:
+        for k, v in res.as_dict(self.params.gzip_outputs != 0).items():
+            self.statistics[k] = self.statistics.get(k, 0) + v
+
     def _out_buffer(self, slot: int, n_bytes: int) -> np.ndarray:
         """Per-slot output buffer, pinned when torch can provide it (the download then needs no bounce)."""
         buf = self._out_bufs.get(slot)
@@ -1017,7 +1043,7 @@ class FastqTrimmer:
 
     def _collect(self, ticket, copy: bool = True):
         slot, n_bytes, chunk = ticket
-        out = self._out_buffer(slot, _output_capacity(n_bytes, self.params.format))
+        out = self._out_buffer(slot, self._capacity(n_bytes))
         while True:
             res = _lib.cg_fastq_result()
             rc = _lib.lib().cg_fastq_collect(
@@ -1030,8 +1056,7 @@ class FastqTrimmer:
                 continue
             _lib.check(rc)
             break
-        for k, v in res.as_dict().items():
-            self.statistics[k] = self.statistics.get(k, 0) + v
+        self._account(res)
         return out[: res.out_bytes].tobytes() if copy else out[: res.out_bytes]
 
     def _no_redirect(self, what: str):
@@ -1045,7 +1070,7 @@ class FastqTrimmer:
 
     def _collect_split(self, ticket, copy: bool = True) -> dict:
         slot, n_bytes, chunk = ticket
-        out = self._out_buffer(slot, _output_capacity(n_bytes, self.params.format))
+        out = self._out_buffer(slot, self._capacity(n_bytes))
         segments = np.zeros(5, dtype=np.int64)
         while True:
             res = _lib.cg_fastq_result()
@@ -1059,8 +1084,7 @@ class FastqTrimmer:
                 continue
             _lib.check(rc)
             break
-        for k, v in res.as_dict().items():
-            self.statistics[k] = self.statistics.get(k, 0) + v
+        self._account(res)
         names = ("output",) + REDIRECT_OUTPUTS
         part = (lambda a, b: out[a:b].tobytes()) if copy else (lambda a, b: out[a:b])
         return {name: part(segments[d], segments[d + 1]) for d, name in enumerate(names)
@@ -1091,14 +1115,13 @@ class FastqTrimmer:
         self._no_redirect("demultiplexing")
         outputs, dest = self._demux_names()
         slot, n_bytes, _ = self._submit(chunk)
-        out = self._out_buffer(slot, _output_capacity(n_bytes, self.params.format))
+        out = self._out_buffer(slot, self._capacity(n_bytes, len(outputs) + 1))
         res = _lib.cg_fastq_result()
         segments = np.zeros(len(outputs) + 2, dtype=np.int64)
         _lib.check(_lib.lib().cg_fastq_collect_demux(
             self.ctx.handle, slot, self._set.handle, C.byref(self.params), dest.ctypes.data, len(outputs),
             out.ctypes.data, out.size, C.byref(res), segments.ctypes.data))
-        for k, v in res.as_dict().items():
-            self.statistics[k] = self.statistics.get(k, 0) + v
+        self._account(res)
         return {name: out[segments[i]:segments[i + 1]].tobytes() for i, name in enumerate(outputs + [unknown])}
 
     def _info_names(self):
@@ -1124,7 +1147,7 @@ class FastqTrimmer:
         capacity = per_read * 2 * n_bytes + (1 << 20)
         while True:
             slot, _, _ = self._submit(chunk)
-            out = self._out_buffer(slot, _output_capacity(n_bytes, self.params.format))
+            out = self._out_buffer(slot, self._capacity(n_bytes))
             rows = np.empty(capacity, dtype=np.uint8)
             res = _lib.cg_fastq_result()
             n_rows = C.c_int64(0)
@@ -1136,8 +1159,7 @@ class FastqTrimmer:
                 continue
             _lib.check(rc)
             break
-        for k, v in res.as_dict().items():
-            self.statistics[k] = self.statistics.get(k, 0) + v
+        self._account(res)
         return out[: res.out_bytes].tobytes(), rows[: n_rows.value].tobytes()
 
     def process_chunk_info(self, chunk) -> Tuple[bytes, bytes]:
@@ -1231,7 +1253,8 @@ class PairedFastqTrimmer:
     ``process_chunks_split`` takes single chunks in place of pairs.  ``interleaved_outputs``: names out of
     ``("output",) + REDIRECT_OUTPUTS`` whose output is written interleaved, R1 then R2 of each pair, returned as
     ``(bytes, b"")`` (the reference interleaves an output whose paired path is missing).  Not with ``pair_adapters``
-    or demultiplexing.
+    or demultiplexing.  ``gzip_outputs`` / ``gzip_outputs2``: as FastqTrimmer's ``gzip_outputs``, for R1's files and for
+    R2's (default: the same names); an interleaved output must be named in both.
     """
 
     MODES = {"any": 0, "both": 1, "first": 2}
@@ -1241,12 +1264,15 @@ class PairedFastqTrimmer:
                  input_format: str = "fastq", output_format: Optional[str] = None,
                  ctx: Optional[_lib.Context] = None, collect_statistics: bool = False,
                  redirect: Sequence[str] = (), redirect_formats: Optional[dict] = None,
-                 interleaved_outputs: Sequence[str] = ()):
+                 interleaved_outputs: Sequence[str] = (), gzip_outputs: Sequence[str] = (),
+                 gzip_outputs2: Optional[Sequence[str]] = None):
         if pair_filter not in self.MODES:
             raise ValueError("pair_filter must be 'any', 'both' or 'first'")
         formats = dict(input_format=input_format, output_format=output_format)
         self.params1 = _fastq_params(**{**(options1 or {}), **formats})
         self.params2 = _fastq_params(**{**(options2 or {}), **formats})
+        self.params1.gzip_outputs = _gzip_bits(gzip_outputs)
+        self.params2.gzip_outputs = _gzip_bits(gzip_outputs if gzip_outputs2 is None else gzip_outputs2)
         self.redirect = tuple(dict.fromkeys(redirect or ()))
         self._redirect, self._fasta_outputs = _redirect_bits(self.redirect, redirect_formats, self.params1)
         _redirect_bits(self.redirect, redirect_formats, self.params2)
@@ -1345,10 +1371,11 @@ class PairedFastqTrimmer:
                                                           buf.size, self.params1.format, C.byref(s1), C.byref(s2)))
         return (s1.value, buf), (s2.value, buf)
 
-    def _out_buffers(self, tickets):
+    def _out_buffers(self, tickets, n_dest: int = 4):
         """Output buffers of a pair: out1 also holds R2 of the interleaved outputs."""
         (_, b1), (_, b2) = tickets
-        n1, n2 = _output_capacity(b1.size, self.params1.format), _output_capacity(b2.size, self.params2.format)
+        n1 = _output_capacity(b1.size, self.params1.format, self.params1.gzip_outputs != 0, n_dest)
+        n2 = _output_capacity(b2.size, self.params2.format, self.params2.gzip_outputs != 0, n_dest)
         return np.empty(n1 + (n2 if self._interleave else 0), dtype=np.uint8), np.empty(n2, dtype=np.uint8)
 
     def _no_interleave(self, what: str):
@@ -1356,8 +1383,8 @@ class PairedFastqTrimmer:
             raise ValueError(f"interleaved outputs ({', '.join(self.interleaved_outputs)}) cannot be combined with {what}")
 
     def _account(self, r1, r2):
-        for st, res in zip(self.statistics, (r1, r2)):
-            for k, v in res.as_dict().items():
+        for st, res, p in zip(self.statistics, (r1, r2), (self.params1, self.params2)):
+            for k, v in res.as_dict(p.gzip_outputs != 0).items():
                 st[k] = st.get(k, 0) + v
 
     def _no_redirect(self, what: str):
@@ -1457,7 +1484,7 @@ class PairedFastqTrimmer:
             keep = np.array([1] * n1 + [0 if discard_untrimmed else 1], dtype=np.uint8)
         tickets = self._submit_pair(chunk1, chunk2)
         (s1, b1), (s2, b2) = tickets
-        out1, out2 = self._out_buffers(tickets)
+        out1, out2 = self._out_buffers(tickets, len(keys))
         r1, r2 = _lib.cg_fastq_result(), _lib.cg_fastq_result()
         seg1 = np.zeros(len(keys) + 1, dtype=np.int64)
         seg2 = np.zeros(len(keys) + 1, dtype=np.int64)

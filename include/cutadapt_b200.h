@@ -336,7 +336,7 @@ typedef struct cg_fastq_params {
     int32_t format;              /* CG_FORMAT_*: what the chunk is and what is written (below); 0 = FASTQ    */
     int32_t stats;               /* 0 = off, else a handle of cg_fastq_stats_create: the call ADDS this mate's
                                     statistics to that accumulator if it succeeds (cg_fastq_stats_read, below) */
-    int32_t reserved;
+    int32_t gzip_outputs;        /* CG_GZIP_MAIN / CG_REDIRECT_* bits: the outputs written as gzip (below); 0 = plain */
 } cg_fastq_params;
 typedef struct cg_fastq_result {
     int64_t n_records, n_written;
@@ -345,7 +345,8 @@ typedef struct cg_fastq_result {
     int64_t with_adapters, quality_trimmed_bp;
     int64_t too_short, too_long, too_many_n, too_many_expected_errors, discarded, casava_filtered;
     int64_t reverse_complemented; /* --revcomp: reads replaced by their reverse complement             */
-    int64_t reserved[2];
+    int64_t out_bytes_plain;     /* size of the same outputs uncompressed (== out_bytes without gzip outputs) */
+    int64_t reserved[1];
 } cg_fastq_result;
 /* Formats (cg_fastq_params.format; both mates of a pair must have the same one, else CG_EINVAL):
  *   CG_FORMAT_FASTQ           FASTQ in, FASTQ out (zeroed parameters)
@@ -505,6 +506,25 @@ int cg_fastq_collect_paired_interleaved(cg_ctx *ctx, int32_t slot1, int32_t slot
                                         int32_t fasta_outputs, int32_t interleaved_outputs, uint8_t *out1,
                                         int64_t out_capacity1, uint8_t *out2, int64_t out_capacity2, cg_fastq_result *res1,
                                         cg_fastq_result *res2, int64_t *segments1, int64_t *segments2);
+
+/* gzip outputs: cg_fastq_params.gzip_outputs names the outputs that every call writing records (cg_fastq_trim_chunk,
+ * cg_fastq_collect, _demux, _info, _rows, _paired, _pair_adapters, _paired_demux, _split, _paired_split,
+ * _paired_interleaved) writes as gzip, compressed on the device before the download:
+ *   CG_GZIP_MAIN      the main output; in the demultiplexing collects every demultiplexed output, "unknown" included;
+ *   CG_REDIRECT_*     the filter outputs of the split collects (a bit for an output that is not redirected compresses
+ *                     nothing).
+ * Any other bit is CG_EINVAL.  params1 governs out1's outputs and params2 out2's; an interleaved output needs its bit set
+ * alike in both, else CG_EINVAL.  The row outputs of _info / _rows stay plain.
+ * Format: each output is cut into pieces of 65 280 bytes (0xff00) from its start, the last one shorter, and every piece is
+ * one gzip member: the header 1f 8b 08 00 00 00 00 00 00 ff (no name, mtime 0, OS unknown), one final deflate block
+ * (dynamic Huffman codes, or stored when that is not larger), CRC-32 and ISIZE.  An empty output is 0 bytes.  The members
+ * follow each other, which is one valid gzip file (RFC 1952 2.2), so chunk outputs can be concatenated.  The bytes depend
+ * on the plain bytes alone.  A member is at most 23 bytes larger than its piece, so an output of n plain bytes needs at
+ * most n + 23 * ceil(n / 65280) bytes.
+ * segments and out_bytes then describe the compressed outputs, out_bytes_plain the plain ones.  "Buffer too small" is
+ * judged on the compressed size (out_bytes says what is needed); counters, n_written, bp_out and the statistics vectors
+ * are those of the same call without compression. */
+#define CG_GZIP_MAIN 8
 
 /* ---- trim statistics (the payload of the end-of-run all-reduce, report.py:81-126) --------
  * Device-side reduction of a batch's match records into a fixed-layout int64 vector that carries everything the

@@ -17,10 +17,19 @@ cg_fastq_collect_split); the output bytes are those of all three outputs.
 mates; the mates of a pair share their name): "paired" streams them as two mate chunks per step
 (PairedFastqTrimmer.process_chunks_split, two uploads, two outputs), "interleaved" as one interleaved chunk in and out
 (cg_fastq_submit_interleaved, interleaved_outputs=("output",)); each step holds the same pairs, chunk_megabytes in all.
+--gzip: the FASTQ variant in three arms, alternating over three rounds in one process: plain output, gzip output
+compressed on the device (gzip_outputs=("output",)), and plain output compressed on the host by zlib level 1 on one
+thread (one stream over the run).  Per arm: host-to-host reads/s, output bytes, compression ratio and device-to-host
+bytes per chunk (Context.transfer_bytes); the card's name and power limit are read in the same run (nvidia-smi, a
+read-only query).  A second line: the device time of gz_compress_kernel and gz_gather_kernel per MiB of plain output
+and per chunk, from torch.profiler's CUDA activity in a run of its own over the warmed chunks, next to the wall time
+per chunk that gzip adds, so that kernel time and the host round trip of the compaction can be told apart.
 """
 import json
+import subprocess
 import sys
 import time
+import zlib
 
 import numpy as np
 import torch
@@ -82,7 +91,82 @@ def build_fasta(n, wrap=None, pinned=True):
     return host.numpy(), rec_len
 
 
+def measure_gzip(n, chunk_mb):
+    data, rec_len = build_fastq(n)
+    per_chunk = max(1, (chunk_mb << 20) // rec_len)
+    chunks = [data[i * rec_len:min(n, i + per_chunk) * rec_len] for i in range(0, n, per_chunk)]
+    adapters = [PA.BackAdapter("AGATCGGAAGAGC", max_errors=0.1)]
+    opts = dict(quality_cutoff=(0, 20), minimum_length=20)
+    arms = {"plain": FastqTrimmer(adapters, **opts), "device_gzip": FastqTrimmer(adapters, **opts, gzip_outputs=("output",)),
+            "host_zlib1": FastqTrimmer(adapters, **opts)}
+
+    def run(name, cs):
+        t = arms[name]
+        if name != "host_zlib1":
+            return sum(len(o) for o in t.process_chunks(cs, copy=False)), 0
+        z = zlib.compressobj(1, zlib.DEFLATED, 31)
+        plain = out = 0
+        for o in t.process_chunks(cs, copy=False):
+            plain += len(o)
+            out += len(z.compress(o))
+        return out + len(z.flush()), plain
+
+    for name in arms:
+        run(name, chunks[:3])                     # warm-up: buffers, module load
+    res = {name: {"wall_s": 0.0, "out_bytes": 0, "d2h_bytes": 0} for name in arms}
+    for _ in range(3):
+        for name in arms:
+            ctx = arms[name].ctx
+            ctx.transfer_bytes(reset=True)
+            t0 = time.perf_counter()
+            out, _ = run(name, chunks)
+            res[name]["wall_s"] += time.perf_counter() - t0
+            res[name]["out_bytes"] = out
+            res[name]["d2h_bytes"] = ctx.transfer_bytes()[1]
+    plain_bytes = res["plain"]["out_bytes"]
+    for name, r in res.items():
+        r["reads_per_s"] = 3 * n / r["wall_s"]
+        r["ratio"] = plain_bytes / r["out_bytes"]
+        r["d2h_bytes_per_chunk"] = r["d2h_bytes"] / len(chunks)
+    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader",
+                           "-i", str(torch.cuda.current_device())], capture_output=True, text=True).stdout.strip()
+    print(json.dumps({"what": "FASTQ -> trimmed FASTQ (-a AGATCGGAAGAGC -q 20 -m 20), host to host: plain, device gzip, "
+                              "plain + host zlib level 1 (one thread)", "reads": n, "chunk_mb": chunk_mb,
+                      "chunks": len(chunks), "gpu": torch.cuda.get_device_name(), "card_and_power_limit": card,
+                      "arms": res}))
+
+    # the compressor's kernels alone, in a profiled run of their own
+    from torch.profiler import ProfilerActivity, profile
+
+    rounds = 3
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(rounds):
+            run("device_gzip", chunks)
+        torch.cuda.synchronize()
+    ms = {"gz_compress_kernel": 0.0, "gz_gather_kernel": 0.0}
+    launches = {k: 0 for k in ms}
+    for ev in prof.key_averages():
+        for k in ms:
+            if k in ev.key:
+                ms[k] += ev.device_time_total / 1000.0
+                launches[k] += ev.count
+    if not launches["gz_compress_kernel"]:
+        raise RuntimeError("the profiler saw no gz_compress_kernel launch")
+    mib = rounds * plain_bytes / 2**20
+    n_chunks = rounds * len(chunks)
+    added = (res["device_gzip"]["wall_s"] - res["plain"]["wall_s"]) / (3 * len(chunks)) * 1000
+    print(json.dumps({"what": "gzip kernels' device time (torch.profiler, CUDA activity)",
+                      "card_and_power_limit": card,
+                      "ms_per_MiB_plain": {k: v / mib for k, v in ms.items()},
+                      "ms_per_chunk": {k: v / n_chunks for k, v in ms.items()},
+                      "launches": launches, "chunk_MiB_plain": plain_bytes / len(chunks) / 2**20,
+                      "wall_ms_per_chunk_added_by_gzip": added}))
+
+
 def main():
+    if "--gzip" in sys.argv:
+        argv = [a for a in sys.argv if a != "--gzip"]
+        return measure_gzip(int(argv[1]) if len(argv) > 1 else 4_000_000, int(argv[2]) if len(argv) > 2 else 64)
     collect = "--statistics" in sys.argv
     redirect = ("too_short", "untrimmed") if "--redirect" in sys.argv else ()
     argv = [a for a in sys.argv if a not in ("--statistics", "--redirect")]

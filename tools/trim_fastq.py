@@ -2,8 +2,7 @@
 """
 Trim FASTQ and FASTA files on the GPU: a minimal driver around cutadapt_b200.pipeline.FastqTrimmer / PairedFastqTrimmer
 that understands the subset of cutadapt's options the device path implements.  Not a replacement for cutadapt's
-command line (no reports, no compressed files): it shows the per-chunk worker of INTEGRATION.md section 3 running
-on real files.
+command line (no reports): it shows the per-chunk worker of INTEGRATION.md section 3 running on real files.
 
   python tools/trim_fastq.py -a AGATCGGAAGAGC -q 20 -m 20 -o out.fastq in.fastq
   python tools/trim_fastq.py -a ADAPT1 -A ADAPT2 -q 20 -m 20 -o out.1.fastq -p out.2.fastq in.1.fastq in.2.fastq
@@ -12,6 +11,7 @@ on real files.
   python tools/trim_fastq.py -a AGATCGGAAGAGC -m 20 --too-short-output short.fastq --untrimmed-output untrimmed.fasta \
       -o out.fastq in.fastq                                                            (filter outputs)
   python tools/trim_fastq.py --interleaved -a ADAPT1 -A ADAPT2 -m 20:25 -o out.fastq in.interleaved.fastq
+  python tools/trim_fastq.py -a AGATCGGAAGAGC -o out.fastq.gz in.fastq.gz                   (gzip)
 
 The input format comes from the first byte of the (first) input, as cutadapt's files.detect_file_format does: '>' or
 '#' is FASTA, anything else (an empty file included) FASTQ.  The output is FASTA when the input is, when -o ends in
@@ -23,8 +23,18 @@ collected on the device (collect_statistics=True); the stderr line stays as it i
 --interleaved, as in the reference: one input is interleaved input (R1 and R2 of each pair one after the other, split
 on the device), no -p means an interleaved main output, and a filter output without its --*-paired-output is written
 interleaved.  -m / -M take LEN[:LEN2], a length for each mate; an empty side means no filter on that mate.
+
+Compressed files: every output whose name ends in .gz (-o, -p, the filter outputs, a {name} template) is written as gzip,
+compressed on the device in members of 65 280 bytes; the others are plain, each decided by its own name.  One
+exception: with demultiplexing the device compresses all demultiplexed outputs alike, so --untrimmed-output (which
+receives the "unknown" output) must end in .gz exactly when the -o template does; otherwise the tool stops with an
+error.  A .gz output
+that receives no read still gets one empty gzip member.  The device has one compression strategy, comparable in size to
+zlib's level 1, so there is no --compression-level.  Inputs ending in .gz are decompressed on the host; the format is
+then detected from the first decompressed byte.
 """
 import argparse
+import gzip
 import json
 import sys
 
@@ -35,10 +45,38 @@ from cutadapt_b200.pipeline import (FastqTrimmer, PairedFastqTrimmer, read_fasta
                                     read_paired_fasta_chunks, read_paired_fastq_chunks)
 
 
+def open_input(path):
+    """An input file for reading; a .gz one is decompressed on the host."""
+    return gzip.open(path, "rb") if path.endswith(".gz") else open(path, "rb")
+
+
 def detect_format(path):
-    """"fasta" or "fastq" from the first byte (files.py:314-333)."""
-    with open(path, "rb") as f:
+    """"fasta" or "fastq" from the first (decompressed) byte (files.py:314-333)."""
+    with open_input(path) as f:
         return "fasta" if f.read(1) in (b">", b"#") else "fastq"
+
+
+# what zlib writes for no data: the device's member header, an empty final block, CRC and size 0
+EMPTY_GZIP = b"\x1f\x8b\x08\x00\x00\x00\x00\x00\x00\xff\x03\x00" + bytes(8)
+
+
+class OutputFile:
+    """An output file.  A .gz one receives gzip members from the device; if it gets no byte at all, close() writes one
+    empty member so that it stays a valid gzip file, as the reference does."""
+
+    def __init__(self, path):
+        self.gzip = path.endswith(".gz")
+        self.f = open(path, "wb")
+        self.written = 0
+
+    def write(self, data):
+        self.written += len(data)
+        self.f.write(data)
+
+    def close(self):
+        if self.gzip and self.written == 0:
+            self.f.write(EMPTY_GZIP)
+        self.f.close()
 
 
 def make_adapters(specs, kind, error_rate, overlap):
@@ -130,8 +168,9 @@ def check_filter_outputs(ap, args, paired, demultiplex, interleaved=False):
 
 
 def file_format(path, input_format, fasta):
-    """Format of an output file: FASTA for FASTA input, with --fasta, or for a .fasta / .fa name."""
-    return "fasta" if input_format == "fasta" or fasta or path.endswith((".fasta", ".fa")) else "fastq"
+    """Format of an output file: FASTA for FASTA input, with --fasta, or for a .fasta / .fa name (.gz behind it)."""
+    name = path[:-3] if path.endswith(".gz") else path
+    return "fasta" if input_format == "fasta" or fasta or name.endswith((".fasta", ".fa")) else "fastq"
 
 
 def main():
@@ -182,7 +221,7 @@ def main():
     max1, max2 = mate_lengths(ap, args.maximum_length, paired)
     check_filter_outputs(ap, args, paired, "{name}" in args.output, args.interleaved)
     input_format = detect_format(args.inputs[0])
-    fasta_out = input_format == "fasta" or args.fasta or args.output.endswith((".fasta", ".fa"))
+    fasta_out = file_format(args.output, input_format, args.fasta) == "fasta"
     output_format = "fasta" if fasta_out and input_format == "fastq" else None
     if input_format == "fasta" and args.max_ee is not None:
         print("WARNING: Ignoring option --max-ee because input does not provide quality values", file=sys.stderr)
@@ -205,6 +244,12 @@ def main():
     split = dict(redirect=redirect,
                  redirect_formats={d: file_format(getattr(args, d + "_output"), input_format, args.fasta)
                                    for d in redirect}) if redirect else {}
+    # the outputs compressed on the device: R1's files, R2's (an interleaved output's R2 goes to R1's file)
+    paths1 = dict({d: getattr(args, d + "_output") for d in redirect}, output=args.output)
+    paths2 = dict({d: getattr(args, d + "_paired_output") or paths1[d] for d in redirect},
+                  output=args.paired_output or args.output)
+    gzip1 = [d for d, p in paths1.items() if p.endswith(".gz")]
+    gzip2 = [d for d, p in paths2.items() if p.endswith(".gz")]
     ads1 = (make_adapters(args.back, "back", args.error_rate, args.overlap)
             + make_adapters(args.front, "front", args.error_rate, args.overlap)
             + make_adapters(args.anywhere, "anywhere", args.error_rate, args.overlap))
@@ -222,17 +267,17 @@ def main():
         interleaved = [d for d in ["output"] + redirect
                        if not (args.paired_output if d == "output" else getattr(args, d + "_paired_output"))]
         t = PairedFastqTrimmer(ads1, ads2, common, options2, args.pair_filter, **formats, **split,
-                               interleaved_outputs=interleaved)
+                               interleaved_outputs=interleaved, gzip_outputs=gzip1, gzip_outputs2=gzip2)
         if len(args.inputs) == 2:
-            f1, f2 = open(args.inputs[0], "rb"), open(args.inputs[1], "rb")
+            f1, f2 = open_input(args.inputs[0]), open_input(args.inputs[1])
             chunks = paired_reader(f1, f2, args.buffer_size)
         else:
-            f1 = f2 = open(args.inputs[0], "rb")
+            f1 = f2 = open_input(args.inputs[0])
             chunks = (read_interleaved_fasta_chunks if input_format == "fasta" else read_interleaved_fastq_chunks)(
                 f1, args.buffer_size)
         paths = {d: (getattr(args, d + "_output"), getattr(args, d + "_paired_output")) for d in redirect}
         paths["output"] = (args.output, args.paired_output)
-        files = {d: tuple(open(p, "wb") if p else None for p in ps) for d, ps in paths.items()}
+        files = {d: tuple(OutputFile(p) if p else None for p in ps) for d, ps in paths.items()}
         for parts in t.process_chunks_split(chunks):
             for name, (r1, r2) in parts.items():
                 files[name][0].write(r1)
@@ -246,9 +291,12 @@ def main():
         f2.close()
         stats = {"read1": t.statistics[0], "read2": t.statistics[1]}
     elif "{name}" in args.output:
-        t = FastqTrimmer(ads1, **common, **formats)
+        # every demultiplexed output, "unknown" included, is compressed alike
+        if args.untrimmed_output and args.untrimmed_output.endswith(".gz") != args.output.endswith(".gz"):
+            ap.error("with demultiplexing, --untrimmed-output must be compressed (.gz) exactly when the -o template is")
+        t = FastqTrimmer(ads1, **common, **formats, gzip_outputs=gzip1)
         files = {}
-        with open(args.inputs[0], "rb") as f:
+        with open_input(args.inputs[0]) as f:
             for chunk in reader(f, args.buffer_size):
                 for name, data in t.process_chunk_demux(chunk).items():
                     if name == "unknown" and args.discard_untrimmed:
@@ -257,16 +305,16 @@ def main():
                         # Demultiplexer(untrimmed_output=...): reads without a match go to --untrimmed-output
                         path = args.untrimmed_output if name == "unknown" and args.untrimmed_output else \
                             args.output.replace("{name}", name)
-                        files[name] = open(path, "wb")
+                        files[name] = OutputFile(path)
                     files[name].write(data)
         for fh in files.values():
             fh.close()
         stats = t.statistics
     elif redirect:
-        t = FastqTrimmer(ads1, **common, **formats, **split)
-        with open(args.inputs[0], "rb") as f:
-            files = {d: open(getattr(args, d + "_output"), "wb") for d in redirect}
-            files["output"] = open(args.output, "wb")
+        t = FastqTrimmer(ads1, **common, **formats, **split, gzip_outputs=gzip1)
+        with open_input(args.inputs[0]) as f:
+            files = {d: OutputFile(getattr(args, d + "_output")) for d in redirect}
+            files["output"] = OutputFile(args.output)
             for parts in t.process_chunks_split(reader(f, args.buffer_size), copy=False):
                 for name, data in parts.items():
                     files[name].write(data)
@@ -274,10 +322,12 @@ def main():
                 fh.close()
         stats = t.statistics
     else:
-        t = FastqTrimmer(ads1, **common, **formats)
-        with open(args.inputs[0], "rb") as f, open(args.output, "wb") as o:
+        t = FastqTrimmer(ads1, **common, **formats, gzip_outputs=gzip1)
+        o = OutputFile(args.output)
+        with open_input(args.inputs[0]) as f:
             for out in t.process_chunks(reader(f, args.buffer_size), copy=False):
                 o.write(out.tobytes() if hasattr(out, "tobytes") else out)
+        o.close()
         stats = t.statistics
     print(json.dumps(stats), file=sys.stderr)
     if args.json is not None:
