@@ -150,6 +150,11 @@ class cg_fastq_result(C.Structure):
                 if name != "reserved" and (plain_bytes or name != "out_bytes_plain")}
 
 
+class cg_gzin_result(C.Structure):
+    _fields_ = [(name, C.c_int64) for name in (
+        "consumed", "members", "plain_bytes", "chunk_bytes", "carry_bytes", "n_records")] + [("reserved", C.c_int64 * 2)]
+
+
 MATCH_DTYPE = np.dtype(
     [
         ("adapter", "<i4"),
@@ -211,6 +216,14 @@ def _declare(lib) -> None:
                                                   C.POINTER(cg_fastq_params), i32, i32, i32, vp, i64, vp, i64,
                                                   C.POINTER(cg_fastq_result), C.POINTER(cg_fastq_result), vp, vp]
     lib.cg_fastq_submit_interleaved.argtypes = [vp, vp, i64, i32, C.POINTER(i32), C.POINTER(i32)]
+    lib.cg_gzin_create.argtypes = [vp, C.POINTER(i32)]
+    lib.cg_fastq_slot_read.argtypes = [vp, i32, vp, i64, C.POINTER(i64)]
+    lib.cg_gzin_destroy.argtypes = [vp, i32]
+    lib.cg_fastq_submit_gzip.argtypes = [vp, i32, vp, i64, i32, i32, C.POINTER(i32), C.POINTER(cg_gzin_result)]
+    lib.cg_fastq_submit_gzip_paired.argtypes = [vp, i32, i32, vp, i64, vp, i64, i32, i32, C.POINTER(i32), C.POINTER(i32),
+                                                C.POINTER(cg_gzin_result), C.POINTER(cg_gzin_result)]
+    lib.cg_fastq_submit_gzip_interleaved.argtypes = [vp, i32, vp, i64, i32, i32, C.POINTER(i32), C.POINTER(i32),
+                                                     C.POINTER(cg_gzin_result)]
     lib.cg_fastq_collect_paired_interleaved.argtypes = [vp, i32, i32, vp, vp, C.POINTER(cg_fastq_params),
                                                         C.POINTER(cg_fastq_params), i32, i32, i32, i32, vp, i64, vp, i64,
                                                         C.POINTER(cg_fastq_result), C.POINTER(cg_fastq_result), vp, vp]

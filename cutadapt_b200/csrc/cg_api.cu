@@ -144,6 +144,30 @@ struct FastqSlot {
     PinBuf<unsigned long long> h_counters;
 };
 
+// A gzip input stream (cg_gzin_create): the carry in d_plain[0, carry) and the scratch of the submissions
+struct GzinStream {
+    DevBuf<uint8_t> d_gz, d_plain;
+    PinBuf<uint8_t> h_gz;
+    DevBuf<int32_t> d_counts, d_cand, d_members, d_flag;
+    DevBuf<int64_t> d_offs;
+    DevBuf<GuMember> d_res;
+    DevBuf<long long> d_moff;
+    DevBuf<unsigned long long> d_scan, d_small;  // d_small: newline total, cut, first bad member, chain
+    DevBuf<uint32_t> d_tiles, d_nl;
+    cudaEvent_t done = nullptr;                  // the last submission's work on the stream's buffers
+    long long carry = 0, consumed = 0, members = 0;
+    // the submission in progress, committed once its slots are known: plain bytes behind the carry, bytes and members
+    long long pend_plain = 0, pend_consumed = 0, pend_members = 0;
+    void release()
+    {
+        d_gz.release(); d_plain.release(); h_gz.release(); d_counts.release(); d_cand.release(); d_members.release();
+        d_flag.release(); d_offs.release(); d_res.release(); d_moff.release(); d_scan.release(); d_small.release();
+        d_tiles.release(); d_nl.release();
+        if (done) cudaEventDestroy(done);
+        done = nullptr;
+    }
+};
+
 // A statistics accumulator of the FASTQ path (cg_fastq_stats_create): the vector of cg_fastq_stats_read at
 // (n_adapters, max_len, kmax); both sizes grow when a chunk needs more.
 struct FqStatsAcc {
@@ -200,6 +224,8 @@ struct cg_ctx {
     int fq_next = 0;
     std::map<int32_t, FqStatsAcc> fq_stats;      // cg_fastq_stats_* by handle
     int32_t fq_stats_next = 1;
+    std::map<int32_t, GzinStream> gzin;          // cg_gzin_* by handle
+    int32_t gzin_next = 1;
 };
 
 struct cg_adapterset {
@@ -313,6 +339,7 @@ extern "C" int cg_ctx_destroy(cg_ctx *c)
         if (f.d_err) cudaFree(f.d_err);
         if (f.stream) cudaStreamDestroy(f.stream);
     }
+    for (auto &kv : c->gzin) kv.second.release();
     if (c->scratch_ev) cudaEventDestroy(c->scratch_ev);
     if (c->d_task_count) cudaFree(c->d_task_count);
     if (c->d_err) cudaFree(c->d_err);
@@ -1639,8 +1666,8 @@ static int fastq_format_error(const int err[2], int mate = 0)
                                (mate ? " of the interleaved chunk: " : ": ") + what[err[0] & 7]);
 }
 
-// Streams, counters and error words of a slot, the host pool; the upload of the chunk and its newline count
-static int fastq_slot_upload(cg_ctx *c, FastqSlot &f, const uint8_t *fastq, int64_t n_bytes)
+// Streams, counters and error words of a slot, the host pool
+static int fastq_slot_init(cg_ctx *c, FastqSlot &f)
 {
     f.ilv = 0;
     if (!f.stream) CU(cudaStreamCreateWithFlags(&f.stream, cudaStreamNonBlocking));
@@ -1651,13 +1678,33 @@ static int fastq_slot_upload(cg_ctx *c, FastqSlot &f, const uint8_t *fastq, int6
         c->exc_scratch.resize((size_t)c->pool->size());
     }
     int rc;
-    if ((rc = f.d_in.ensure((size_t)n_bytes + 64)) != CG_OK) return rc;
-    if ((rc = f.d_tiles.ensure((size_t)cg_fastq_tiles(n_bytes) + 1)) != CG_OK) return rc;
     if ((rc = f.h_counters.ensure(1 + CG_FQ_COUNTERS)) != CG_OK) return rc;
-    f.n_bytes = n_bytes;
     CU(cudaMemsetAsync(f.d_counters, 0, (1 + CG_FQ_COUNTERS) * sizeof(unsigned long long), f.stream));
     const int err_init[2] = {0, 0x7FFFFFFF};
     CU(cudaMemcpyAsync(f.d_err, err_init, sizeof err_init, cudaMemcpyHostToDevice, f.stream));
+    return CG_OK;
+}
+
+// The newline count of the chunk in f.d_in[0, n_bytes)
+static int fastq_slot_count(cg_ctx *c, FastqSlot &f, int64_t n_bytes)
+{
+    int rc;
+    if ((rc = f.d_tiles.ensure((size_t)cg_fastq_tiles(n_bytes) + 1)) != CG_OK) return rc;
+    f.n_bytes = n_bytes;
+    if (n_bytes) {
+        CU(cg_launch_fastq_index(f.d_in.p, n_bytes, f.d_tiles.p, f.d_counters, nullptr, 0, f.stream));
+        c->launches += 2;
+    }
+    CU(cudaMemcpyAsync(f.h_counters.p, f.d_counters, sizeof(unsigned long long), cudaMemcpyDeviceToHost, f.stream));
+    return CG_OK;
+}
+
+// init, the upload of the chunk and its newline count
+static int fastq_slot_upload(cg_ctx *c, FastqSlot &f, const uint8_t *fastq, int64_t n_bytes)
+{
+    int rc;
+    if ((rc = fastq_slot_init(c, f)) != CG_OK) return rc;
+    if ((rc = f.d_in.ensure((size_t)n_bytes + 64)) != CG_OK) return rc;
     if (n_bytes) {
         const uint8_t *src = fastq;
         if (!is_pinned(fastq)) {
@@ -1667,11 +1714,8 @@ static int fastq_slot_upload(cg_ctx *c, FastqSlot &f, const uint8_t *fastq, int6
         }
         CU(cudaMemcpyAsync(f.d_in.p, src, (size_t)n_bytes, cudaMemcpyHostToDevice, f.stream));
         c->h2d_bytes += n_bytes;
-        CU(cg_launch_fastq_index(f.d_in.p, n_bytes, f.d_tiles.p, f.d_counters, nullptr, 0, f.stream));
-        c->launches += 2;
     }
-    CU(cudaMemcpyAsync(f.h_counters.p, f.d_counters, sizeof(unsigned long long), cudaMemcpyDeviceToHost, f.stream));
-    return CG_OK;
+    return fastq_slot_count(c, f, n_bytes);
 }
 
 extern "C" int cg_fastq_submit(cg_ctx *c, const uint8_t *fastq, int64_t n_bytes, int32_t *slot_out)
@@ -1710,6 +1754,370 @@ extern "C" int cg_fastq_submit_interleaved(cg_ctx *c, const uint8_t *chunk, int6
     f2.ilv = 2; f2.ilv_peer = s1;
     f1.ilv_format = f2.ilv_format = format == CG_FORMAT_FASTA ? CG_FORMAT_FASTA : CG_FORMAT_FASTQ;
     f1.busy = f2.busy = true;
+    *slot1 = s1;
+    *slot2 = s2;
+    return CG_OK;
+}
+
+// ------------------------------------------------------------------------------------------
+// gzip input (cg_fastq_submit_gzip*): the compressed bytes are uploaded, their members inflated on the device
+// (cg_gunzip.cu) behind the stream's carry, and the longest prefix of whole records becomes a slot's chunk.  Small
+// readbacks per file and submission size the buffers and decide: the candidate count, the chain, the first bad CRC, the
+// newline count, the flagged-newline count and the cut.  Everything runs on the stream of the slot the submission
+// reserved.
+// ------------------------------------------------------------------------------------------
+#define CG_GZIN_LIMIT (1LL << 31)        // plain bytes of one submission stay under the slot limit
+
+extern "C" int cg_gzin_create(cg_ctx *c, int32_t *handle)
+{
+    if (!c || !handle) return fail(CG_EINVAL, "cg_gzin_create: bad argument");
+    CU(cudaSetDevice(c->device));
+    const int32_t h = c->gzin_next++;
+    GzinStream &g = c->gzin[h];
+    int rc;
+    if ((rc = g.d_small.ensure(4 + (sizeof(GuChain) + 7) / 8)) != CG_OK) { c->gzin.erase(h); return rc; }
+    CU(cudaEventCreateWithFlags(&g.done, cudaEventDisableTiming));
+    *handle = h;
+    return CG_OK;
+}
+
+extern "C" int cg_gzin_destroy(cg_ctx *c, int32_t handle)
+{
+    if (!c) return fail(CG_EINVAL, "cg_gzin_destroy: bad argument");
+    auto it = c->gzin.find(handle);
+    if (it == c->gzin.end()) return fail(CG_EINVAL, "cg_gzin_destroy: unknown handle");
+    CU(cudaSetDevice(c->device));
+    if (it->second.done) CU(cudaEventSynchronize(it->second.done));
+    it->second.release();
+    c->gzin.erase(it);
+    return CG_OK;
+}
+
+// Upload gz[0, n), inflate the chain of whole members behind the carry (not committed yet).  *fin: final and every byte
+// consumed.
+static int gzin_inflate(cg_ctx *c, GzinStream &g, const uint8_t *gz, int64_t n, bool final, cudaStream_t st,
+                        cg_gzin_result *res, bool *fin)
+{
+    int rc;
+    CU(cudaStreamWaitEvent(st, g.done, 0));
+    if ((rc = g.d_gz.ensure((size_t)n + 16)) != CG_OK) return rc;
+    if (n) {
+        if ((rc = g.h_gz.ensure((size_t)n)) != CG_OK) return rc;
+        parallel_copy(c, g.h_gz.p, gz, (size_t)n);
+        CU(cudaMemcpyAsync(g.d_gz.p, g.h_gz.p, (size_t)n, cudaMemcpyHostToDevice, st));
+        c->h2d_bytes += n;
+    }
+    const long long tiles = cg_gunzip_tiles(n);
+    if ((rc = g.d_counts.ensure((size_t)tiles + 1)) != CG_OK) return rc;
+    if ((rc = g.d_offs.ensure((size_t)tiles + 1)) != CG_OK) return rc;
+    if ((rc = g.d_scan.ensure((size_t)cg_scan_tiles(tiles) + 1)) != CG_OK) return rc;
+    int64_t n_cand = 0;
+    if (tiles) {
+        CU(cg_launch_gunzip_candidates(0, g.d_gz.p, n, g.d_counts.p, nullptr, nullptr, st));
+        CU(cg_launch_scan_i32(g.d_counts.p, tiles, g.d_scan.p, g.d_offs.p, st));
+        CU(cudaMemcpyAsync(&n_cand, g.d_offs.p + tiles, sizeof n_cand, cudaMemcpyDeviceToHost, st));
+        CU(cudaStreamSynchronize(st));
+        c->launches += 3;
+    }
+    if ((rc = g.d_cand.ensure((size_t)n_cand + 1)) != CG_OK) return rc;
+    if ((rc = g.d_res.ensure((size_t)n_cand + 1)) != CG_OK) return rc;
+    if ((rc = g.d_members.ensure((size_t)n_cand + 1)) != CG_OK) return rc;
+    if ((rc = g.d_moff.ensure((size_t)n_cand + 1)) != CG_OK) return rc;
+    GuChain *d_chain = reinterpret_cast<GuChain *>(g.d_small.p + 4);
+    if (n_cand) {
+        CU(cg_launch_gunzip_candidates(1, g.d_gz.p, n, nullptr, g.d_offs.p, g.d_cand.p, st));
+        CU(cg_launch_gunzip_parse(g.d_gz.p, n, g.d_cand.p, (int)n_cand, g.d_res.p, st));
+        c->launches += 2;
+    }
+    CU(cg_launch_gunzip_chain(g.d_gz.p, n, g.d_cand.p, g.d_res.p, (int)n_cand, g.members > 0, final, g.carry,
+                              CG_GZIN_LIMIT, g.d_members.p, g.d_moff.p, d_chain, st));
+    c->launches += 1;
+    GuChain ch;
+    CU(cudaMemcpyAsync(&ch, d_chain, sizeof ch, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    const long long at = g.consumed + ch.err_at;
+    if (ch.status == GU_INVALID)
+        return fail(CG_EINVAL, "gzip input: invalid or truncated gzip member at byte " + std::to_string(at) +
+                                   " of the compressed file");
+    if (ch.status == GU_UNSUPPORTED)
+        return fail(CG_EUNSUPPORTED, "gzip input: the member at byte " + std::to_string(at) +
+                                         " inflates to more than one submission can hold (2 GiB); decompress this input "
+                                         "on the host");
+    // the carry stays where it is; a larger buffer gets a copy of it
+    const long long total = g.carry + ch.plain;
+    if ((size_t)total + 64 > g.d_plain.cap) {
+        DevBuf<uint8_t> nb;
+        if ((rc = nb.ensure((size_t)total + 64)) != CG_OK) return rc;
+        if (g.carry) CU(cudaMemcpyAsync(nb.p, g.d_plain.p, (size_t)g.carry, cudaMemcpyDeviceToDevice, st));
+        CU(cudaStreamSynchronize(st));
+        g.d_plain.release();
+        g.d_plain = nb;
+    }
+    if (ch.n_members) {
+        int *d_bad = reinterpret_cast<int *>(g.d_small.p + 2);
+        const int none = 0x7FFFFFFF;
+        CU(cudaMemcpyAsync(d_bad, &none, sizeof none, cudaMemcpyHostToDevice, st));
+        CU(cg_launch_gunzip_place(g.d_gz.p, n, g.d_cand.p, g.d_members.p, g.d_moff.p, d_chain, ch.n_members, g.d_res.p,
+                                  g.d_plain.p, d_bad, st));
+        c->launches += 2;
+        int bad = none;
+        CU(cudaMemcpyAsync(&bad, d_bad, sizeof bad, cudaMemcpyDeviceToHost, st));
+        CU(cudaStreamSynchronize(st));
+        if (bad != none) {
+            int32_t k = 0, pos = 0;
+            CU(cudaMemcpy(&k, g.d_members.p + bad, sizeof k, cudaMemcpyDeviceToHost));
+            CU(cudaMemcpy(&pos, g.d_cand.p + k, sizeof pos, cudaMemcpyDeviceToHost));
+            return fail(CG_EINVAL, "gzip input: CRC-32 mismatch in the gzip member at byte " +
+                                       std::to_string(g.consumed + pos) + " of the compressed file");
+        }
+    }
+    g.pend_plain = ch.plain;
+    g.pend_consumed = ch.consumed;
+    g.pend_members = ch.n_members;
+    res->consumed = ch.consumed;
+    res->members = ch.n_members;
+    res->plain_bytes = ch.plain;
+    *fin = final && ch.consumed == n;
+    return CG_OK;
+}
+
+// The flagged newlines of the carry plus the new plain bytes (gu_flag): their number *F, whether the buffer starts
+// with '>', whether it ends in a newline; the line index and the flags' scan stay in g for gzin_cut.
+struct GzinCount {
+    long long total = 0, n_nl = 0, F = 0;
+    int b0 = 0, nl_end = 1, fasta = 0;
+};
+
+static int gzin_count(cg_ctx *c, GzinStream &g, int fasta, cudaStream_t st, GzinCount *k)
+{
+    k->total = g.carry + g.pend_plain;
+    k->fasta = fasta;
+    if (!k->total) return CG_OK;
+    int rc;
+    if ((rc = g.d_tiles.ensure((size_t)cg_fastq_tiles(k->total) + 1)) != CG_OK) return rc;
+    CU(cg_launch_fastq_index(g.d_plain.p, k->total, g.d_tiles.p, g.d_small.p, nullptr, 0, st));
+    uint8_t ends[2];
+    CU(cudaMemcpyAsync(&k->n_nl, g.d_small.p, sizeof k->n_nl, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(&ends[0], g.d_plain.p, 1, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(&ends[1], g.d_plain.p + k->total - 1, 1, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    c->launches += 2;
+    k->b0 = ends[0] == '>';
+    k->nl_end = ends[1] == '\n';
+    const long long L = k->n_nl;
+    if (!L) return CG_OK;
+    if ((rc = g.d_nl.ensure((size_t)L + 1)) != CG_OK) return rc;
+    if ((rc = g.d_flag.ensure((size_t)L + 1)) != CG_OK) return rc;
+    if ((rc = g.d_offs.ensure((size_t)L + 1)) != CG_OK) return rc;
+    if ((rc = g.d_scan.ensure((size_t)cg_scan_tiles(L) + 1)) != CG_OK) return rc;
+    CU(cg_launch_fastq_index(g.d_plain.p, k->total, g.d_tiles.p, nullptr, g.d_nl.p, 1, st));
+    CU(cg_launch_gunzip_flags(g.d_plain.p, k->total, g.d_nl.p, L, fasta, g.d_flag.p, st));
+    CU(cg_launch_scan_i32(g.d_flag.p, L, g.d_scan.p, g.d_offs.p, st));
+    CU(cudaMemcpyAsync(&k->F, g.d_offs.p + L, sizeof k->F, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    c->launches += 4;
+    return CG_OK;
+}
+
+// the offset behind flagged newline s (s < 0: 0); *n_records: the records in front of it
+static int gzin_cut(cg_ctx *c, GzinStream &g, const GzinCount &k, long long s, cudaStream_t st, long long *cut,
+                    long long *n_records)
+{
+    *cut = 0;
+    *n_records = 0;
+    if (s < 0) return CG_OK;
+    long long *d_cut = reinterpret_cast<long long *>(g.d_small.p + 1);
+    CU(cg_launch_gunzip_select(g.d_nl.p, k.n_nl, g.d_flag.p, g.d_offs.p, s, d_cut, st));
+    CU(cudaMemcpyAsync(cut, d_cut, sizeof *cut, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    c->launches += 1;
+    *n_records = k.fasta ? k.b0 + s : (s + 1) / 4;
+    return CG_OK;
+}
+
+// final: the whole buffer is the chunk
+static void gzin_all(const GzinCount &k, long long *cut, long long *n_records)
+{
+    *cut = k.total;
+    *n_records = k.fasta ? k.b0 + k.F : (k.n_nl + (k.total && !k.nl_end ? 1 : 0)) / 4;
+}
+
+// Commit the submission: the chunk [0, cut) goes to slot f (f == nullptr: cut must be 0), the rest becomes the carry.
+// The slot takes the stream's buffer; the rest is copied into the slot's old one, which the stream keeps.
+static int gzin_commit(cg_ctx *c, GzinStream &g, FastqSlot *f, long long cut, long long n_records, cudaStream_t st,
+                       cg_gzin_result *res)
+{
+    const long long total = g.carry + g.pend_plain;
+    int rc;
+    if (f && cut) {
+        std::swap(g.d_plain, f->d_in);
+        const long long rest = total - cut;
+        if ((rc = g.d_plain.ensure((size_t)rest + 64)) != CG_OK) return rc;
+        if (rest) CU(cudaMemcpyAsync(g.d_plain.p, f->d_in.p + cut, (size_t)rest, cudaMemcpyDeviceToDevice, st));
+        if ((rc = fastq_slot_count(c, *f, cut)) != CG_OK) return rc;
+        g.carry = rest;
+    } else {
+        g.carry = total;
+    }
+    g.consumed += g.pend_consumed;
+    g.members += g.pend_members;
+    g.pend_plain = g.pend_consumed = g.pend_members = 0;
+    CU(cudaEventRecord(g.done, st));
+    res->chunk_bytes = f ? cut : 0;
+    res->carry_bytes = g.carry;
+    res->n_records = f ? n_records : 0;
+    return CG_OK;
+}
+
+static GzinStream *gzin_lookup(cg_ctx *c, int32_t handle)
+{
+    auto it = c->gzin.find(handle);
+    return it == c->gzin.end() ? nullptr : &it->second;
+}
+
+extern "C" int cg_fastq_submit_gzip(cg_ctx *c, int32_t handle, const uint8_t *gz, int64_t n_bytes, int32_t format,
+                                    int32_t final, int32_t *slot, cg_gzin_result *res)
+{
+    if (!c || !slot || !res || n_bytes < 0 || (n_bytes && !gz) || format < CG_FORMAT_FASTQ ||
+        format > CG_FORMAT_FASTQ_TO_FASTA)
+        return fail(CG_EINVAL, "cg_fastq_submit_gzip: bad argument");
+    if (n_bytes >= (1LL << 31)) return fail(CG_EINVAL, "cg_fastq_submit_gzip: a submission must be smaller than 2 GiB");
+    GzinStream *g = gzin_lookup(c, handle);
+    if (!g) return fail(CG_EINVAL, "cg_fastq_submit_gzip: unknown handle");
+    CU(cudaSetDevice(c->device));
+    *slot = -1;
+    memset(res, 0, sizeof *res);
+    const int si = c->fq_next;
+    FastqSlot &f = c->fq[si];
+    if (f.busy) return fail(CG_EINVAL, "cg_fastq_submit_gzip: all slots are in flight, collect one first");
+    int rc;
+    bool fin = false;
+    if ((rc = fastq_slot_init(c, f)) != CG_OK) return rc;
+    if ((rc = gzin_inflate(c, *g, gz, n_bytes, final != 0, f.stream, res, &fin)) != CG_OK) return rc;
+    GzinCount k;
+    if ((rc = gzin_count(c, *g, format == CG_FORMAT_FASTA, f.stream, &k)) != CG_OK) return rc;
+    long long cut, n_records;
+    if (fin) gzin_all(k, &cut, &n_records);
+    else if ((rc = gzin_cut(c, *g, k, gu_select_single(k.fasta, k.F, k.b0, 0), f.stream, &cut, &n_records)) != CG_OK)
+        return rc;
+    if ((rc = gzin_commit(c, *g, cut ? &f : nullptr, cut, n_records, f.stream, res)) != CG_OK) return rc;
+    if (cut) {
+        c->fq_next = (si + 1) % CG_FQ_SLOTS;
+        f.busy = true;
+        *slot = si;
+    }
+    return CG_OK;
+}
+
+extern "C" int cg_fastq_slot_read(cg_ctx *c, int32_t slot, uint8_t *dst, int64_t capacity, int64_t *n_bytes)
+{
+    if (!c || !n_bytes || slot < 0 || slot >= CG_FQ_SLOTS || capacity < 0 || (capacity && !dst))
+        return fail(CG_EINVAL, "cg_fastq_slot_read: bad argument");
+    FastqSlot &f = c->fq[slot];
+    if (!f.busy || f.ilv) return fail(CG_EINVAL, "cg_fastq_slot_read: the slot holds no chunk of its own");
+    CU(cudaSetDevice(c->device));
+    *n_bytes = f.n_bytes;
+    if (capacity < f.n_bytes) return fail(CG_EINVAL, "cg_fastq_slot_read: buffer too small");
+    if (f.n_bytes) CU(cudaMemcpyAsync(dst, f.d_in.p, (size_t)f.n_bytes, cudaMemcpyDeviceToHost, f.stream));
+    CU(cudaStreamSynchronize(f.stream));
+    c->d2h_bytes += f.n_bytes;
+    return CG_OK;
+}
+
+extern "C" int cg_fastq_submit_gzip_interleaved(cg_ctx *c, int32_t handle, const uint8_t *gz, int64_t n_bytes,
+                                                int32_t format, int32_t final, int32_t *slot1, int32_t *slot2,
+                                                cg_gzin_result *res)
+{
+    if (!c || !slot1 || !slot2 || !res || n_bytes < 0 || (n_bytes && !gz) || format < CG_FORMAT_FASTQ ||
+        format > CG_FORMAT_FASTQ_TO_FASTA)
+        return fail(CG_EINVAL, "cg_fastq_submit_gzip_interleaved: bad argument");
+    if (n_bytes >= (1LL << 31))
+        return fail(CG_EINVAL, "cg_fastq_submit_gzip_interleaved: a submission must be smaller than 2 GiB");
+    GzinStream *g = gzin_lookup(c, handle);
+    if (!g) return fail(CG_EINVAL, "cg_fastq_submit_gzip_interleaved: unknown handle");
+    CU(cudaSetDevice(c->device));
+    *slot1 = *slot2 = -1;
+    memset(res, 0, sizeof *res);
+    const int s1 = c->fq_next, s2 = (s1 + 1) % CG_FQ_SLOTS;
+    FastqSlot &f1 = c->fq[s1], &f2 = c->fq[s2];
+    if (f1.busy || f2.busy)
+        return fail(CG_EINVAL, "cg_fastq_submit_gzip_interleaved: two free slots are needed, collect one first");
+    int rc;
+    bool fin = false;
+    if ((rc = fastq_slot_init(c, f1)) != CG_OK) return rc;
+    if ((rc = gzin_inflate(c, *g, gz, n_bytes, final != 0, f1.stream, res, &fin)) != CG_OK) return rc;
+    GzinCount k;
+    if ((rc = gzin_count(c, *g, format == CG_FORMAT_FASTA, f1.stream, &k)) != CG_OK) return rc;
+    long long cut, n_records;
+    if (fin) gzin_all(k, &cut, &n_records);
+    else if ((rc = gzin_cut(c, *g, k, gu_select_single(k.fasta, k.F, k.b0, 1), f1.stream, &cut, &n_records)) != CG_OK)
+        return rc;
+    if ((rc = gzin_commit(c, *g, cut ? &f1 : nullptr, cut, n_records, f1.stream, res)) != CG_OK) return rc;
+    if (!cut) return CG_OK;
+    if ((rc = fastq_slot_init(c, f2)) != CG_OK) return rc;          // its chunk comes from the split
+    if ((rc = fastq_slot_count(c, f2, 0)) != CG_OK) return rc;
+    f1.ilv = 1; f1.ilv_peer = s2;
+    f2.ilv = 2; f2.ilv_peer = s1;
+    f1.ilv_format = f2.ilv_format = format == CG_FORMAT_FASTA ? CG_FORMAT_FASTA : CG_FORMAT_FASTQ;
+    f1.busy = f2.busy = true;
+    c->fq_next = (s2 + 1) % CG_FQ_SLOTS;
+    *slot1 = s1;
+    *slot2 = s2;
+    return CG_OK;
+}
+
+extern "C" int cg_fastq_submit_gzip_paired(cg_ctx *c, int32_t handle1, int32_t handle2, const uint8_t *gz1,
+                                           int64_t n_bytes1, const uint8_t *gz2, int64_t n_bytes2, int32_t format,
+                                           int32_t final, int32_t *slot1, int32_t *slot2, cg_gzin_result *res1,
+                                           cg_gzin_result *res2)
+{
+    if (!c || !slot1 || !slot2 || !res1 || !res2 || n_bytes1 < 0 || n_bytes2 < 0 || (n_bytes1 && !gz1) ||
+        (n_bytes2 && !gz2) || format < CG_FORMAT_FASTQ || format > CG_FORMAT_FASTQ_TO_FASTA || handle1 == handle2)
+        return fail(CG_EINVAL, "cg_fastq_submit_gzip_paired: bad argument");
+    if (n_bytes1 >= (1LL << 31) || n_bytes2 >= (1LL << 31))
+        return fail(CG_EINVAL, "cg_fastq_submit_gzip_paired: a submission must be smaller than 2 GiB");
+    GzinStream *g1 = gzin_lookup(c, handle1), *g2 = gzin_lookup(c, handle2);
+    if (!g1 || !g2) return fail(CG_EINVAL, "cg_fastq_submit_gzip_paired: unknown handle");
+    CU(cudaSetDevice(c->device));
+    *slot1 = *slot2 = -1;
+    memset(res1, 0, sizeof *res1);
+    memset(res2, 0, sizeof *res2);
+    const int s1 = c->fq_next, s2 = (s1 + 1) % CG_FQ_SLOTS;
+    FastqSlot &f1 = c->fq[s1], &f2 = c->fq[s2];
+    if (f1.busy || f2.busy)
+        return fail(CG_EINVAL, "cg_fastq_submit_gzip_paired: two free slots are needed, collect one first");
+    int rc;
+    bool fin1 = false, fin2 = false;
+    if ((rc = fastq_slot_init(c, f1)) != CG_OK) return rc;
+    if ((rc = fastq_slot_init(c, f2)) != CG_OK) return rc;
+    if ((rc = gzin_inflate(c, *g1, gz1, n_bytes1, final != 0, f1.stream, res1, &fin1)) != CG_OK)
+        return fail(rc, "mate 1 (first input): " + g_err);
+    if ((rc = gzin_inflate(c, *g2, gz2, n_bytes2, final != 0, f2.stream, res2, &fin2)) != CG_OK)
+        return fail(rc, "mate 2 (second input): " + g_err);
+    const int fasta = format == CG_FORMAT_FASTA;
+    GzinCount k1, k2;
+    if ((rc = gzin_count(c, *g1, fasta, f1.stream, &k1)) != CG_OK) return rc;
+    if ((rc = gzin_count(c, *g2, fasta, f2.stream, &k2)) != CG_OK) return rc;
+    long long cut1, cut2, n1, n2;
+    if (fin1 && fin2) {
+        gzin_all(k1, &cut1, &n1);
+        gzin_all(k2, &cut2, &n2);
+    } else {
+        const long long r = std::min(gu_records(fasta, k1.F, k1.b0), gu_records(fasta, k2.F, k2.b0));
+        const long long sel1 = r > 0 ? gu_select_records(fasta, r, k1.b0) : -1;
+        const long long sel2 = r > 0 ? gu_select_records(fasta, r, k2.b0) : -1;
+        if ((rc = gzin_cut(c, *g1, k1, sel1, f1.stream, &cut1, &n1)) != CG_OK) return rc;
+        if ((rc = gzin_cut(c, *g2, k2, sel2, f2.stream, &cut2, &n2)) != CG_OK) return rc;
+    }
+    const bool take = cut1 || cut2;
+    if ((rc = gzin_commit(c, *g1, take ? &f1 : nullptr, cut1, n1, f1.stream, res1)) != CG_OK) return rc;
+    if ((rc = gzin_commit(c, *g2, take ? &f2 : nullptr, cut2, n2, f2.stream, res2)) != CG_OK) return rc;
+    if (!take) return CG_OK;
+    // a mate without bytes (the other file's last records) gets an empty chunk
+    if (!cut1 && (rc = fastq_slot_count(c, f1, 0)) != CG_OK) return rc;
+    if (!cut2 && (rc = fastq_slot_count(c, f2, 0)) != CG_OK) return rc;
+    f1.busy = f2.busy = true;
+    c->fq_next = (s2 + 1) % CG_FQ_SLOTS;
     *slot1 = s1;
     *slot2 = s2;
     return CG_OK;

@@ -202,6 +202,27 @@ cudaError_t cg_launch_gzip_compress(const uint8_t *d_src, const CgGzPiece *d_pie
                                     int32_t *d_sizes, cudaStream_t st);
 cudaError_t cg_launch_gzip_gather(const uint8_t *d_slots, const int32_t *d_sizes, const int64_t *d_dst_off, int n_pieces,
                                   uint8_t *d_out, cudaStream_t st);
+// gzip input (cg_gunzip.cu, decisions in cg_gunzip_core.cuh): phase 0 counts the positions of 1f 8b 08 per tile of
+// cg_gunzip_tiles, phase 1 (after an exclusive scan of the counts) writes them in order; parse every candidate (no
+// output); the chain (one thread); inflate the chain's members into d_out + their offsets and check their CRC-32
+// (*d_bad: the first bad member, start it at INT_MAX).  Record cut: flag the newlines of the line index (gu_flag); after
+// an exclusive scan of the flags, the select writes the offset behind flagged newline number s to *d_cut.
+#include "cg_gunzip_core.cuh"
+long long cg_gunzip_tiles(long long n_bytes);
+cudaError_t cg_launch_gunzip_candidates(int phase, const uint8_t *d_gz, long long n, int32_t *d_counts,
+                                        const int64_t *d_offs, int32_t *d_cand, cudaStream_t st);
+cudaError_t cg_launch_gunzip_parse(const uint8_t *d_gz, long long n, const int32_t *d_cand, int n_cand, GuMember *d_res,
+                                   cudaStream_t st);
+cudaError_t cg_launch_gunzip_chain(const uint8_t *d_gz, long long n, const int32_t *d_cand, const GuMember *d_res,
+                                   int n_cand, int after_member, int final, long long base, long long limit,
+                                   int32_t *d_members, long long *d_moff, GuChain *d_chain, cudaStream_t st);
+cudaError_t cg_launch_gunzip_place(const uint8_t *d_gz, long long n, const int32_t *d_cand, const int32_t *d_members,
+                                   const long long *d_moff, const GuChain *d_chain, int n_members, const GuMember *d_res,
+                                   uint8_t *d_out, int *d_bad, cudaStream_t st);
+cudaError_t cg_launch_gunzip_flags(const uint8_t *d_buf, long long n, const uint32_t *d_nl, long long n_nl, int fasta,
+                                   int32_t *d_flag, cudaStream_t st);
+cudaError_t cg_launch_gunzip_select(const uint32_t *d_nl, long long n_nl, const int32_t *d_flag, const int64_t *d_offs,
+                                    long long s, long long *d_cut, cudaStream_t st);
 // --pair-adapters: fold the records of adapter pair `pair` into the best pair per read (modifiers.py:480-503)
 cudaError_t cg_launch_fastq_pair_select(long long n_records, int pair, const cg_match_rec *d_cur1, int slots1,
                                         const cg_match_rec *d_cur2, int slots2, cg_match_rec *d_best1, cg_match_rec *d_best2,

@@ -814,6 +814,126 @@ def read_paired_fasta_chunks(f1, f2, buffer_size: int = 4 * 1024 * 1024):
         yield bytes(bufs[0][:starts[0]]), bytes(bufs[1][:starts[1]])
 
 
+class DeviceChunk:
+    """A chunk that a device gzip reader (read_gzip_device_chunks and its paired / interleaved twins) has already
+    submitted: its plain bytes are in ``slot`` of the trimmer's context (``slot2``: mate 2 of an interleaved chunk).
+    The trimmers' chunk methods take it in place of bytes; ``size`` / ``len()`` is its plain size."""
+
+    def __init__(self, slot: int, size: int, slot2: int = -1):
+        self.slot, self.size, self.slot2 = slot, size, slot2
+
+    def __len__(self) -> int:
+        return self.size
+
+
+class _GzipInput:
+    """One compressed input file on a context (cg_gzin_create): the bytes read but not yet consumed, and the carry."""
+
+    def __init__(self, ctx, f, buffer_size: int):
+        h = C.c_int32(0)
+        _lib.check(_lib.lib().cg_gzin_create(ctx.handle, C.byref(h)))
+        self.ctx, self.handle, self.f = ctx, h.value, f
+        self.buf, self.end, self.eof = bytearray(buffer_size), 0, False
+
+    def fill(self):
+        """Read more of the file; the buffer doubles when it is full (nothing consumed from a whole buffer)."""
+        if self.eof:
+            return
+        if self.end == len(self.buf):
+            self.buf.extend(bytes(len(self.buf)))
+        n = self.f.readinto(memoryview(self.buf)[self.end:])
+        self.eof = not n
+        self.end += n or 0
+
+    def pointer(self):
+        a = np.frombuffer(self.buf, dtype=np.uint8)
+        return a.ctypes.data if self.end else None
+
+    def consume(self, n: int):
+        self.buf[0:self.end - n] = self.buf[n:self.end]
+        self.end -= n
+
+    @property
+    def done(self) -> bool:
+        return self.eof and self.end == 0
+
+    def close(self):
+        if self.handle:
+            _lib.check(_lib.lib().cg_gzin_destroy(self.ctx.handle, self.handle))
+            self.handle = 0
+
+
+def _add_gzip_bytes(statistics: dict, n: int):
+    statistics["in_bytes_gzip"] = statistics.get("in_bytes_gzip", 0) + n
+
+
+def read_gzip_device_chunks(f, trimmer, buffer_size: int = 4 * 1024 * 1024):
+    """
+    Chunks of a gzip file (a binary file object of the compressed bytes) inflated on the device
+    (``cg_fastq_submit_gzip``): every member is inflated on the GPU and the plain bytes never cross PCIe.  Yields
+    ``DeviceChunk`` objects for ``trimmer`` (a FastqTrimmer; its context and format decide how the chunks are cut: the
+    records of read_fastq_chunks / read_fasta_chunks).  A chunk is submitted when the generator is advanced, so the
+    trimmer's one chunk in flight stays as it is.  ``trimmer.statistics["in_bytes_gzip"]`` counts the compressed bytes
+    consumed.  Meant for files of many members (BGZF, concatenated .gz files, this project's gzip outputs); a member
+    that does not fit one submission makes the buffer grow.
+    """
+    g = _GzipInput(trimmer.ctx, f, buffer_size)
+    try:
+        while not g.done:
+            g.fill()
+            slot, res = C.c_int32(-1), _lib.cg_gzin_result()
+            _lib.check(_lib.lib().cg_fastq_submit_gzip(trimmer.ctx.handle, g.handle, g.pointer(), g.end,
+                                                       trimmer.params.format, int(g.eof), C.byref(slot), C.byref(res)))
+            _add_gzip_bytes(trimmer.statistics, res.consumed)
+            g.consume(res.consumed)
+            if slot.value >= 0:
+                yield DeviceChunk(slot.value, res.chunk_bytes)
+    finally:
+        g.close()
+
+
+def read_gzip_device_interleaved_chunks(f, trimmer, buffer_size: int = 4 * 1024 * 1024):
+    """read_gzip_device_chunks for an interleaved file and a PairedFastqTrimmer: every chunk holds whole pairs (the
+    cuts of read_interleaved_fastq_chunks / read_interleaved_fasta_chunks) and is split on the device as
+    ``cg_fastq_submit_interleaved`` splits it.  Pass each chunk with ``chunk2=None``."""
+    g = _GzipInput(trimmer.ctx, f, buffer_size)
+    try:
+        while not g.done:
+            g.fill()
+            s1, s2, res = C.c_int32(-1), C.c_int32(-1), _lib.cg_gzin_result()
+            _lib.check(_lib.lib().cg_fastq_submit_gzip_interleaved(
+                trimmer.ctx.handle, g.handle, g.pointer(), g.end, trimmer.params1.format, int(g.eof), C.byref(s1),
+                C.byref(s2), C.byref(res)))
+            _add_gzip_bytes(trimmer.statistics[0], res.consumed)
+            g.consume(res.consumed)
+            if s1.value >= 0:
+                yield DeviceChunk(s1.value, res.chunk_bytes, s2.value)
+    finally:
+        g.close()
+
+
+def read_gzip_device_paired_chunks(f1, f2, trimmer, buffer_size: int = 4 * 1024 * 1024):
+    """read_gzip_device_chunks for the two files of a pair and a PairedFastqTrimmer: yields (chunk1, chunk2) with the
+    same number of records (read_paired_fastq_chunks / read_paired_fasta_chunks)."""
+    g1, g2 = _GzipInput(trimmer.ctx, f1, buffer_size), _GzipInput(trimmer.ctx, f2, buffer_size)
+    try:
+        while not (g1.done and g2.done):
+            g1.fill()
+            g2.fill()
+            s1, s2, r1, r2 = C.c_int32(-1), C.c_int32(-1), _lib.cg_gzin_result(), _lib.cg_gzin_result()
+            _lib.check(_lib.lib().cg_fastq_submit_gzip_paired(
+                trimmer.ctx.handle, g1.handle, g2.handle, g1.pointer(), g1.end, g2.pointer(), g2.end,
+                trimmer.params1.format, int(g1.eof and g2.eof), C.byref(s1), C.byref(s2), C.byref(r1), C.byref(r2)))
+            for st, g, r in ((trimmer.statistics[0], g1, r1), (trimmer.statistics[1], g2, r2)):
+                _add_gzip_bytes(st, r.consumed)
+                g.consume(r.consumed)
+            if s1.value >= 0:
+                yield DeviceChunk(s1.value, r1.chunk_bytes), DeviceChunk(s2.value, r2.chunk_bytes)
+    finally:
+        g1.close()
+        g2.close()
+
+
 _FORMATS = {("fastq", None): _lib.CG_FORMAT_FASTQ, ("fastq", "fastq"): _lib.CG_FORMAT_FASTQ,
             ("fasta", None): _lib.CG_FORMAT_FASTA, ("fasta", "fasta"): _lib.CG_FORMAT_FASTA,
             ("fastq", "fasta"): _lib.CG_FORMAT_FASTQ_TO_FASTA}
@@ -827,12 +947,16 @@ def _format_code(input_format: str, output_format: Optional[str]) -> int:
     return _FORMATS[(input_format, output_format)]
 
 
-def _output_capacity(n_bytes: int, fmt: int, gzip: bool = False, n_dest: int = 4) -> int:
+def _output_capacity(n_bytes: int, fmt: int, gzip: bool = False, n_dest: int = 4, rc_suffixes: bool = False) -> int:
     """Output bytes a chunk of n_bytes can need: trimming only shortens a record ("\\r\\n" -> "\\n" and "+name" -> "+"
     too), except for the newline a chunk without a final one gets and, in FASTA, the empty line of a record without
-    sequence (">a\\n" -> ">a\\n\\n", at most 1.5 x).  gzip outputs: a member adds at most 23 bytes to its 65 280, and
+    sequence (">a\\n" -> ">a\\n\\n", at most 1.5 x).  rc_suffixes: FASTA output that may append " rc" to every
+    record, at most 3 x (">\\n" -> "> rc\\n\\n").  gzip outputs: a member adds at most 23 bytes to its 65 280, and
     each of the n_dest outputs can end in a short member."""
-    plain = (n_bytes + n_bytes // 2 if fmt == _lib.CG_FORMAT_FASTA else n_bytes) + 16
+    if rc_suffixes and fmt != _lib.CG_FORMAT_FASTQ:
+        plain = 3 * n_bytes + 16
+    else:
+        plain = (n_bytes + n_bytes // 2 if fmt == _lib.CG_FORMAT_FASTA else n_bytes) + 16
     return plain + (_lib.GZ_OVERHEAD * (plain // _lib.GZ_MEMBER + n_dest) if gzip else 0)
 
 
@@ -1013,14 +1137,18 @@ class FastqTrimmer:
         self._out_bufs, self._out_keep = {}, {}
 
     def _submit(self, chunk) -> Tuple[int, int, object]:
+        if isinstance(chunk, DeviceChunk):
+            return chunk.slot, chunk.size, chunk
         buf = np.frombuffer(chunk, dtype=np.uint8) if not isinstance(chunk, np.ndarray) else chunk
         slot = C.c_int32(-1)
         _lib.check(_lib.lib().cg_fastq_submit(self.ctx.handle, buf.ctypes.data if buf.size else None, buf.size,
                                               C.byref(slot)))
         return slot.value, buf.size, buf    # buf is kept alive until collect
 
-    def _capacity(self, n_bytes: int, n_dest: int = 4) -> int:
-        return _output_capacity(n_bytes, self.params.format, self.params.gzip_outputs != 0, n_dest)
+    def _capacity(self, n_bytes: int, n_dest: int = 4, chunk=None) -> int:
+        # a device chunk cannot be submitted again, so FASTA output with " rc" suffixes gets room for all of them
+        rc = isinstance(chunk, DeviceChunk) and self.params.revcomp != 0
+        return _output_capacity(n_bytes, self.params.format, self.params.gzip_outputs != 0, n_dest, rc)
 
     def _account(self, res) -> None:
         for k, v in res.as_dict(self.params.gzip_outputs != 0).items():
@@ -1043,14 +1171,15 @@ class FastqTrimmer:
 
     def _collect(self, ticket, copy: bool = True):
         slot, n_bytes, chunk = ticket
-        out = self._out_buffer(slot, self._capacity(n_bytes))
+        out = self._out_buffer(slot, self._capacity(n_bytes, chunk=chunk))
         while True:
             res = _lib.cg_fastq_result()
             rc = _lib.lib().cg_fastq_collect(
                 self.ctx.handle, slot, self._set.handle if self._set is not None else None, C.byref(self.params),
                 out.ctypes.data, out.size, C.byref(res))
             # FASTA output: " rc" suffixes can exceed the bound; the call says how much it needs, run the chunk again
-            if rc != 0 and self.params.format != _lib.CG_FORMAT_FASTQ and res.out_bytes > out.size:
+            if (rc != 0 and self.params.format != _lib.CG_FORMAT_FASTQ and res.out_bytes > out.size
+                    and not isinstance(chunk, DeviceChunk)):
                 slot, _, chunk = self._submit(chunk)
                 out = self._out_buffer(slot, res.out_bytes)
                 continue
@@ -1070,7 +1199,7 @@ class FastqTrimmer:
 
     def _collect_split(self, ticket, copy: bool = True) -> dict:
         slot, n_bytes, chunk = ticket
-        out = self._out_buffer(slot, self._capacity(n_bytes))
+        out = self._out_buffer(slot, self._capacity(n_bytes, chunk=chunk))
         segments = np.zeros(5, dtype=np.int64)
         while True:
             res = _lib.cg_fastq_result()
@@ -1078,7 +1207,7 @@ class FastqTrimmer:
                 self.ctx.handle, slot, self._set.handle if self._set is not None else None, C.byref(self.params),
                 self._redirect, self._fasta_outputs, out.ctypes.data, out.size, C.byref(res), segments.ctypes.data)
             # " rc" suffixes can exceed the bound; the call says how much it needs, run the chunk again
-            if rc != 0 and res.out_bytes > out.size:
+            if rc != 0 and res.out_bytes > out.size and not isinstance(chunk, DeviceChunk):
                 slot, _, chunk = self._submit(chunk)
                 out = self._out_buffer(slot, res.out_bytes)
                 continue
@@ -1145,8 +1274,18 @@ class FastqTrimmer:
         per_read = max(1, self.params.trim.times) * 2
         n_bytes = len(chunk)
         capacity = per_read * 2 * n_bytes + (1 << 20)
+        if isinstance(chunk, DeviceChunk):
+            # a chunk inflated on the device can only be collected once: its plain bytes are kept on the host, so
+            # that a second try with a larger row buffer submits them as an ordinary chunk
+            plain, got = np.empty(n_bytes, dtype=np.uint8), C.c_int64(0)
+            _lib.check(_lib.lib().cg_fastq_slot_read(self.ctx.handle, chunk.slot, plain.ctypes.data, plain.size,
+                                                     C.byref(got)))
+            first, chunk = chunk, plain[: got.value]
+        else:
+            first = chunk
         while True:
-            slot, _, _ = self._submit(chunk)
+            slot, _, _ = self._submit(first)
+            first = chunk
             out = self._out_buffer(slot, self._capacity(n_bytes))
             rows = np.empty(capacity, dtype=np.uint8)
             res = _lib.cg_fastq_result()
@@ -1355,6 +1494,8 @@ class PairedFastqTrimmer:
         return tuple(written_lengths(v, max_len) for v, max_len, _ in self.statistics_vector())
 
     def _submit(self, chunk):
+        if isinstance(chunk, DeviceChunk):
+            return chunk.slot, chunk
         buf = np.frombuffer(chunk, dtype=np.uint8) if not isinstance(chunk, np.ndarray) else chunk
         slot = C.c_int32(-1)
         _lib.check(_lib.lib().cg_fastq_submit(self.ctx.handle, buf.ctypes.data if buf.size else None, buf.size,
@@ -1365,6 +1506,8 @@ class PairedFastqTrimmer:
         """((slot1, chunk), (slot2, chunk)): two chunks, or one interleaved chunk (chunk2 None) split on the device."""
         if chunk2 is not None:
             return self._submit(chunk1), self._submit(chunk2)
+        if isinstance(chunk1, DeviceChunk):            # interleaved, already split into two slots
+            return (chunk1.slot, chunk1), (chunk1.slot2, chunk1)
         buf = np.frombuffer(chunk1, dtype=np.uint8) if not isinstance(chunk1, np.ndarray) else chunk1
         s1, s2 = C.c_int32(-1), C.c_int32(-1)
         _lib.check(_lib.lib().cg_fastq_submit_interleaved(self.ctx.handle, buf.ctypes.data if buf.size else None,

@@ -380,6 +380,46 @@ int cg_fastq_submit(cg_ctx *ctx, const uint8_t *fastq, int64_t n_bytes, int32_t 
 int cg_fastq_collect(cg_ctx *ctx, int32_t slot, const cg_adapterset *set, const cg_fastq_params *params,
                      uint8_t *out, int64_t out_capacity, cg_fastq_result *res);
 
+/* gzip input, inflated on the device.  A stream per input file (cg_gzin_create) keeps on the device the plain bytes
+ * that do not yet form a whole record (the carry) and counts the compressed bytes consumed, so that errors can name an
+ * offset in the file.  cg_fastq_submit_gzip takes the next compressed bytes of the file (host memory, starting at a
+ * member boundary), uploads them, inflates every whole member they hold (zero bytes after a member are skipped), appends
+ * the plain bytes to the carry and cuts the longest prefix of whole records into a slot -- the rules of read_fastq_chunks
+ * / read_fasta_chunks (format CG_FORMAT_FASTQ_TO_FASTA cuts as FASTQ).  The caller passes the bytes not consumed again,
+ * in front of the next ones.  No whole record yet: no slot is taken, *slot = -1.  final: every byte must be consumed and
+ * the carry becomes the last chunk, which may lack its final newline.  The slot is indistinguishable from cg_fastq_submit
+ * of the same plain bytes: every collect accepts it.
+ * Errors: CG_EINVAL for what Python's gzip module rejects (the message names the byte offset of the bad member in the
+ * file; no slot is taken and the stream is unchanged); CG_EUNSUPPORTED when not even one member fits under the 2 GiB
+ * plain-size limit of a submission (the chain otherwise stops early to stay under it; `consumed` says where).  The
+ * paired call's messages name the mate (first or second input). */
+typedef struct cg_gzin_result {
+    int64_t consumed;      /* compressed bytes of whole members (and the zeros behind them) used */
+    int64_t members;       /* members inflated */
+    int64_t plain_bytes;   /* their plain bytes */
+    int64_t chunk_bytes;   /* bytes of the chunk in the slot (0 without a slot) */
+    int64_t carry_bytes;   /* plain bytes kept for the next submission */
+    int64_t n_records;     /* records of the chunk (pairs count two) */
+    int64_t reserved[2];
+} cg_gzin_result;
+int cg_gzin_create(cg_ctx *ctx, int32_t *handle);
+int cg_gzin_destroy(cg_ctx *ctx, int32_t handle);
+int cg_fastq_submit_gzip(cg_ctx *ctx, int32_t handle, const uint8_t *gz, int64_t n_bytes, int32_t format, int32_t final,
+                         int32_t *slot, cg_gzin_result *res);
+/* The plain chunk of a submitted, not yet collected slot (not a mate of an interleaved chunk), copied to host memory:
+ * what a caller keeps to submit a chunk from cg_fastq_submit_gzip again (a collect that needs a larger row buffer).
+ * *n_bytes: its size; CG_EINVAL when capacity is smaller. */
+int cg_fastq_slot_read(cg_ctx *ctx, int32_t slot, uint8_t *dst, int64_t capacity, int64_t *n_bytes);
+/* Two files of a pair: both chunks hold the same number of records (read_paired_fastq_chunks / read_paired_fasta_chunks);
+ * slots -1 until both have one. */
+int cg_fastq_submit_gzip_paired(cg_ctx *ctx, int32_t handle1, int32_t handle2, const uint8_t *gz1, int64_t n_bytes1,
+                                const uint8_t *gz2, int64_t n_bytes2, int32_t format, int32_t final, int32_t *slot1,
+                                int32_t *slot2, cg_gzin_result *res1, cg_gzin_result *res2);
+/* An interleaved file: the chunk holds whole pairs (8 lines, or an even number of FASTA records) and becomes the two
+ * slots cg_fastq_submit_interleaved gives for it. */
+int cg_fastq_submit_gzip_interleaved(cg_ctx *ctx, int32_t handle, const uint8_t *gz, int64_t n_bytes, int32_t format,
+                                     int32_t final, int32_t *slot1, int32_t *slot2, cg_gzin_result *res);
+
 /* Demultiplexing (Demultiplexer.__call__, steps.py:397-409; SURVEY.md section 8(f) N4): every surviving record
  * goes to the output of the adapter of its most recent match, records without a match to the last output
  * ("unknown"; combine with discard_untrimmed to drop them).  adapter_dest[a] in [0, n_named) names the output of

@@ -24,6 +24,15 @@ bytes per chunk (Context.transfer_bytes); the card's name and power limit are re
 read-only query).  A second line: the device time of gz_compress_kernel and gz_gather_kernel per MiB of plain output
 and per chunk, from torch.profiler's CUDA activity in a run of its own over the warmed chunks, next to the wall time
 per chunk that gzip adds, so that kernel time and the host round trip of the compaction can be told apart.
+--gzip-input [n_reads] [submission_megabytes]: gzip input, three arms alternating over three rounds in one process on
+each of two inputs of the same reads (-a AGATCGGAAGAGC -q 20 -m 20, plain output): "plain" (read_fastq_chunks on the
+plain bytes), "host_gzip" (Python's gzip module on one core, the tool's path for single-member files) and "device"
+(read_gzip_device_chunks: the compressed bytes are uploaded and inflated on the device).  Inputs: "multi_member"
+(members of 65 280 plain bytes at zlib level 6), "mib_members" (members of 2 MiB plain, about 1 MiB compressed: the
+tool's threshold) and "single_member" (one zlib level 6 member).  One thread inflates a
+member, so the device arm of the single-member input runs on its first 8 MiB only and is reported per MiB.  Per arm:
+host-to-host reads/s and MiB/s of plain input, and the bytes uploaded.  A last line: the inflate kernels' device time
+per MiB of plain output from torch.profiler in a run of its own.  The card's name and power limit are read in the run.
 """
 import json
 import subprocess
@@ -163,7 +172,92 @@ def measure_gzip(n, chunk_mb):
                       "wall_ms_per_chunk_added_by_gzip": added}))
 
 
+def measure_gzip_input(n, submit_mb):
+    import gzip
+    import io
+    from concurrent.futures import ThreadPoolExecutor
+
+    from cutadapt_b200.pipeline import read_fastq_chunks, read_gzip_device_chunks
+
+    data, rec_len = build_fastq(n, pinned=False)
+    plain = data.tobytes()
+    pieces = [plain[i:i + 65280] for i in range(0, len(plain), 65280)]
+    with ThreadPoolExecutor(16) as ex:
+        multi = b"".join(ex.map(lambda p: gzip.compress(p, 6, mtime=0), pieces))
+    single = gzip.compress(plain, 6, mtime=0)
+    big = [plain[i:i + (2 << 20)] for i in range(0, len(plain), 2 << 20)]
+    with ThreadPoolExecutor(16) as ex:
+        mib = b"".join(ex.map(lambda p: gzip.compress(p, 6, mtime=0), big))
+    small = len(plain) if len(plain) <= 8 << 20 else (8 << 20) // rec_len * rec_len
+    inputs = {"multi_member": (multi, plain), "mib_members": (mib, plain), "single_member": (single, plain)}
+    adapters = [PA.BackAdapter("AGATCGGAAGAGC", max_errors=0.1)]
+    opts = dict(quality_cutoff=(0, 20), minimum_length=20)
+    chunk = 64 << 20
+
+    def run(arm, gz, pl):
+        t = FastqTrimmer(adapters, **opts)
+        if arm == "plain":
+            src = read_fastq_chunks(io.BytesIO(pl), chunk)
+        elif arm == "host_gzip":
+            src = read_fastq_chunks(gzip.GzipFile(fileobj=io.BytesIO(gz)), chunk)
+        else:
+            src = read_gzip_device_chunks(io.BytesIO(gz), t, submit_mb << 20)
+        t.ctx.transfer_bytes(reset=True)
+        t0 = time.perf_counter()
+        out = sum(len(o) for o in t.process_chunks(src, copy=False))
+        return time.perf_counter() - t0, out, t.ctx.transfer_bytes()[0]
+
+    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader",
+                           "-i", str(torch.cuda.current_device())], capture_output=True, text=True).stdout.strip()
+    single_small = gzip.compress(plain[:small], 6, mtime=0)
+    res = {}
+    for name, (gz, pl) in inputs.items():
+        arms = {"plain": (gz, pl), "host_gzip": (gz, pl),
+                "device": (gz, pl) if name != "single_member" else (single_small, plain[:small])}
+        warm = plain[:rec_len * 1000]
+        for arm in arms:                          # warm-up: buffers, module load
+            run(arm, gzip.compress(warm, 6), warm)
+        r = {arm: {"wall_s": 0.0, "plain_bytes": len(p), "gz_bytes": len(g)} for arm, (g, p) in arms.items()}
+        outs = {}
+        for _ in range(3):
+            for arm, (g, p) in arms.items():
+                w, out, up = run(arm, g, p)
+                r[arm]["wall_s"] += w
+                r[arm]["h2d_bytes"] = up
+                outs.setdefault(len(p), set()).add(out)
+        for arm, x in r.items():
+            reads = x["plain_bytes"] // rec_len
+            x["M_reads_per_s"] = 3 * reads / x["wall_s"] / 1e6
+            x["plain_MiB_per_s"] = 3 * x["plain_bytes"] / x["wall_s"] / 2**20
+        assert all(len(v) == 1 for v in outs.values()), "the arms wrote different amounts"
+        res[name] = r
+    print(json.dumps({"what": "gzip input -> trimmed FASTQ (-a AGATCGGAAGAGC -q 20 -m 20), host to host", "reads": n,
+                      "submission_MiB": submit_mb, "gpu": torch.cuda.get_device_name(), "card_and_power_limit": card,
+                      "inputs": res}))
+
+    from torch.profiler import ProfilerActivity, profile
+
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        run("device", multi, plain)
+        torch.cuda.synchronize()
+    ms, launches = {}, {}
+    for ev in prof.key_averages():
+        for k in ("gu_cand_count", "gu_cand_write", "gu_parse", "gu_chain", "gu_place", "gu_crc", "gu_flag", "gu_select"):
+            if k + "_kernel" in ev.key:
+                ms[k] = ms.get(k, 0.0) + ev.device_time_total / 1000.0
+                launches[k] = launches.get(k, 0) + ev.count
+    if "gu_parse" not in ms:
+        raise RuntimeError("the profiler saw no gu_parse_kernel launch")
+    mib = len(plain) / 2**20
+    print(json.dumps({"what": "inflate kernels' device time on the multi-member input (torch.profiler, CUDA activity)",
+                      "card_and_power_limit": card, "ms_per_MiB_plain": {k: v / mib for k, v in ms.items()},
+                      "ms_per_MiB_plain_total": sum(ms.values()) / mib, "launches": launches}))
+
+
 def main():
+    if "--gzip-input" in sys.argv:
+        argv = [a for a in sys.argv if a != "--gzip-input"]
+        return measure_gzip_input(int(argv[1]) if len(argv) > 1 else 4_000_000, int(argv[2]) if len(argv) > 2 else 64)
     if "--gzip" in sys.argv:
         argv = [a for a in sys.argv if a != "--gzip"]
         return measure_gzip(int(argv[1]) if len(argv) > 1 else 4_000_000, int(argv[2]) if len(argv) > 2 else 64)

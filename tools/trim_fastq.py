@@ -30,24 +30,52 @@ exception: with demultiplexing the device compresses all demultiplexed outputs a
 receives the "unknown" output) must end in .gz exactly when the -o template does; otherwise the tool stops with an
 error.  A .gz output
 that receives no read still gets one empty gzip member.  The device has one compression strategy, comparable in size to
-zlib's level 1, so there is no --compression-level.  Inputs ending in .gz are decompressed on the host; the format is
-then detected from the first decompressed byte.
+zlib's level 1, so there is no --compression-level.  An input ending in .gz whose first gzip member ends within its
+first MiB (BGZF, concatenated .gz files, this tool's own .gz outputs) is inflated on the device: the compressed bytes are
+uploaded (read_gzip_device_chunks; for two paired inputs only when both qualify).  Any other .gz input is decompressed on
+the host with Python's gzip module.  The outputs are the same either way; the stderr line's "in_bytes_gzip" (the
+compressed bytes consumed) appears only when the device inflated the input.  The format is detected from the first
+decompressed byte.
 """
 import argparse
 import gzip
+import zlib
 import json
 import sys
 
 sys.path.insert(0, __file__.rsplit("/", 2)[0])
 import cutadapt_b200.adapters as PA  # noqa: E402
 from cutadapt_b200.pipeline import (FastqTrimmer, PairedFastqTrimmer, read_fasta_chunks,  # noqa: E402
-                                    read_fastq_chunks, read_interleaved_fasta_chunks, read_interleaved_fastq_chunks,
-                                    read_paired_fasta_chunks, read_paired_fastq_chunks)
+                                    read_fastq_chunks, read_gzip_device_chunks, read_gzip_device_interleaved_chunks,
+                                    read_gzip_device_paired_chunks, read_interleaved_fasta_chunks,
+                                    read_interleaved_fastq_chunks, read_paired_fasta_chunks, read_paired_fastq_chunks)
 
 
 def open_input(path):
     """An input file for reading; a .gz one is decompressed on the host."""
     return gzip.open(path, "rb") if path.endswith(".gz") else open(path, "rb")
+
+
+# A .gz input goes to the device (read_gzip_device_chunks) when its first member ends within this many compressed
+# bytes: one GPU thread inflates a member, so only files of many members gain (DESIGN.md section 4.8 has the measurement).
+DEVICE_GZIP_FIRST_MEMBER = 1 << 20
+
+
+def gzip_on_device(path):
+    """Whether a .gz input is inflated on the device: host zlib inflates its first member from a prefix of the file,
+    and the member must end within the first DEVICE_GZIP_FIRST_MEMBER compressed bytes."""
+    if not path.endswith(".gz"):
+        return False
+    with open(path, "rb") as f:
+        head = f.read(DEVICE_GZIP_FIRST_MEMBER)
+    d = zlib.decompressobj(31)
+    try:
+        while head and not d.eof:
+            d.decompress(head, 1 << 20)           # bounded output: only where the member ends matters
+            head = d.unconsumed_tail
+    except zlib.error:
+        return False                              # the host path reports the error as Python's gzip module does
+    return d.eof
 
 
 def detect_format(path):
@@ -226,7 +254,18 @@ def main():
     if input_format == "fasta" and args.max_ee is not None:
         print("WARNING: Ignoring option --max-ee because input does not provide quality values", file=sys.stderr)
         args.max_ee = None
-    reader = read_fasta_chunks if input_format == "fasta" else read_fastq_chunks
+    host_reader = read_fasta_chunks if input_format == "fasta" else read_fastq_chunks
+    # compressed bytes per submission of a device-inflated input: one thread inflates a member, so a submission must hold
+    # many members; with --buffer-size 64 MiB, members of up to 1 MiB give 64 or more at once
+    gz_buffer = args.buffer_size
+
+    def single_input(t):
+        """(file, chunks) of the single input for trimmer t."""
+        if gzip_on_device(args.inputs[0]):
+            f = open(args.inputs[0], "rb")
+            return f, read_gzip_device_chunks(f, t, gz_buffer)
+        f = open_input(args.inputs[0])
+        return f, host_reader(f, args.buffer_size)
     paired_reader = read_paired_fasta_chunks if input_format == "fasta" else read_paired_fastq_chunks
 
     qc = None
@@ -268,9 +307,15 @@ def main():
                        if not (args.paired_output if d == "output" else getattr(args, d + "_paired_output"))]
         t = PairedFastqTrimmer(ads1, ads2, common, options2, args.pair_filter, **formats, **split,
                                interleaved_outputs=interleaved, gzip_outputs=gzip1, gzip_outputs2=gzip2)
-        if len(args.inputs) == 2:
+        if len(args.inputs) == 2 and all(map(gzip_on_device, args.inputs)):
+            f1, f2 = open(args.inputs[0], "rb"), open(args.inputs[1], "rb")
+            chunks = read_gzip_device_paired_chunks(f1, f2, t, gz_buffer)
+        elif len(args.inputs) == 2:
             f1, f2 = open_input(args.inputs[0]), open_input(args.inputs[1])
             chunks = paired_reader(f1, f2, args.buffer_size)
+        elif gzip_on_device(args.inputs[0]):
+            f1 = f2 = open(args.inputs[0], "rb")
+            chunks = read_gzip_device_interleaved_chunks(f1, t, gz_buffer)
         else:
             f1 = f2 = open_input(args.inputs[0])
             chunks = (read_interleaved_fasta_chunks if input_format == "fasta" else read_interleaved_fastq_chunks)(
@@ -296,8 +341,9 @@ def main():
             ap.error("with demultiplexing, --untrimmed-output must be compressed (.gz) exactly when the -o template is")
         t = FastqTrimmer(ads1, **common, **formats, gzip_outputs=gzip1)
         files = {}
-        with open_input(args.inputs[0]) as f:
-            for chunk in reader(f, args.buffer_size):
+        f, chunks = single_input(t)
+        with f:
+            for chunk in chunks:
                 for name, data in t.process_chunk_demux(chunk).items():
                     if name == "unknown" and args.discard_untrimmed:
                         continue
@@ -312,10 +358,11 @@ def main():
         stats = t.statistics
     elif redirect:
         t = FastqTrimmer(ads1, **common, **formats, **split, gzip_outputs=gzip1)
-        with open_input(args.inputs[0]) as f:
+        f, chunks = single_input(t)
+        with f:
             files = {d: OutputFile(getattr(args, d + "_output")) for d in redirect}
             files["output"] = OutputFile(args.output)
-            for parts in t.process_chunks_split(reader(f, args.buffer_size), copy=False):
+            for parts in t.process_chunks_split(chunks, copy=False):
                 for name, data in parts.items():
                     files[name].write(data)
             for fh in files.values():
@@ -324,8 +371,9 @@ def main():
     else:
         t = FastqTrimmer(ads1, **common, **formats, gzip_outputs=gzip1)
         o = OutputFile(args.output)
-        with open_input(args.inputs[0]) as f:
-            for out in t.process_chunks(reader(f, args.buffer_size), copy=False):
+        f, chunks = single_input(t)
+        with f:
+            for out in t.process_chunks(chunks, copy=False):
                 o.write(out.tobytes() if hasattr(out, "tobytes") else out)
         o.close()
         stats = t.statistics
