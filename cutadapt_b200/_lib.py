@@ -37,6 +37,9 @@ CG_GROUP_INDEXED = 2
 CG_FORMAT_FASTQ = 0              # cg_fastq_params.format: FASTQ in, FASTQ out
 CG_FORMAT_FASTA = 1              # FASTA in, FASTA out
 CG_FORMAT_FASTQ_TO_FASTA = 2     # FASTQ in, FASTA out
+CG_GZIN_SPLIT_MEMBERS = 1        # cg_gzin_create_ex: long members inflated block-parallel, consumed in part
+CG_GZIN_LONG_MEMBER = 64 * 1024  # compressed bytes above which a split stream takes a member block-parallel
+CG_GZIN_STRIDE = 64 * 1024       # compressed bytes between speculative chunk starts
 CG_REDIRECT_TOO_SHORT = 1        # cg_fastq_collect_split: --too-short-output (destination 1)
 CG_REDIRECT_TOO_LONG = 2         # --too-long-output (destination 2)
 CG_REDIRECT_UNTRIMMED = 4        # --untrimmed-output (destination 3)
@@ -152,7 +155,7 @@ class cg_fastq_result(C.Structure):
 
 class cg_gzin_result(C.Structure):
     _fields_ = [(name, C.c_int64) for name in (
-        "consumed", "members", "plain_bytes", "chunk_bytes", "carry_bytes", "n_records")] + [("reserved", C.c_int64 * 2)]
+        "consumed", "members", "plain_bytes", "chunk_bytes", "carry_bytes", "n_records", "in_member", "respeculated")]
 
 
 MATCH_DTYPE = np.dtype(
@@ -217,6 +220,7 @@ def _declare(lib) -> None:
                                                   C.POINTER(cg_fastq_result), C.POINTER(cg_fastq_result), vp, vp]
     lib.cg_fastq_submit_interleaved.argtypes = [vp, vp, i64, i32, C.POINTER(i32), C.POINTER(i32)]
     lib.cg_gzin_create.argtypes = [vp, C.POINTER(i32)]
+    lib.cg_gzin_create_ex.argtypes = [vp, i32, C.POINTER(i32)]
     lib.cg_fastq_slot_read.argtypes = [vp, i32, vp, i64, C.POINTER(i64)]
     lib.cg_gzin_destroy.argtypes = [vp, i32]
     lib.cg_fastq_submit_gzip.argtypes = [vp, i32, vp, i64, i32, i32, C.POINTER(i32), C.POINTER(cg_gzin_result)]

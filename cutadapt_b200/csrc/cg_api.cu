@@ -158,11 +158,26 @@ struct GzinStream {
     long long carry = 0, consumed = 0, members = 0;
     // the submission in progress, committed once its slots are known: plain bytes behind the carry, bytes and members
     long long pend_plain = 0, pend_consumed = 0, pend_members = 0;
+    // CG_GZIN_SPLIT_MEMBERS: a long member is inflated block-parallel and may be consumed in part.  Then the stream
+    // keeps the bit offset into the next byte, the running CRC-32 register and plain length, the member's offset in the
+    // file, whether only its trailer is left, and its last GU_WIN plain bytes (d_win); the p* copies are pending.
+    bool split = false;
+    long long stride = CG_GZIN_STRIDE;
+    struct Member { int in = 0, bitoff = 0, trailer = 0; uint32_t crc = 0; long long len = 0, start = 0; } mem, pmem;
+    long long pend_respec = 0;
+    DevBuf<uint8_t> d_win, d_pwin, d_wins;
+    DevBuf<GuChunk> d_ch;
+    DevBuf<long long> d_coff, d_room;
+    DevBuf<uint16_t> d_sym;
+    DevBuf<int32_t> d_redo;
+    DevBuf<uint32_t> d_part;
     void release()
     {
         d_gz.release(); d_plain.release(); h_gz.release(); d_counts.release(); d_cand.release(); d_members.release();
         d_flag.release(); d_offs.release(); d_res.release(); d_moff.release(); d_scan.release(); d_small.release();
         d_tiles.release(); d_nl.release();
+        d_win.release(); d_pwin.release(); d_wins.release(); d_ch.release(); d_coff.release(); d_room.release();
+        d_sym.release(); d_redo.release(); d_part.release();
         if (done) cudaEventDestroy(done);
         done = nullptr;
     }
@@ -1768,18 +1783,33 @@ extern "C" int cg_fastq_submit_interleaved(cg_ctx *c, const uint8_t *chunk, int6
 // ------------------------------------------------------------------------------------------
 #define CG_GZIN_LIMIT (1LL << 31)        // plain bytes of one submission stay under the slot limit
 
-extern "C" int cg_gzin_create(cg_ctx *c, int32_t *handle)
+extern "C" int cg_gzin_create_ex(cg_ctx *c, int32_t flags, int32_t *handle)
 {
-    if (!c || !handle) return fail(CG_EINVAL, "cg_gzin_create: bad argument");
+    if (!c || !handle || (flags & ~CG_GZIN_SPLIT_MEMBERS)) return fail(CG_EINVAL, "cg_gzin_create: bad argument");
     CU(cudaSetDevice(c->device));
     const int32_t h = c->gzin_next++;
     GzinStream &g = c->gzin[h];
     int rc;
-    if ((rc = g.d_small.ensure(4 + (sizeof(GuChain) + 7) / 8)) != CG_OK) { c->gzin.erase(h); return rc; }
+    if ((rc = g.d_small.ensure(4 + (std::max(sizeof(GuChain), sizeof(GuWalk)) + 7) / 8)) != CG_OK) {
+        c->gzin.erase(h);
+        return rc;
+    }
+    if (flags & CG_GZIN_SPLIT_MEMBERS) {
+        g.split = true;
+        // CUTADAPT_B200_GZIN_STRIDE (cutadapt_b200.h): the stride sweep of tools/measure_fastq.py --gzip-input
+        if (const char *e = getenv("CUTADAPT_B200_GZIN_STRIDE")) g.stride = std::max(32768LL, atoll(e));
+        if ((rc = g.d_win.ensure(GU_WIN)) != CG_OK || (rc = g.d_pwin.ensure(GU_WIN)) != CG_OK) {
+            g.release();
+            c->gzin.erase(h);
+            return rc;
+        }
+    }
     CU(cudaEventCreateWithFlags(&g.done, cudaEventDisableTiming));
     *handle = h;
     return CG_OK;
 }
+
+extern "C" int cg_gzin_create(cg_ctx *c, int32_t *handle) { return cg_gzin_create_ex(c, 0, handle); }
 
 extern "C" int cg_gzin_destroy(cg_ctx *c, int32_t handle)
 {
@@ -1790,6 +1820,268 @@ extern "C" int cg_gzin_destroy(cg_ctx *c, int32_t handle)
     if (it->second.done) CU(cudaEventSynchronize(it->second.done));
     it->second.release();
     c->gzin.erase(it);
+    return CG_OK;
+}
+
+// d_plain holds at least `total` bytes (+ 64); its first `keep` bytes stay
+static int gzin_plain_room(GzinStream &g, long long keep, long long total, cudaStream_t st)
+{
+    if ((size_t)total + 64 <= g.d_plain.cap) return CG_OK;
+    DevBuf<uint8_t> nb;
+    int rc;
+    if ((rc = nb.ensure((size_t)total + 64)) != CG_OK) return rc;
+    if (keep) CU(cudaMemcpyAsync(nb.p, g.d_plain.p, (size_t)keep, cudaMemcpyDeviceToDevice, st));
+    CU(cudaStreamSynchronize(st));
+    g.d_plain.release();
+    g.d_plain = nb;
+    return CG_OK;
+}
+
+// The chain of whole members from byte `from` inflated behind d_plain[0, base) and their CRC-32 checked (*ch).  split:
+// the chain may end at a member for the block path (ch->status GU_LONG).
+static int gzin_members(cg_ctx *c, GzinStream &g, long long n, int n_cand, long long from, bool after_member, bool final,
+                        long long base, bool split, cudaStream_t st, GuChain *out)
+{
+    int rc;
+    GuChain *d_chain = reinterpret_cast<GuChain *>(g.d_small.p + 4);
+    CU(cg_launch_gunzip_chain(g.d_gz.p, n, g.d_cand.p, g.d_res.p, n_cand, after_member, final, base, CG_GZIN_LIMIT,
+                              g.d_members.p, g.d_moff.p, d_chain, from, split, st));
+    c->launches += 1;
+    GuChain &ch = *out;
+    CU(cudaMemcpyAsync(&ch, d_chain, sizeof ch, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    const long long at = g.consumed + ch.err_at;
+    if (ch.status == GU_INVALID)
+        return fail(CG_EINVAL, "gzip input: invalid or truncated gzip member at byte " + std::to_string(at) +
+                                   " of the compressed file");
+    if (ch.status == GU_UNSUPPORTED && !split)
+        return fail(CG_EUNSUPPORTED, "gzip input: the member at byte " + std::to_string(at) +
+                                         " inflates to more than one submission can hold (2 GiB); decompress this input "
+                                         "on the host");
+    // the carry stays where it is; a larger buffer gets a copy of it
+    if ((rc = gzin_plain_room(g, base, base + ch.plain, st)) != CG_OK) return rc;
+    if (ch.n_members) {
+        int *d_bad = reinterpret_cast<int *>(g.d_small.p + 2);
+        const int none = 0x7FFFFFFF;
+        CU(cudaMemcpyAsync(d_bad, &none, sizeof none, cudaMemcpyHostToDevice, st));
+        CU(cg_launch_gunzip_place(g.d_gz.p, n, g.d_cand.p, g.d_members.p, g.d_moff.p, d_chain, ch.n_members, g.d_res.p,
+                                  g.d_plain.p, d_bad, st));
+        c->launches += 2;
+        int bad = none;
+        CU(cudaMemcpyAsync(&bad, d_bad, sizeof bad, cudaMemcpyDeviceToHost, st));
+        CU(cudaStreamSynchronize(st));
+        if (bad != none) {
+            int32_t k = 0, pos = 0;
+            CU(cudaMemcpy(&k, g.d_members.p + bad, sizeof k, cudaMemcpyDeviceToHost));
+            CU(cudaMemcpy(&pos, g.d_cand.p + k, sizeof pos, cudaMemcpyDeviceToHost));
+            return fail(CG_EINVAL, "gzip input: CRC-32 mismatch in the gzip member at byte " +
+                                       std::to_string(g.consumed + pos) + " of the compressed file");
+        }
+    }
+    return CG_OK;
+}
+
+// The block path (cg_gunzip_core.cuh, gu_chunk / gu_walk): the member's deflate bits from bit s0 of the uploaded bytes,
+// inflated behind d_plain[0, base).  The stream's pending member (g.pmem) says how far the member got before; its
+// window is g.d_win.  *r: the walk's verdict (r->plain bytes placed, r->end the bit behind them); the pending window,
+// CRC register and length advance.
+static int gzin_blocks(cg_ctx *c, GzinStream &g, long long n, long long bound, long long s0, long long base,
+                       cudaStream_t st, GuWalk *r,
+                       long long *respec)
+{
+    int rc;
+    const long long S = g.stride, limit = CG_GZIN_LIMIT - base;
+    const int K = (int)std::max(1LL, (bound * 8 - s0 + S * 8 - 1) / (S * 8));     // chunks up to gu_member_bound
+    if ((rc = g.d_ch.ensure((size_t)K)) != CG_OK || (rc = g.d_coff.ensure((size_t)K)) != CG_OK ||
+        (rc = g.d_room.ensure((size_t)K)) != CG_OK || (rc = g.d_redo.ensure((size_t)K)) != CG_OK)
+        return rc;
+    // room for the symbols of a chunk: 8 per compressed byte of its stride, more for a chunk that overflows
+    std::vector<long long> off(K), room(K, std::min(limit, 8 * S));
+    long long arena = 0;
+    for (int k = 0; k < K; ++k) { off[k] = arena; arena += room[k]; }
+    if ((rc = g.d_sym.ensure((size_t)arena)) != CG_OK) return rc;
+    CU(cudaMemcpyAsync(g.d_coff.p, off.data(), K * sizeof(long long), cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(g.d_room.p, room.data(), K * sizeof(long long), cudaMemcpyHostToDevice, st));
+    const GuChunk c0 = {s0, s0, 0, 0, GU_INVALID, 0};
+    CU(cudaMemcpyAsync(g.d_ch.p, &c0, sizeof c0, cudaMemcpyHostToDevice, st));
+    CU(cg_launch_gunzip_search(g.d_gz.p, n, s0, S, K, g.d_ch.p, st));
+    CU(cg_launch_gunzip_spec(g.d_gz.p, n, s0, S, K, nullptr, K, g.d_coff.p, g.d_room.p, g.d_sym.p, g.d_ch.p, st));
+    c->launches += 2;
+    GuWalk *d_walk = reinterpret_cast<GuWalk *>(g.d_small.p + 4);      // the chain's place: no chain runs meanwhile
+    std::vector<int32_t> redo;
+    std::vector<GuChunk> ch;
+    const long long max_rounds = gu_walk_rounds(K, room[0], limit);
+    for (long long round = 0;; ++round) {
+        CU(cg_launch_gunzip_walk(g.d_ch.p, K, limit, g.d_redo.p, d_walk, st));
+        c->launches += 1;
+        CU(cudaMemcpyAsync(r, d_walk, sizeof *r, cudaMemcpyDeviceToHost, st));
+        CU(cudaStreamSynchronize(st));
+        if (r->status != GU_MORE) break;
+        if (round >= max_rounds)                      // unreachable by gu_walk_rounds: a defect, not bad input
+            return fail(CG_EUNSUPPORTED, "gzip input: internal error: the block walk did not settle within " +
+                                             std::to_string(max_rounds) + " rounds");
+        *respec += r->respec;
+        redo.resize(r->n_redo);
+        ch.resize(K);
+        CU(cudaMemcpyAsync(redo.data(), g.d_redo.p, r->n_redo * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+        CU(cudaMemcpyAsync(ch.data(), g.d_ch.p, K * sizeof(GuChunk), cudaMemcpyDeviceToHost, st));
+        CU(cudaStreamSynchronize(st));
+        long long grown = 0, old_arena = arena;
+        for (int32_t k : redo) {
+            if (ch[k].status != GU_OVER || (grown && grown >= limit)) continue;
+            if (room[k] >= limit) {
+                if (k != r->n_ok) continue;
+                // the next chunk alone reaches the limit: the submission ends in front of it
+                r->status = r->n_ok ? GU_OK : GU_UNSUPPORTED;
+                break;
+            }
+            room[k] = std::min(limit, room[k] * 8);
+            off[k] = arena;
+            arena += room[k];
+            grown += room[k];
+        }
+        if (r->status != GU_MORE) break;
+        if (arena > old_arena) {
+            DevBuf<uint16_t> nb;
+            if ((rc = nb.ensure((size_t)arena)) != CG_OK) return rc;
+            CU(cudaMemcpyAsync(nb.p, g.d_sym.p, (size_t)old_arena * sizeof(uint16_t), cudaMemcpyDeviceToDevice, st));
+            CU(cudaStreamSynchronize(st));
+            g.d_sym.release();
+            g.d_sym = nb;
+            CU(cudaMemcpyAsync(g.d_coff.p, off.data(), K * sizeof(long long), cudaMemcpyHostToDevice, st));
+            CU(cudaMemcpyAsync(g.d_room.p, room.data(), K * sizeof(long long), cudaMemcpyHostToDevice, st));
+        }
+        CU(cg_launch_gunzip_spec(g.d_gz.p, n, s0, S, K, g.d_redo.p, r->n_redo, g.d_coff.p, g.d_room.p, g.d_sym.p,
+                                 g.d_ch.p, st));
+        c->launches += 1;
+    }
+    if (r->status != GU_OK) return CG_OK;
+    // the resolve grid is sized by the largest confirmed chunk
+    ch.resize(K);
+    CU(cudaMemcpyAsync(ch.data(), g.d_ch.p, r->n_ok * sizeof(GuChunk), cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    long long max_n = 0;
+    for (int k = 0; k < r->n_ok; ++k) max_n = std::max(max_n, ch[k].n);
+    if ((rc = gzin_plain_room(g, base, base + r->plain, st)) != CG_OK) return rc;
+    if ((rc = g.d_wins.ensure((size_t)(r->n_ok + 1) * GU_WIN)) != CG_OK) return rc;
+    CU(cudaMemcpyAsync(g.d_wins.p, g.d_win.p, GU_WIN, cudaMemcpyDeviceToDevice, st));
+    int *d_bad = reinterpret_cast<int *>(g.d_small.p + 2);
+    uint32_t *d_state = reinterpret_cast<uint32_t *>(g.d_small.p + 3);
+    const int none = 0x7FFFFFFF;
+    CU(cudaMemcpyAsync(d_bad, &none, sizeof none, cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(d_state, &g.pmem.crc, sizeof g.pmem.crc, cudaMemcpyHostToDevice, st));
+    CU(cg_launch_gunzip_resolve(g.d_ch.p, r->n_ok, max_n, g.d_coff.p, g.d_sym.p, g.d_wins.p, g.pmem.len,
+                                g.d_plain.p + base, d_bad, st));
+    if ((rc = g.d_part.ensure((size_t)(r->plain / cg_gunzip_crc_piece()) + 1)) != CG_OK) return rc;
+    CU(cg_launch_gunzip_crc(g.d_plain.p + base, r->plain, g.d_part.p, d_state, st));
+    CU(cudaMemcpyAsync(g.d_pwin.p, g.d_wins.p + (long long)r->n_ok * GU_WIN, GU_WIN, cudaMemcpyDeviceToDevice, st));
+    c->launches += 4;
+    int bad = none;
+    CU(cudaMemcpyAsync(&bad, d_bad, sizeof bad, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(&g.pmem.crc, d_state, sizeof g.pmem.crc, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    if (bad != none) r->status = GU_INVALID;
+    g.pmem.len += r->plain;
+    return CG_OK;
+}
+
+static uint32_t gzin_le32(const uint8_t *p) { return p[0] | (p[1] << 8) | (p[2] << 16) | ((uint32_t)p[3] << 24); }
+
+// A split stream's submission: whole members through the chain, a long member (or the rest of one) through the block
+// path, then the chain again behind it, until the bytes run out or a member stops inside.
+static int gzin_inflate_split(cg_ctx *c, GzinStream &g, const uint8_t *gz, long long n, int n_cand, bool final,
+                              cudaStream_t st, cg_gzin_result *res, bool *fin)
+{
+    int rc;
+    GzinStream::Member &m = g.pmem;
+    std::vector<int32_t> hcand;                  // the candidates and their parses, read back for gu_member_bound
+    std::vector<GuMember> hres;
+    const auto bound = [&](long long at, long long *b) {
+        if (n_cand && hcand.empty()) {
+            hcand.resize(n_cand);
+            hres.resize(n_cand);
+            CU(cudaMemcpyAsync(hcand.data(), g.d_cand.p, n_cand * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+            CU(cudaMemcpyAsync(hres.data(), g.d_res.p, n_cand * sizeof(GuMember), cudaMemcpyDeviceToHost, st));
+            CU(cudaStreamSynchronize(st));
+        }
+        *b = gu_member_bound(hcand.data(), hres.data(), n_cand, at, n);
+        return CG_OK;
+    };
+    m = g.mem;
+    long long p = 0, base = g.carry, members = 0, respec = 0;
+    bool after = g.members > 0;
+    const auto bad_member = [&]() {
+        return fail(CG_EINVAL, "gzip input: invalid or truncated gzip member at byte " + std::to_string(m.start) +
+                                   " of the compressed file");
+    };
+    for (;;) {
+        if (m.in && m.trailer) {
+            const long long t = p + (m.bitoff ? 1 : 0);
+            if (t + 8 > n) {
+                if (final) return bad_member();
+                break;
+            }
+            if (gzin_le32(gz + t) != ~m.crc || gzin_le32(gz + t + 4) != (uint32_t)m.len)
+                return fail(CG_EINVAL, "gzip input: CRC-32 mismatch in the gzip member at byte " + std::to_string(m.start) +
+                                           " of the compressed file");
+            p = t + 8;
+            m = GzinStream::Member();
+            members += 1;
+            after = true;
+            continue;
+        }
+        if (m.in) {
+            GuWalk r;
+            long long b;
+            if ((rc = bound(p, &b)) != CG_OK) return rc;
+            if ((rc = gzin_blocks(c, g, n, b, p * 8 + m.bitoff, base, st, &r, &respec)) != CG_OK) return rc;
+            if (r.status == GU_INVALID) return bad_member();
+            if (r.status == GU_UNSUPPORTED) {
+                if (base == g.carry && p == 0 && !members)
+                    return fail(CG_EUNSUPPORTED, "gzip input: a stretch of deflate blocks of the member at byte " +
+                                                     std::to_string(m.start) +
+                                                     " inflates to more than one submission can hold (2 GiB); "
+                                                     "decompress this input on the host");
+                break;
+            }
+            base += r.plain;
+            p = r.end >> 3;
+            m.bitoff = (int)(r.end & 7);
+            if (r.last) {
+                m.trailer = 1;
+                continue;
+            }
+            if (r.more && final) return bad_member();
+            break;
+        }
+        GuChain ch;
+        if ((rc = gzin_members(c, g, n, n_cand, p, after, final, base, true, st, &ch)) != CG_OK) return rc;
+        if (ch.status == GU_UNSUPPORTED) {
+            if (base == g.carry && p == 0 && !members)
+                return fail(CG_EUNSUPPORTED, "gzip input: the member at byte " + std::to_string(g.consumed + ch.err_at) +
+                                                 " inflates to more than one submission can hold (2 GiB); decompress "
+                                                 "this input on the host");
+        }
+        base += ch.plain;
+        members += ch.n_members;
+        after = after || ch.n_members > 0;
+        p = ch.consumed;
+        if (ch.status != GU_LONG) break;
+        m.in = 1;
+        m.crc = 0xffffffffu;
+        m.start = g.consumed + ch.err_at;
+        p = ch.err_at + gu_head(gz + ch.err_at, n - ch.err_at);
+    }
+    g.pend_plain = base - g.carry;
+    g.pend_consumed = p;
+    g.pend_members = members;
+    g.pend_respec = respec;
+    res->consumed = p;
+    res->members = members;
+    res->plain_bytes = base - g.carry;
+    res->in_member = m.in;
+    res->respeculated = respec;
+    *fin = final && p == n && !m.in;
     return CG_OK;
 }
 
@@ -1823,54 +2115,14 @@ static int gzin_inflate(cg_ctx *c, GzinStream &g, const uint8_t *gz, int64_t n, 
     if ((rc = g.d_res.ensure((size_t)n_cand + 1)) != CG_OK) return rc;
     if ((rc = g.d_members.ensure((size_t)n_cand + 1)) != CG_OK) return rc;
     if ((rc = g.d_moff.ensure((size_t)n_cand + 1)) != CG_OK) return rc;
-    GuChain *d_chain = reinterpret_cast<GuChain *>(g.d_small.p + 4);
     if (n_cand) {
         CU(cg_launch_gunzip_candidates(1, g.d_gz.p, n, nullptr, g.d_offs.p, g.d_cand.p, st));
-        CU(cg_launch_gunzip_parse(g.d_gz.p, n, g.d_cand.p, (int)n_cand, g.d_res.p, st));
+        CU(cg_launch_gunzip_parse(g.d_gz.p, n, g.d_cand.p, (int)n_cand, g.split ? CG_GZIN_LONG_MEMBER : 0, g.d_res.p, st));
         c->launches += 2;
     }
-    CU(cg_launch_gunzip_chain(g.d_gz.p, n, g.d_cand.p, g.d_res.p, (int)n_cand, g.members > 0, final, g.carry,
-                              CG_GZIN_LIMIT, g.d_members.p, g.d_moff.p, d_chain, st));
-    c->launches += 1;
+    if (g.split) return gzin_inflate_split(c, g, gz, n, (int)n_cand, final, st, res, fin);
     GuChain ch;
-    CU(cudaMemcpyAsync(&ch, d_chain, sizeof ch, cudaMemcpyDeviceToHost, st));
-    CU(cudaStreamSynchronize(st));
-    const long long at = g.consumed + ch.err_at;
-    if (ch.status == GU_INVALID)
-        return fail(CG_EINVAL, "gzip input: invalid or truncated gzip member at byte " + std::to_string(at) +
-                                   " of the compressed file");
-    if (ch.status == GU_UNSUPPORTED)
-        return fail(CG_EUNSUPPORTED, "gzip input: the member at byte " + std::to_string(at) +
-                                         " inflates to more than one submission can hold (2 GiB); decompress this input "
-                                         "on the host");
-    // the carry stays where it is; a larger buffer gets a copy of it
-    const long long total = g.carry + ch.plain;
-    if ((size_t)total + 64 > g.d_plain.cap) {
-        DevBuf<uint8_t> nb;
-        if ((rc = nb.ensure((size_t)total + 64)) != CG_OK) return rc;
-        if (g.carry) CU(cudaMemcpyAsync(nb.p, g.d_plain.p, (size_t)g.carry, cudaMemcpyDeviceToDevice, st));
-        CU(cudaStreamSynchronize(st));
-        g.d_plain.release();
-        g.d_plain = nb;
-    }
-    if (ch.n_members) {
-        int *d_bad = reinterpret_cast<int *>(g.d_small.p + 2);
-        const int none = 0x7FFFFFFF;
-        CU(cudaMemcpyAsync(d_bad, &none, sizeof none, cudaMemcpyHostToDevice, st));
-        CU(cg_launch_gunzip_place(g.d_gz.p, n, g.d_cand.p, g.d_members.p, g.d_moff.p, d_chain, ch.n_members, g.d_res.p,
-                                  g.d_plain.p, d_bad, st));
-        c->launches += 2;
-        int bad = none;
-        CU(cudaMemcpyAsync(&bad, d_bad, sizeof bad, cudaMemcpyDeviceToHost, st));
-        CU(cudaStreamSynchronize(st));
-        if (bad != none) {
-            int32_t k = 0, pos = 0;
-            CU(cudaMemcpy(&k, g.d_members.p + bad, sizeof k, cudaMemcpyDeviceToHost));
-            CU(cudaMemcpy(&pos, g.d_cand.p + k, sizeof pos, cudaMemcpyDeviceToHost));
-            return fail(CG_EINVAL, "gzip input: CRC-32 mismatch in the gzip member at byte " +
-                                       std::to_string(g.consumed + pos) + " of the compressed file");
-        }
-    }
+    if ((rc = gzin_members(c, g, n, (int)n_cand, 0, g.members > 0, final, g.carry, false, st, &ch)) != CG_OK) return rc;
     g.pend_plain = ch.plain;
     g.pend_consumed = ch.consumed;
     g.pend_members = ch.n_members;
@@ -1962,6 +2214,10 @@ static int gzin_commit(cg_ctx *c, GzinStream &g, FastqSlot *f, long long cut, lo
     g.consumed += g.pend_consumed;
     g.members += g.pend_members;
     g.pend_plain = g.pend_consumed = g.pend_members = 0;
+    if (g.split) {
+        g.mem = g.pmem;
+        if (g.mem.in) std::swap(g.d_win, g.d_pwin);
+    }
     CU(cudaEventRecord(g.done, st));
     res->chunk_bytes = f ? cut : 0;
     res->carry_bytes = g.carry;

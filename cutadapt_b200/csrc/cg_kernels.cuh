@@ -211,11 +211,29 @@ cudaError_t cg_launch_gzip_gather(const uint8_t *d_slots, const int32_t *d_sizes
 long long cg_gunzip_tiles(long long n_bytes);
 cudaError_t cg_launch_gunzip_candidates(int phase, const uint8_t *d_gz, long long n, int32_t *d_counts,
                                         const int64_t *d_offs, int32_t *d_cand, cudaStream_t st);
-cudaError_t cg_launch_gunzip_parse(const uint8_t *d_gz, long long n, const int32_t *d_cand, int n_cand, GuMember *d_res,
-                                   cudaStream_t st);
+cudaError_t cg_launch_gunzip_parse(const uint8_t *d_gz, long long n, const int32_t *d_cand, int n_cand, long long budget,
+                                   GuMember *d_res, cudaStream_t st);
 cudaError_t cg_launch_gunzip_chain(const uint8_t *d_gz, long long n, const int32_t *d_cand, const GuMember *d_res,
                                    int n_cand, int after_member, int final, long long base, long long limit,
-                                   int32_t *d_members, long long *d_moff, GuChain *d_chain, cudaStream_t st);
+                                   int32_t *d_members, long long *d_moff, GuChain *d_chain, long long from, int split,
+                                   cudaStream_t st);
+// Block path of one member (split streams): the start search of chunks 1..K-1 (warp per chunk); the speculative decode
+// of the listed chunks (d_list == nullptr: chunks 0..n_list-1) into d_sym + d_off[k] with d_room[k] symbols; the walk
+// (one thread); the windows (d_win: (n_ok + 1) x GU_WIN bytes, the first one the member's window so far) and the
+// resolve of the n_ok confirmed chunks into d_out (*d_bad: the first chunk with a marker in front of the member, start
+// it at INT_MAX); the raw CRC-32 register *d_state advanced over d_plain[0, len) (d_part: len / cg_gunzip_crc_piece()).
+cudaError_t cg_launch_gunzip_search(const uint8_t *d_gz, long long n, long long s0, long long stride, int K, GuChunk *d_ch,
+                                    cudaStream_t st);
+cudaError_t cg_launch_gunzip_spec(const uint8_t *d_gz, long long n, long long s0, long long stride, int K,
+                                  const int32_t *d_list, int n_list, const long long *d_off, const long long *d_room,
+                                  uint16_t *d_sym, GuChunk *d_ch, cudaStream_t st);
+cudaError_t cg_launch_gunzip_walk(GuChunk *d_ch, int K, long long limit, int32_t *d_redo, GuWalk *d_walk, cudaStream_t st);
+cudaError_t cg_launch_gunzip_resolve(const GuChunk *d_ch, int n_ok, long long max_n, const long long *d_off,
+                                     const uint16_t *d_sym, uint8_t *d_win, long long mpos, uint8_t *d_out, int *d_bad,
+                                     cudaStream_t st);
+int cg_gunzip_crc_piece();
+cudaError_t cg_launch_gunzip_crc(const uint8_t *d_plain, long long len, uint32_t *d_part, uint32_t *d_state,
+                                 cudaStream_t st);
 cudaError_t cg_launch_gunzip_place(const uint8_t *d_gz, long long n, const int32_t *d_cand, const int32_t *d_members,
                                    const long long *d_moff, const GuChain *d_chain, int n_members, const GuMember *d_res,
                                    uint8_t *d_out, int *d_bad, cudaStream_t st);

@@ -829,9 +829,12 @@ class DeviceChunk:
 class _GzipInput:
     """One compressed input file on a context (cg_gzin_create): the bytes read but not yet consumed, and the carry."""
 
-    def __init__(self, ctx, f, buffer_size: int):
+    def __init__(self, ctx, f, buffer_size: int, split_members: bool = False):
         h = C.c_int32(0)
-        _lib.check(_lib.lib().cg_gzin_create(ctx.handle, C.byref(h)))
+        if split_members:
+            _lib.check(_lib.lib().cg_gzin_create_ex(ctx.handle, _lib.CG_GZIN_SPLIT_MEMBERS, C.byref(h)))
+        else:
+            _lib.check(_lib.lib().cg_gzin_create(ctx.handle, C.byref(h)))
         self.ctx, self.handle, self.f = ctx, h.value, f
         self.buf, self.end, self.eof = bytearray(buffer_size), 0, False
 
@@ -867,7 +870,7 @@ def _add_gzip_bytes(statistics: dict, n: int):
     statistics["in_bytes_gzip"] = statistics.get("in_bytes_gzip", 0) + n
 
 
-def read_gzip_device_chunks(f, trimmer, buffer_size: int = 4 * 1024 * 1024):
+def read_gzip_device_chunks(f, trimmer, buffer_size: int = 4 * 1024 * 1024, split_members: bool = False):
     """
     Chunks of a gzip file (a binary file object of the compressed bytes) inflated on the device
     (``cg_fastq_submit_gzip``): every member is inflated on the GPU and the plain bytes never cross PCIe.  Yields
@@ -875,9 +878,11 @@ def read_gzip_device_chunks(f, trimmer, buffer_size: int = 4 * 1024 * 1024):
     records of read_fastq_chunks / read_fasta_chunks).  A chunk is submitted when the generator is advanced, so the
     trimmer's one chunk in flight stays as it is.  ``trimmer.statistics["in_bytes_gzip"]`` counts the compressed bytes
     consumed.  Meant for files of many members (BGZF, concatenated .gz files, this project's gzip outputs); a member
-    that does not fit one submission makes the buffer grow.
+    that does not fit one submission makes the buffer grow.  ``split_members=True`` (``CG_GZIN_SPLIT_MEMBERS``) inflates
+    a long member -- the one member of a file from ``gzip`` or ``pigz`` -- block-parallel instead, over as many
+    submissions as it takes.
     """
-    g = _GzipInput(trimmer.ctx, f, buffer_size)
+    g = _GzipInput(trimmer.ctx, f, buffer_size, split_members)
     try:
         while not g.done:
             g.fill()
@@ -892,11 +897,11 @@ def read_gzip_device_chunks(f, trimmer, buffer_size: int = 4 * 1024 * 1024):
         g.close()
 
 
-def read_gzip_device_interleaved_chunks(f, trimmer, buffer_size: int = 4 * 1024 * 1024):
+def read_gzip_device_interleaved_chunks(f, trimmer, buffer_size: int = 4 * 1024 * 1024, split_members: bool = False):
     """read_gzip_device_chunks for an interleaved file and a PairedFastqTrimmer: every chunk holds whole pairs (the
     cuts of read_interleaved_fastq_chunks / read_interleaved_fasta_chunks) and is split on the device as
     ``cg_fastq_submit_interleaved`` splits it.  Pass each chunk with ``chunk2=None``."""
-    g = _GzipInput(trimmer.ctx, f, buffer_size)
+    g = _GzipInput(trimmer.ctx, f, buffer_size, split_members)
     try:
         while not g.done:
             g.fill()
@@ -912,10 +917,12 @@ def read_gzip_device_interleaved_chunks(f, trimmer, buffer_size: int = 4 * 1024 
         g.close()
 
 
-def read_gzip_device_paired_chunks(f1, f2, trimmer, buffer_size: int = 4 * 1024 * 1024):
+def read_gzip_device_paired_chunks(f1, f2, trimmer, buffer_size: int = 4 * 1024 * 1024, split_members=False):
     """read_gzip_device_chunks for the two files of a pair and a PairedFastqTrimmer: yields (chunk1, chunk2) with the
-    same number of records (read_paired_fastq_chunks / read_paired_fasta_chunks)."""
-    g1, g2 = _GzipInput(trimmer.ctx, f1, buffer_size), _GzipInput(trimmer.ctx, f2, buffer_size)
+    same number of records (read_paired_fastq_chunks / read_paired_fasta_chunks).  split_members: a bool for both
+    files, or a pair of them."""
+    sp1, sp2 = split_members if isinstance(split_members, (tuple, list)) else (split_members, split_members)
+    g1, g2 = _GzipInput(trimmer.ctx, f1, buffer_size, sp1), _GzipInput(trimmer.ctx, f2, buffer_size, sp2)
     try:
         while not (g1.done and g2.done):
             g1.fill()

@@ -400,9 +400,26 @@ typedef struct cg_gzin_result {
     int64_t chunk_bytes;   /* bytes of the chunk in the slot (0 without a slot) */
     int64_t carry_bytes;   /* plain bytes kept for the next submission */
     int64_t n_records;     /* records of the chunk (pairs count two) */
-    int64_t reserved[2];
+    int64_t in_member;     /* split streams: 1 when `consumed` stopped inside a member (else 0) */
+    int64_t respeculated;  /* split streams: chunks decoded again because their speculative start was wrong */
 } cg_gzin_result;
 int cg_gzin_create(cg_ctx *ctx, int32_t *handle);
+/* cg_gzin_create with flags.  CG_GZIN_SPLIT_MEMBERS: a member that runs past the bytes given, or that is longer than
+ * CG_GZIN_LONG_MEMBER compressed bytes, is inflated block-parallel (speculative block starts every CG_GZIN_STRIDE
+ * compressed bytes, back-references into the unknown window resolved afterwards) and may be consumed in part: then
+ * `consumed` stops at a deflate block boundary inside it and in_member is 1.  The stream keeps the bit offset into the
+ * first byte passed again, the member's last 32 KiB of plain bytes, its running CRC-32 and length, and its offset in
+ * the file; the caller still passes the unconsumed bytes again.  Such a member may exceed 2 GiB (it streams over
+ * submissions); CG_EUNSUPPORTED remains for a stretch of deflate blocks that alone reaches the limit.  Every other
+ * member, and every result field, is as on a default stream.  Any other flag bit is CG_EINVAL.
+ * The environment variable CUTADAPT_B200_GZIN_STRIDE, read when a split stream is created, replaces CG_GZIN_STRIDE
+ * (in bytes, at least 32 KiB) for that stream; tools/measure_fastq.py --gzip-input sweeps it.
+ * Device memory of a split stream, held until cg_gzin_destroy: 16 bytes of symbol room per compressed byte of the
+ * largest submission (grown for chunks that inflate further), 32 KiB of window per chunk, and the plain bytes. */
+#define CG_GZIN_SPLIT_MEMBERS 1
+#define CG_GZIN_LONG_MEMBER (64 * 1024)
+#define CG_GZIN_STRIDE (64 * 1024)
+int cg_gzin_create_ex(cg_ctx *ctx, int32_t flags, int32_t *handle);
 int cg_gzin_destroy(cg_ctx *ctx, int32_t handle);
 int cg_fastq_submit_gzip(cg_ctx *ctx, int32_t handle, const uint8_t *gz, int64_t n_bytes, int32_t format, int32_t final,
                          int32_t *slot, cg_gzin_result *res);

@@ -29,10 +29,15 @@ each of two inputs of the same reads (-a AGATCGGAAGAGC -q 20 -m 20, plain output
 plain bytes), "host_gzip" (Python's gzip module on one core, the tool's path for single-member files) and "device"
 (read_gzip_device_chunks: the compressed bytes are uploaded and inflated on the device).  Inputs: "multi_member"
 (members of 65 280 plain bytes at zlib level 6), "mib_members" (members of 2 MiB plain, about 1 MiB compressed: the
-tool's threshold) and "single_member" (one zlib level 6 member).  One thread inflates a
-member, so the device arm of the single-member input runs on its first 8 MiB only and is reported per MiB.  Per arm:
-host-to-host reads/s and MiB/s of plain input, and the bytes uploaded.  A last line: the inflate kernels' device time
-per MiB of plain output from torch.profiler in a run of its own.  The card's name and power limit are read in the run.
+tool's threshold) and "single_member" (one zlib level 6 member), whose device arm reads the whole input on a split
+stream (split_members=True: the member inflated block-parallel).  Per arm: host-to-host reads/s and MiB/s of plain
+input, and the bytes uploaded.  Then, on the single member: the stride sweep (CUTADAPT_B200_GZIN_STRIDE of 32, 64, 128
+and 256 KiB, two rounds alternating), with the chunks decoded again because their speculative start was wrong
+(cg_gzin_result.respeculated, from an untimed pass per stride) against the chunks searched; the file-size sweep of the
+tool's rule (prefixes of the reads compressed as one member of about 4 to 64 MiB, host gzip against the split stream,
+three rounds alternating) and the smallest size from which the device wins at every larger size.  Last lines: the
+inflate kernels' device time per MiB of plain output from torch.profiler, in runs of their own, on the multi-member
+input and on the split stream.  The card's name and power limit are read in the run.
 """
 import json
 import subprocess
@@ -188,7 +193,6 @@ def measure_gzip_input(n, submit_mb):
     big = [plain[i:i + (2 << 20)] for i in range(0, len(plain), 2 << 20)]
     with ThreadPoolExecutor(16) as ex:
         mib = b"".join(ex.map(lambda p: gzip.compress(p, 6, mtime=0), big))
-    small = len(plain) if len(plain) <= 8 << 20 else (8 << 20) // rec_len * rec_len
     inputs = {"multi_member": (multi, plain), "mib_members": (mib, plain), "single_member": (single, plain)}
     adapters = [PA.BackAdapter("AGATCGGAAGAGC", max_errors=0.1)]
     opts = dict(quality_cutoff=(0, 20), minimum_length=20)
@@ -201,7 +205,7 @@ def measure_gzip_input(n, submit_mb):
         elif arm == "host_gzip":
             src = read_fastq_chunks(gzip.GzipFile(fileobj=io.BytesIO(gz)), chunk)
         else:
-            src = read_gzip_device_chunks(io.BytesIO(gz), t, submit_mb << 20)
+            src = read_gzip_device_chunks(io.BytesIO(gz), t, submit_mb << 20, split_members=arm == "split")
         t.ctx.transfer_bytes(reset=True)
         t0 = time.perf_counter()
         out = sum(len(o) for o in t.process_chunks(src, copy=False))
@@ -209,11 +213,10 @@ def measure_gzip_input(n, submit_mb):
 
     card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader",
                            "-i", str(torch.cuda.current_device())], capture_output=True, text=True).stdout.strip()
-    single_small = gzip.compress(plain[:small], 6, mtime=0)
     res = {}
     for name, (gz, pl) in inputs.items():
-        arms = {"plain": (gz, pl), "host_gzip": (gz, pl),
-                "device": (gz, pl) if name != "single_member" else (single_small, plain[:small])}
+        dev = "split" if name == "single_member" else "device"
+        arms = {"plain": (gz, pl), "host_gzip": (gz, pl), dev: (gz, pl)}
         warm = plain[:rec_len * 1000]
         for arm in arms:                          # warm-up: buffers, module load
             run(arm, gzip.compress(warm, 6), warm)
@@ -235,23 +238,101 @@ def measure_gzip_input(n, submit_mb):
                       "submission_MiB": submit_mb, "gpu": torch.cuda.get_device_name(), "card_and_power_limit": card,
                       "inputs": res}))
 
+    # the stride sweep on the single member
+    import os
+
+    from cutadapt_b200 import _lib
+    from cutadapt_b200.pipeline import DeviceChunk
+
+    def respeculated(gz):
+        """(chunks decoded again, chunks searched) of one untimed pass, submissions as the reader makes them."""
+        import ctypes as C
+
+        stride = int(os.environ["CUTADAPT_B200_GZIN_STRIDE"])
+        t = FastqTrimmer(adapters, **opts)
+        h = C.c_int32(0)
+        _lib.check(_lib.lib().cg_gzin_create_ex(t.ctx.handle, _lib.CG_GZIN_SPLIT_MEMBERS, C.byref(h)))
+        pos, buf, again, searched = 0, b"", 0, 0
+        try:
+            while True:
+                take = gz[pos:pos + (submit_mb << 20) - len(buf)]
+                pos += len(take)
+                buf += take
+                final = pos >= len(gz)
+                slot, r = C.c_int32(-1), _lib.cg_gzin_result()
+                _lib.check(_lib.lib().cg_fastq_submit_gzip(t.ctx.handle, h.value, buf, len(buf), 0, int(final),
+                                                           C.byref(slot), C.byref(r)))
+                again += r.respeculated
+                searched += max(0, (len(buf) + stride - 1) // stride - 1)
+                if slot.value >= 0:
+                    t.process_chunk(DeviceChunk(slot.value, r.chunk_bytes))
+                buf = buf[r.consumed:]
+                if final and not buf:
+                    return again, searched
+        finally:
+            _lib.check(_lib.lib().cg_gzin_destroy(t.ctx.handle, h.value))
+
+    strides = [32 << 10, 64 << 10, 128 << 10, 256 << 10]
+    sweep = {s: {"wall_s": 0.0} for s in strides}
+    for _ in range(2):
+        for s in strides:
+            os.environ["CUTADAPT_B200_GZIN_STRIDE"] = str(s)
+            w, out, _ = run("split", single, plain)
+            sweep[s]["wall_s"] += w
+            outs.setdefault(len(plain), set()).add(out)
+    for s in strides:
+        os.environ["CUTADAPT_B200_GZIN_STRIDE"] = str(s)
+        again, searched = respeculated(single)
+        sweep[s].update(M_reads_per_s=2 * n / sweep[s]["wall_s"] / 1e6, respeculated=again, chunks_searched=searched,
+                        false_start_rate=again / max(searched, 1))
+    os.environ.pop("CUTADAPT_B200_GZIN_STRIDE")
+    assert all(len(v) == 1 for v in outs.values()), "the arms wrote different amounts"
+    print(json.dumps({"what": "split stream on the single member by stride S (bytes)", "reads": n,
+                      "card_and_power_limit": card, "strides": sweep}))
+
+    # the file-size sweep of the tool's rule: one member of about `mib` MiB compressed
+    ratio = len(single) / len(plain)
+    sizes = {}
+    for mib_gz in (4, 8, 16, 32, 64):
+        k = min(len(plain), int((mib_gz << 20) / ratio) // rec_len * rec_len)
+        sizes[mib_gz] = (gzip.compress(plain[:k], 6, mtime=0), plain[:k])
+    size_res = {m: {"host_gzip": 0.0, "split": 0.0, "gz_bytes": len(g)} for m, (g, _) in sizes.items()}
+    for _ in range(3):
+        for m, (g, p) in sizes.items():
+            for arm in ("host_gzip", "split"):
+                size_res[m][arm] += run(arm, g, p)[0]
+    win = None
+    for m in sorted(size_res, reverse=True):
+        x = size_res[m]
+        x["speedup"] = x["host_gzip"] / x["split"]
+        if x["speedup"] > 1:
+            win = m
+        else:
+            break
+    print(json.dumps({"what": "one member by compressed size: host gzip against the split stream (wall s, 3 rounds)",
+                      "card_and_power_limit": card, "sizes_MiB": size_res,
+                      "device_wins_from_MiB": win}))
+
     from torch.profiler import ProfilerActivity, profile
 
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        run("device", multi, plain)
-        torch.cuda.synchronize()
-    ms, launches = {}, {}
-    for ev in prof.key_averages():
-        for k in ("gu_cand_count", "gu_cand_write", "gu_parse", "gu_chain", "gu_place", "gu_crc", "gu_flag", "gu_select"):
-            if k + "_kernel" in ev.key:
-                ms[k] = ms.get(k, 0.0) + ev.device_time_total / 1000.0
-                launches[k] = launches.get(k, 0) + ev.count
-    if "gu_parse" not in ms:
-        raise RuntimeError("the profiler saw no gu_parse_kernel launch")
-    mib = len(plain) / 2**20
-    print(json.dumps({"what": "inflate kernels' device time on the multi-member input (torch.profiler, CUDA activity)",
-                      "card_and_power_limit": card, "ms_per_MiB_plain": {k: v / mib for k, v in ms.items()},
-                      "ms_per_MiB_plain_total": sum(ms.values()) / mib, "launches": launches}))
+    kernels = ("gu_cand_count", "gu_cand_write", "gu_parse", "gu_chain", "gu_place", "gu_crc", "gu_flag", "gu_select",
+               "gu_search", "gu_spec", "gu_walk", "gu_window", "gu_resolve", "gu_crc_piece", "gu_crc_fold")
+    for name, arm, gz in (("multi-member input", "device", multi), ("single member, split stream", "split", single)):
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            run(arm, gz, plain)
+            torch.cuda.synchronize()
+        ms, launches = {}, {}
+        for ev in prof.key_averages():
+            for k in kernels:
+                if "::" + k + "_kernel" in ev.key or ev.key.startswith(k + "_kernel"):
+                    ms[k] = ms.get(k, 0.0) + ev.device_time_total / 1000.0
+                    launches[k] = launches.get(k, 0) + ev.count
+        if not ms:
+            raise RuntimeError("the profiler saw no inflate kernel launch")
+        mib = len(plain) / 2**20
+        print(json.dumps({"what": "inflate kernels' device time on the %s (torch.profiler, CUDA activity)" % name,
+                          "card_and_power_limit": card, "ms_per_MiB_plain": {k: v / mib for k, v in ms.items()},
+                          "ms_per_MiB_plain_total": sum(ms.values()) / mib, "launches": launches}))
 
 
 def main():

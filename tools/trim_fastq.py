@@ -32,8 +32,9 @@ error.  A .gz output
 that receives no read still gets one empty gzip member.  The device has one compression strategy, comparable in size to
 zlib's level 1, so there is no --compression-level.  An input ending in .gz whose first gzip member ends within its
 first MiB (BGZF, concatenated .gz files, this tool's own .gz outputs) is inflated on the device: the compressed bytes are
-uploaded (read_gzip_device_chunks; for two paired inputs only when both qualify).  Any other .gz input is decompressed on
-the host with Python's gzip module.  The outputs are the same either way; the stderr line's "in_bytes_gzip" (the
+uploaded (read_gzip_device_chunks; for two paired inputs only when each qualifies under either rule).  Any other .gz
+input of at least 16 MiB (DEVICE_GZIP_SPLIT_MIN; the single member that gzip and pigz write) is inflated on the device
+block-parallel (split_members=True).  Smaller ones are decompressed on the host with Python's gzip module.  The outputs are the same either way; the stderr line's "in_bytes_gzip" (the
 compressed bytes consumed) appears only when the device inflated the input.  The format is detected from the first
 decompressed byte.
 """
@@ -41,6 +42,7 @@ import argparse
 import gzip
 import zlib
 import json
+import os
 import sys
 
 sys.path.insert(0, __file__.rsplit("/", 2)[0])
@@ -76,6 +78,23 @@ def gzip_on_device(path):
     except zlib.error:
         return False                              # the host path reports the error as Python's gzip module does
     return d.eof
+
+
+# A .gz input that fails gzip_on_device (typically the one member written by gzip or pigz) still goes to the device when
+# it holds at least this many compressed bytes: read_gzip_device_chunks(split_members=True) inflates the member
+# block-parallel.  Measured by file size (DESIGN.md section 4.8): the device wins from 16 MiB on and loses at 8 MiB,
+# where one submission holds too few deflate blocks to occupy the GPU.
+DEVICE_GZIP_SPLIT_MIN = 16 << 20
+
+
+def gzip_route(path):
+    """How a .gz input is read: "members" (gzip_on_device), "split" (a long member of a file of at least
+    DEVICE_GZIP_SPLIT_MIN compressed bytes, inflated block-parallel on the device) or None (Python's gzip module)."""
+    if gzip_on_device(path):
+        return "members"
+    if path.endswith(".gz") and os.path.getsize(path) >= DEVICE_GZIP_SPLIT_MIN:
+        return "split"
+    return None
 
 
 def detect_format(path):
@@ -261,9 +280,10 @@ def main():
 
     def single_input(t):
         """(file, chunks) of the single input for trimmer t."""
-        if gzip_on_device(args.inputs[0]):
+        route = gzip_route(args.inputs[0])
+        if route:
             f = open(args.inputs[0], "rb")
-            return f, read_gzip_device_chunks(f, t, gz_buffer)
+            return f, read_gzip_device_chunks(f, t, gz_buffer, split_members=route == "split")
         f = open_input(args.inputs[0])
         return f, host_reader(f, args.buffer_size)
     paired_reader = read_paired_fasta_chunks if input_format == "fasta" else read_paired_fastq_chunks
@@ -307,15 +327,16 @@ def main():
                        if not (args.paired_output if d == "output" else getattr(args, d + "_paired_output"))]
         t = PairedFastqTrimmer(ads1, ads2, common, options2, args.pair_filter, **formats, **split,
                                interleaved_outputs=interleaved, gzip_outputs=gzip1, gzip_outputs2=gzip2)
-        if len(args.inputs) == 2 and all(map(gzip_on_device, args.inputs)):
+        routes = [gzip_route(p) for p in args.inputs]
+        if len(args.inputs) == 2 and all(routes):
             f1, f2 = open(args.inputs[0], "rb"), open(args.inputs[1], "rb")
-            chunks = read_gzip_device_paired_chunks(f1, f2, t, gz_buffer)
+            chunks = read_gzip_device_paired_chunks(f1, f2, t, gz_buffer, split_members=tuple(r == "split" for r in routes))
         elif len(args.inputs) == 2:
             f1, f2 = open_input(args.inputs[0]), open_input(args.inputs[1])
             chunks = paired_reader(f1, f2, args.buffer_size)
-        elif gzip_on_device(args.inputs[0]):
+        elif routes[0]:
             f1 = f2 = open(args.inputs[0], "rb")
-            chunks = read_gzip_device_interleaved_chunks(f1, t, gz_buffer)
+            chunks = read_gzip_device_interleaved_chunks(f1, t, gz_buffer, split_members=routes[0] == "split")
         else:
             f1 = f2 = open_input(args.inputs[0])
             chunks = (read_interleaved_fasta_chunks if input_format == "fasta" else read_interleaved_fastq_chunks)(
