@@ -204,10 +204,11 @@ struct cg_ctx {
     DevBuf<int> scratch_w;
     DevBuf<unsigned long long> d_stats;  // cg_process_batch_stats: the statistics vector of the batch in flight
     // statistics wanted together with the next trimming pass (launch_trim_with_stats): the split pipeline counts the
-    // reads its first stage settles while it has them in shared memory and the others from its task list
+    // reads its first stage settles while it has them in shared memory, the plan and run kernels list the others
     struct { unsigned long long *d_stats = nullptr; int max_len = 0, kmax = 0; bool armed = false, done = false; } fuse;
     DevBuf<uint4> tasks;                 // split pipeline: 2 x uint4 per read of a sub-batch
     DevBuf<uint4> tasks2, tasks3;        // run-record lists (ping-pong): 4 x uint4 per read of a sub-batch
+    DevBuf<uint2> stat_ents;             // fused statistics: one entry per read the plan and run kernels finish
     unsigned long long *d_task_count = nullptr;
     DevBuf<cg_match_rec> pass_tmp;       // multi-pass schedule: records of every pass for one sub-batch
     DevBuf<int32_t> view_base, view_back;
@@ -337,7 +338,7 @@ extern "C" int cg_ctx_destroy(cg_ctx *c)
         l.h_seq.release(); l.h_qual.release(); l.h_offs.release(); l.h_out.release(); l.h_qtrim.release();
         if (l.stream) cudaStreamDestroy(l.stream);
     }
-    c->scratch_p.release(); c->scratch_w.release(); c->tasks.release(); c->tasks2.release(); c->tasks3.release();
+    c->scratch_p.release(); c->scratch_w.release(); c->tasks.release(); c->tasks2.release(); c->tasks3.release(); c->stat_ents.release();
     c->pass_tmp.release(); c->view_base.release(); c->view_back.release();
     for (FastqSlot &f : c->fq) {
         f.d_in.release(); f.d_out.release(); f.d_seq.release(); f.d_qual.release(); f.d_tiles.release(); f.d_nl.release();
@@ -611,8 +612,8 @@ static int launch_trim_single(cg_ctx *c, const cg_adapterset *s, const uint8_t *
             if (scan_smem <= c->smem_optin && list_smem <= c->smem_optin) {
                 if (plane_w) CU(cg_pscan_occupancy(want_q, plane_w, false, scan_smem, &scan_occ));
                 else CU(cg_scan_occupancy(want_q, scan_smem, &scan_occ));
-                CU(cg_list_occupancy(true, s->host.max_m, list_smem, &plan_occ));
-                CU(cg_list_occupancy(false, s->host.max_m, list_smem, &run_occ));
+                CU(cg_list_occupancy(true, s->host.max_m, false, list_smem, &plan_occ));
+                CU(cg_list_occupancy(false, s->host.max_m, false, list_smem, &run_occ));
                 split = scan_occ >= 1 && plan_occ >= 1 && run_occ >= 1;
             }
         }
@@ -636,17 +637,23 @@ static int launch_trim_single(cg_ctx *c, const cg_adapterset *s, const uint8_t *
     // statistics counted inside the pass: one plain adapter, one round, the whole set in this call (not a pass of the
     // multi-pass schedule), no quality trimming, and the first stage keeps its CTAs per SM with the histogram in shared
     // memory.  The first stage counts the reads it settles (88 % on the benchmark's reads) while they are in shared
-    // memory, one cg_stats_kernel launch per sub-batch counts the rest from the task list; otherwise
-    // launch_trim_with_stats runs cg_stats_kernel over all records after the pass.  Measured on an H100 (DESIGN.md
-    // section 4.1): 1.4 ms less per step of config 2; with quality trimming (config 4) the first stage grew by more than
+    // memory; the plan and run kernels list an entry for each of the others where they write its final record, and one
+    // cg_stats_entries_kernel launch per sub-batch counts them (its histograms must fit 48 KiB of shared memory).
+    // Otherwise launch_trim_with_stats runs cg_stats_kernel over all records after the pass.
+    // Measured on an H100 (DESIGN.md section 4.1): with quality trimming (config 4) the first stage grew by more than
     // the statistics kernel costs, so quality-trimmed passes keep the kernel.
     bool fuse_stats = split && plane_w && c->fuse.armed && !d_view && s->host.n_adapters == 1 && times == 1 &&
-                      s->host.slots == 1 && !want_q && !getenv("CUTADAPT_B200_TWO_LISTS") && c->fuse.max_len <= 4096;
+                      s->host.slots == 1 && !want_q && !getenv("CUTADAPT_B200_TWO_LISTS") && c->fuse.max_len <= 4096 &&
+                      cg_stats_entries_smem_bytes(c->fuse.max_len, c->fuse.kmax) <= 48 * 1024;
     if (fuse_stats) {
         const size_t fsmem = cg_pscan_smem_bytes(a.blob_bytes, a.mini_cap, want_q, c->fuse.max_len);
         int focc = 0;
         if (fsmem <= c->smem_optin) CU(cg_pscan_occupancy(want_q, plane_w, true, fsmem, &focc));
-        fuse_stats = focc >= 1 && focc >= scan_occ;
+        // (the listing variants of the plan and run kernels: same shared memory, the attribute set for them too)
+        int pocc = 0, rocc = 0;
+        CU(cg_list_occupancy(true, s->host.max_m, true, list_smem, &pocc));
+        CU(cg_list_occupancy(false, s->host.max_m, true, list_smem, &rocc));
+        fuse_stats = focc >= 1 && focc >= scan_occ && pocc >= plan_occ && rocc >= run_occ;
         if (fuse_stats) {
             a.stats = c->fuse.d_stats; a.stats_max_len = c->fuse.max_len; a.stats_kmax = c->fuse.kmax;
             scan_smem = fsmem; scan_occ = focc;
@@ -722,6 +729,7 @@ static int launch_trim_single(cg_ctx *c, const cg_adapterset *s, const uint8_t *
         int rc = c->tasks.ensure((size_t)cap * plane_rec);
         if (rc == CG_OK) rc = c->tasks2.ensure((size_t)cap * 4);
         if (rc == CG_OK) rc = c->tasks3.ensure((size_t)cap * 4);
+        if (rc == CG_OK && fuse_stats) rc = c->stat_ents.ensure((size_t)cap);
         if (rc != CG_OK) return rc;
         unsigned long long *cnt = c->d_task_count;
         for (long long r0 = 0; r0 < n_reads; r0 += SUB) {
@@ -755,6 +763,7 @@ static int launch_trim_single(cg_ctx *c, const cg_adapterset *s, const uint8_t *
             else if (plane_w) CU(cg_launch_pscan(b, want_q, plane_w, grid_for(scan_occ), scan_smem, st));
             else CU(cg_launch_scan(b, want_q, grid_for(scan_occ), scan_smem, st));
             if (sev[0]) CU(cudaEventRecord(sev[1], st));
+            b.stat_ents = c->stat_ents.p; b.stat_count = cnt + 6;
             b.tasks2 = c->tasks2.p; b.task2_count = cnt + 1;
             b.tasks3 = c->tasks3.p; b.task3_count = cnt + 2;
             // run records of the plane path go to two lists (banded first runs / the others): cnt[5] counts the second
@@ -787,10 +796,9 @@ static int launch_trim_single(cg_ctx *c, const cg_adapterset *s, const uint8_t *
             }
             if (sev[0]) { CU(cudaEventRecord(sev[3], st)); c->stage_events.push_back(sev); }
             if (fuse_stats) {
-                // the reads the first stage handed on: their records are final now (the event pair of the call
-                // brackets these launches too)
-                CU(cg_launch_stats(b.seq, b.offsets, n_sub, want_q && b.qtrim, 1, 1, b.out, b.qtrim, 1, a.stats_max_len,
-                                   a.stats_kmax, a.stats, st, c->tasks.p, plane_rec, cnt));
+                // the reads the first stage handed on, as the plan and run kernels listed them (the event pair of the
+                // call brackets these launches too)
+                CU(cg_launch_stats_entries(c->stat_ents.p, cnt + 6, n_sub, a.stats_max_len, a.stats_kmax, a.stats, st));
                 c->launches += 1;
             }
         }
@@ -2788,7 +2796,7 @@ static int fastq_stage_stats(cg_ctx *c, FastqSlot &f, FqStage &g, int kmax, cuda
     CU(cudaMemsetAsync(f.d_fqstats.p, 0, total * sizeof(unsigned long long), st));
     if (g.d_matches && a.n_adapters > 0) {
         CU(cg_launch_stats(f.d_seq.p, f.d_offs.p, g.n, g.d_qtrim != nullptr, g.times, g.slots, g.d_matches, g.d_qtrim,
-                           a.n_adapters, a.max_len, a.kmax, f.d_fqstats.p, st, nullptr, 0, nullptr, 0,
+                           a.n_adapters, a.max_len, a.kmax, f.d_fqstats.p, st, 0,
                            g.action == CG_FQ_ACTION_LOWERCASE ? 1 : 0));
         c->launches += 1;
     }

@@ -48,11 +48,14 @@ struct CgKernelArgs {
     uint4 *tasks3;                    // plan stage only: reads of cg_pscan_kernel whose window holds other letters than
     unsigned long long *task3_count;  //   A/C/G/T go here (2 x uint4, CG_TASK_RESCAN) for a second, dense plan launch
     int no_band;                      // 1: the DP runs keep all rows (CUTADAPT_B200_NO_BAND=1, for A/B runs)
-    // statistics fused into the first stage (cg_pscan.cuh): the reads it settles are counted here, the rest by
-    // cg_stats_kernel over the task list once their records are final.  null = not fused (the variant of the first
-    // stage without the statistics code runs).
+    // statistics fused into the pass: the first stage (cg_pscan.cuh) counts the reads it settles; the plan and run
+    // kernels (cg_list_kernel) list one entry per read they finish in stat_ents (counted in stat_count), which
+    // cg_stats_entries_kernel counts after the DP rounds.  null = not fused (the variants without the statistics code
+    // run).
     unsigned long long *stats;
     int stats_max_len, stats_kmax;
+    uint2 *stat_ents;
+    unsigned long long *stat_count;
     // generic-kernel scratch
     uint32_t *scratch_p;
     int *scratch_w;

@@ -765,6 +765,64 @@ __host__ __device__ inline DpSmem dp_smem_layout(uint32_t blob_bytes, int slot_b
 }
 size_t cg_dp_smem_bytes(uint32_t blob_bytes, int slot_bytes) { return dp_smem_layout(blob_bytes, slot_bytes).total; }
 
+// Fused statistics of the reads the list kernels finish (one round, one slot, no quality trimming: the only passes
+// that fuse the statistics, launch_trim_single): every lane that writes a final record now (fin; the window is the
+// whole read) appends what stats_read_core needs of it as one 8-byte entry to a.stat_ents, which
+// cg_stats_entries_kernel counts after the DP rounds -- a stream instead of the gather of every record and of the
+// base in front of its match.  Entry: x = read length | final length << 16, y = match | 3' side << 1 | adjacent-base
+// class << 2 | errors << 5 (at most 2047) | removed length << 16.  The base in front of a 3' match: in a DP round from
+// `slot`, this lane's staged bytes, where they hold it (only the run's columns are staged), otherwise -- and in the
+// plan stage -- from HBM (L2 serves it: the warp staged that read a moment ago).  All 32 lanes call it.
+template <bool PLAN>
+__device__ __forceinline__ void list_stats_append(const CgKernelArgs &a, const CgAdapter &A, bool fin, const CgHit &hit,
+                                                  const uint4 &ta, const uint4 &tc, const uint4 &td, const uint8_t *slot)
+{
+    uint32_t ex = 0, ey = 0;
+    if (fin) {
+        const int n = (int)ta.w;
+        int len = n;
+        if (hit.adapter >= 0) {
+            const bool after = hit.remove == CGK_REMOVE_AFTER;
+            int removed = after ? n - hit.rstart : hit.rstop;
+            removed = removed < 0 ? 0 : removed;
+            const int E = hit.errors < 0 ? 0 : (hit.errors > 2047 ? 2047 : hit.errors);
+            int k = 4;
+            if (after) {
+                if (hit.rstart > 0 && hit.rstart <= n) {
+                    // read position rstart - 1; a DP round's load_task staged the 16-byte pieces around the characters
+                    // [first, first + count) of the window (the run's columns, counted from the other end for
+                    // reversed reads)
+                    int first = 0, count = 0;
+                    if (!PLAN) {
+                        const int ri = (int)tc.z;
+                        const uint32_t pk = ri == 0 ? td.x : (ri == 1 ? td.y : (ri == 2 ? td.z : td.w));
+                        const int lo = (int)(pk & 0xffffu), hi = (int)(pk >> 16);
+                        count = hi > lo ? hi - lo : 0;
+                        first = A.reverse ? n - hi : lo;
+                    }
+                    const uintptr_t w0 = (uintptr_t)a.seq + (((uintptr_t)ta.y << 32) | ta.z);   // the window in HBM
+                    const uintptr_t s0 = (w0 + first) & ~(uintptr_t)15, s1 = (w0 + first + count + 15) & ~(uintptr_t)15;
+                    const uintptr_t at = w0 + (hit.rstart - 1);
+                    const uint8_t c = (count > 0 && at >= s0 && at < s1) ? slot[at - s0] : *(const uint8_t *)at;
+                    k = c == 'A' ? 0 : (c == 'C' ? 1 : (c == 'G' ? 2 : (c == 'T' ? 3 : 4)));
+                }
+                len = hit.rstart < 0 ? 0 : (hit.rstart > n ? n : hit.rstart);
+            } else {
+                len = n - (hit.rstop < 0 ? 0 : (hit.rstop > n ? n : hit.rstop));
+            }
+            ey = 1u | (after ? 2u : 0u) | ((uint32_t)k << 2) | ((uint32_t)E << 5) | ((uint32_t)removed << 16);
+        }
+        ex = (uint32_t)n | ((uint32_t)len << 16);
+    }
+    const uint32_t ballot = __ballot_sync(0xffffffffu, fin);
+    if (!ballot) return;
+    const int lane = threadIdx.x & 31;
+    unsigned long long base = 0;
+    if (lane == 0) base = atomicAdd(a.stat_count, (unsigned long long)__popc(ballot));
+    base = __shfl_sync(0xffffffffu, base, 0);
+    if (fin) a.stat_ents[base + __popc(ballot & ((1u << lane) - 1u))] = make_uint2(ex, ey);
+}
+
 // Common frame of the list-driven kernels: a warp walks groups of 32 list records; every lane
 // fetches the bytes its record needs into its own shared-memory slot with its own TMA bulk copy
 // (SASS: one UBLKCP per lane, one mbarrier per stage), double buffered against the work on the
@@ -788,7 +846,9 @@ size_t cg_dp_smem_bytes(uint32_t blob_bytes, int slot_bytes) { return dp_smem_la
 #ifndef CG_RUN48_BLOCKS
 #define CG_RUN48_BLOCKS 3      // resident CTAs per SM of the 48-row run kernel (168 registers, some spills; 2 = 255 registers)
 #endif
-template <bool PLAN, int MR>
+// STATS: the variant that lists the statistics of the reads it finishes (a.stats, list_stats_append); the other variant
+// carries none of that code.
+template <bool PLAN, int MR, bool STATS>
 __global__ void __launch_bounds__(CG_NT, PLAN ? CG_PLAN_BLOCKS : (MR <= 16 ? CG_RUN16_BLOCKS : (MR <= 32 ? 3 : (MR <= 48 ? CG_RUN48_BLOCKS : 2)))) cg_list_kernel(const CgKernelArgs a)
 {
     extern __shared__ __align__(128) uint8_t smem[];
@@ -952,6 +1012,8 @@ __global__ void __launch_bounds__(CG_NT, PLAN ? CG_PLAN_BLOCKS : (MR <= 16 ? CG_
             }
         }
         if (has_task && !cont && !defer) store_hit(a.out + (size_t)r * a.slots, hit, 0, n);
+        // (deferred reads are counted by the second plan launch, continuing ones by a later DP round)
+        if (STATS) list_stats_append<PLAN>(a, A, has_task && !cont && !defer, hit, ta, tc, td, s_slot + (size_t)lane * slot_bytes);
         if (PLAN) {
             const uint32_t dballot = __ballot_sync(0xffffffffu, defer);
             if (dballot) {
@@ -990,24 +1052,29 @@ __global__ void __launch_bounds__(CG_NT, PLAN ? CG_PLAN_BLOCKS : (MR <= 16 ? CG_
 }
 
 typedef void (*list_kernel_t)(const CgKernelArgs);
-static list_kernel_t pick_list(bool plan, int mr)
+template <bool STATS>
+static list_kernel_t pick_list_v(bool plan, int mr)
 {
-    if (plan) return cg_list_kernel<true, 16>;
-    if (mr <= 16) return cg_list_kernel<false, 16>;
-    if (mr <= 32) return cg_list_kernel<false, 32>;
-    if (mr <= 40) return cg_list_kernel<false, 40>;      // (the 33/34-base Illumina adapters: 8 rows fewer in registers)
-    return mr <= 48 ? cg_list_kernel<false, 48> : cg_list_kernel<false, 64>;
+    if (plan) return cg_list_kernel<true, 16, STATS>;
+    if (mr <= 16) return cg_list_kernel<false, 16, STATS>;
+    if (mr <= 32) return cg_list_kernel<false, 32, STATS>;
+    if (mr <= 40) return cg_list_kernel<false, 40, STATS>;      // (the 33/34-base Illumina adapters: 8 rows fewer in registers)
+    return mr <= 48 ? cg_list_kernel<false, 48, STATS> : cg_list_kernel<false, 64, STATS>;
 }
-cudaError_t cg_list_occupancy(bool plan, int mr, size_t smem, int *blocks_per_sm)
+static list_kernel_t pick_list(bool plan, int mr, bool stats)
 {
-    list_kernel_t k = pick_list(plan, mr);
+    return stats ? pick_list_v<true>(plan, mr) : pick_list_v<false>(plan, mr);
+}
+cudaError_t cg_list_occupancy(bool plan, int mr, bool stats, size_t smem, int *blocks_per_sm)
+{
+    list_kernel_t k = pick_list(plan, mr, stats);
     cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
     return cudaOccupancyMaxActiveBlocksPerMultiprocessor(blocks_per_sm, k, CG_NT, smem);
 }
 cudaError_t cg_launch_list(const CgKernelArgs &a, bool plan, int mr, int grid, size_t smem, cudaStream_t st)
 {
-    pick_list(plan, mr)<<<grid, CG_NT, smem, st>>>(a);
+    pick_list(plan, mr, a.stats != nullptr)<<<grid, CG_NT, smem, st>>>(a);
     return cudaGetLastError();
 }
 
@@ -1518,9 +1585,8 @@ cudaError_t cg_launch_max_len(const int64_t *d_offsets, long long n_reads, int *
 template <bool SMEM_HIST>
 __global__ void cg_stats_kernel(const uint8_t *seq, const int64_t *offsets, long long n_reads, int quality_trim, int times,
                                 int slots, const cg_match_rec *matches, const int32_t *qtrim,
-                                int n_adapters, int max_len, int kmax, unsigned long long *stats,
-                                const uint4 *task_list, int task_rec, const unsigned long long *task_count,
-                                int count_lengths, int upper)
+                                int n_adapters, int max_len, int kmax, unsigned long long *stats, int count_lengths,
+                                int upper)
 {
     // per-CTA histograms in shared memory (32-bit counts, flushed once): the read-length histogram always (every
     // read adds to it, mostly to the same few bins), the per-adapter part if it fits (SMEM_HIST); a global
@@ -1534,18 +1600,7 @@ __global__ void cg_stats_kernel(const uint8_t *seq, const int64_t *offsets, long
     unsigned long long n = 0;
     StatsScalars sc; sc.bp = sc.with_adapters = sc.qtrim_bp = sc.adapter_bp = 0;
     unsigned long long *hist = stats + CG_STATS_SCALARS;
-    // task_list: only the reads of a task list of the split pipeline (those its first stage did not count itself)
-    long long n_items = n_reads;
-    if (task_list) {
-        const unsigned long long t = *task_count;
-        n_items = t < (unsigned long long)n_reads ? (long long)t : n_reads;
-    }
-    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n_items; i += nthreads) {
-        long long r = i;
-        if (task_list) {
-            const uint4 t = task_list[(size_t)task_rec * i];
-            r = (long long)t.x;
-        }
+    for (long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x; r < n_reads; r += nthreads) {
         const long long o0 = offsets[r];
         const int len = (int)(offsets[r + 1] - o0);
         n += 1;
@@ -1581,8 +1636,7 @@ __global__ void cg_stats_kernel(const uint8_t *seq, const int64_t *offsets, long
 cudaError_t cg_launch_stats(const uint8_t *d_seq, const int64_t *d_offsets, long long n_reads, int quality_trim, int times,
                             int slots, const cg_match_rec *d_matches, const int32_t *d_qtrim,
                             int n_adapters, int max_len, int kmax, unsigned long long *d_stats,
-                            cudaStream_t st, const uint4 *d_task_list, int task_rec, const unsigned long long *d_task_count,
-                            int count_lengths, int upper)
+                            cudaStream_t st, int count_lengths, int upper)
 {
     const int block = 256;
     long long grid = (n_reads + block - 1) / block;
@@ -1595,12 +1649,61 @@ cudaError_t cg_launch_stats(const uint8_t *d_seq, const int64_t *d_offsets, long
     if (hist_bytes <= 48 * 1024 && n_reads / grid < (1LL << 31))
         cg_stats_kernel<true><<<(int)grid, block, hist_bytes, st>>>(d_seq, d_offsets, n_reads, quality_trim, times, slots,
                                                                      d_matches, d_qtrim, n_adapters, max_len, kmax, d_stats,
-                                                                     d_task_list, task_rec, d_task_count, count_lengths,
-                                                                     upper);
+                                                                     count_lengths, upper);
     else
         cg_stats_kernel<false><<<(int)grid, block, len_bytes, st>>>(d_seq, d_offsets, n_reads, quality_trim, times, slots,
                                                                      d_matches, d_qtrim, n_adapters, max_len, kmax, d_stats,
-                                                                     d_task_list, task_rec, d_task_count, count_lengths,
-                                                                     upper);
+                                                                     count_lengths, upper);
+    return cudaGetLastError();
+}
+
+// The statistics of the reads the plan and run kernels listed (list_stats_append), one adapter: per-CTA histograms in
+// shared memory as the first stage keeps them, removed lengths at every error count.  One launch per sub-batch.
+__global__ void __launch_bounds__(CG_NT) cg_stats_entries_kernel(const uint2 *ents, const unsigned long long *count,
+                                                                 int max_len, int kmax, unsigned long long *stats)
+{
+    extern __shared__ __align__(16) uint8_t s_ent_hist[];
+    const StatsSmem H = stats_smem_view(s_ent_hist, max_len, kmax + 1);
+    stats_smem_zero(H, max_len, kmax + 1);
+    __syncthreads();
+    const long long n = (long long)*count;
+    const int lane = threadIdx.x & 31;
+    // warp-uniform trip count: stats_warp_add wants all 32 lanes
+    for (long long w = (long long)blockIdx.x * CG_NT + (threadIdx.x & ~31); w < n; w += (long long)gridDim.x * CG_NT) {
+        const long long i = w + lane;
+        int bin = -1;
+        uint32_t p1 = 0, p2 = 0, p3 = 0;
+        if (i < n) {
+            const uint2 e = ents[i];
+            const int len = (int)(e.x >> 16);
+            p1 = e.x & 0xffffu;
+            p2 = 1u << 16;
+            if (e.y & 1u) {
+                const bool after = (e.y & 2u) != 0;
+                const int removed = (int)(e.y >> 16), E = (int)((e.y >> 5) & 2047u);
+                p2 |= (uint32_t)removed | (1u << 22);
+                atomicAdd(&H.hrem[((after ? max_len + 1 : 0) + (removed > max_len ? max_len : removed)) * (kmax + 1) +
+                                  (E > kmax ? kmax : E)], 1u);
+                if (after) p3 = 1u << (6 * ((e.y >> 2) & 7u));
+            }
+            bin = len > max_len ? max_len : len;
+        }
+        stats_warp_add(H, bin, p1, p2, p3);
+    }
+    __syncthreads();
+    stats_cta_flush(H, max_len, kmax, kmax + 1, stats);
+}
+
+size_t cg_stats_entries_smem_bytes(int max_len, int kmax) { return stats_smem_bytes(max_len, kmax + 1); }
+
+cudaError_t cg_launch_stats_entries(const uint2 *d_ents, const unsigned long long *d_count, long long cap, int max_len,
+                                    int kmax, unsigned long long *d_stats, cudaStream_t st)
+{
+    const size_t smem = stats_smem_bytes(max_len, kmax + 1);
+    if (smem > 48 * 1024) return cudaErrorInvalidValue;
+    long long grid = (cap + CG_NT - 1) / CG_NT;
+    grid = cg_grid_cap(grid, 2);
+    if (grid < 1) grid = 1;
+    cg_stats_entries_kernel<<<(int)grid, CG_NT, smem, st>>>(d_ents, d_count, max_len, kmax, d_stats);
     return cudaGetLastError();
 }

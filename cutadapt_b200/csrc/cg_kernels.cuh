@@ -52,7 +52,9 @@ size_t cg_pscan_smem_bytes(uint32_t blob_bytes, int mini_cap, bool has_qual, int
 cudaError_t cg_pscan_occupancy(bool has_qual, int w, bool stats, size_t smem, int *blocks_per_sm);
 cudaError_t cg_launch_pscan(const CgKernelArgs &a, bool has_qual, int w, int grid, size_t smem, cudaStream_t st);
 size_t cg_dp_smem_bytes(uint32_t blob_bytes, int slot_bytes);
-cudaError_t cg_list_occupancy(bool plan, int mr, size_t smem, int *blocks_per_sm);
+// stats: the variant that lists the statistics of the reads it finishes (a.stat_ents); cg_launch_list runs it when a.stats
+// is set
+cudaError_t cg_list_occupancy(bool plan, int mr, bool stats, size_t smem, int *blocks_per_sm);
 cudaError_t cg_launch_list(const CgKernelArgs &a, bool plan, int mr, int grid, size_t smem, cudaStream_t st);
 cudaError_t cg_launch_generic(const CgKernelArgs &a, int grid, int block, cudaStream_t st);
 cudaError_t cg_launch_locate_debug(const uint8_t *d_blob, const uint8_t *d_enc, const uint8_t *d_query, int n,
@@ -67,10 +69,14 @@ cudaError_t cg_launch_max_len(const int64_t *d_offsets, long long n_reads, int *
 cudaError_t cg_launch_stats(const uint8_t *d_seq, const int64_t *d_offsets, long long n_reads, int quality_trim, int times,
                             int slots, const cg_match_rec *d_matches, const int32_t *d_qtrim,
                             int n_adapters, int max_len, int kmax, unsigned long long *d_stats,
-                            cudaStream_t st, const uint4 *d_task_list = nullptr, int task_rec = 0,
-                            const unsigned long long *d_task_count = nullptr,    // task list: only its reads
+                            cudaStream_t st,
                             int count_lengths = 1,     // 0: leave the read-length histogram alone
                             int upper = 0);            // adjacent bases of the upper-cased read (--action=lowercase)
+// the statistics of the *d_count (at most cap) entries the plan and run kernels listed (one adapter); the launch needs
+// cg_stats_entries_smem_bytes(max_len, kmax) <= 48 KiB of shared memory
+size_t cg_stats_entries_smem_bytes(int max_len, int kmax);
+cudaError_t cg_launch_stats_entries(const uint2 *d_ents, const unsigned long long *d_count, long long cap, int max_len,
+                                    int kmax, unsigned long long *d_stats, cudaStream_t st);
 cudaError_t cg_launch_nextseq_trim(const uint8_t *d_seq, const uint8_t *d_qual, const int64_t *d_offsets,
                                    long long n_reads, int cutoff, int base, int32_t *d_out, cudaStream_t st);
 cudaError_t cg_launch_poly_a_trim(const uint8_t *d_seq, const int64_t *d_offsets, long long n_reads, int revcomp,

@@ -32,8 +32,90 @@ struct ScanSmem { size_t blob_off, enc_off, stats_off, warp_off, warp_stride, ba
 #define CG_TASK_PLANES 0x200u     // a 4 x uint4 task of cg_pscan_kernel: {read, window offset hi, lo, length},
                                   // {M0, flags, M1, M2}, {M3 .. M6}, {M7, window offset, 0, 0} with M = PlaneOut::M (+ CG_TASK_BYTES);
                                   // flags bits 12-15: plane words W, bit 20: PlaneOut::end_hit, bit 21: PlaneOut::no_end
-// stats_max_len >= 0: room for the per-CTA histograms of the fused statistics (read lengths, removed lengths at 0
-// errors for 5' and for 3' matches, adjacent bases): 3 (max_len + 1) + 8 counters, then 8 64-bit scalars
+// ------------------------------------------------------------------------------------------
+// Fused statistics (one plain adapter, one round, one slot: the passes launch_trim_single fuses them into): per-CTA
+// histograms in shared memory, flushed once at the end of the CTA.  Layout: read lengths (max_len + 1), removed
+// lengths for 5' then for 3' matches ((max_len + 1) x cols each: cols = 1 keeps 0 errors only, kmax + 1 every error
+// count), adjacent bases (8), then 8 64-bit scalars (reads, matches, bases, quality-trimmed, adapter bases).
+// ------------------------------------------------------------------------------------------
+struct StatsSmem { uint32_t *hlen, *hrem, *hadj; unsigned long long *scal; };
+__host__ __device__ inline size_t stats_smem_bytes(int max_len, int cols)
+{
+    return cg_align_up((size_t)((1 + 2 * cols) * (max_len + 1) + 8) * sizeof(uint32_t), 8) + 8 * sizeof(unsigned long long);
+}
+__device__ __forceinline__ StatsSmem stats_smem_view(uint8_t *base, int max_len, int cols)
+{
+    StatsSmem H;
+    H.hlen = (uint32_t *)base;
+    H.hrem = H.hlen + (max_len + 1);
+    H.hadj = H.hrem + 2 * cols * (max_len + 1);
+    H.scal = (unsigned long long *)(base + stats_smem_bytes(max_len, cols) - 8 * sizeof(unsigned long long));
+    return H;
+}
+// (before the CTA's first __syncthreads)
+__device__ __forceinline__ void stats_smem_zero(const StatsSmem &H, int max_len, int cols)
+{
+    for (int i = threadIdx.x; i < (1 + 2 * cols) * (max_len + 1) + 8; i += CG_NT) H.hlen[i] = 0;
+    if (threadIdx.x < 8) H.scal[threadIdx.x] = 0;
+}
+// One warp's reads.  fin: this lane's final-length bin (-1 = nothing to count); its contributions to the scalars,
+// packed for three warp sums: p1 = bases | quality-trimmed bases << 16, p2 = adapter bases | read << 16 | match << 22,
+// p3 = one 6-bit count per adjacent-base class (the fields hold the sums of 32 reads of at most 256 bases).  The
+// removed-length bins are the caller's.  All 32 lanes call it.
+__device__ __forceinline__ void stats_warp_add(const StatsSmem &H, int fin, uint32_t p1, uint32_t p2, uint32_t p3)
+{
+    const int lane = threadIdx.x & 31;
+    // most reads of a tile end in the same length bin: one shared-memory atomic for the bin of the first
+    // counted lane and its peers, one each for the others
+    const uint32_t counted = __ballot_sync(0xffffffffu, fin >= 0);
+    if (!counted) return;
+    const int leader = __ffs(counted) - 1;
+    const int common = __shfl_sync(0xffffffffu, fin, leader);
+    const uint32_t same = __ballot_sync(0xffffffffu, fin == common);
+    if (lane == leader) atomicAdd(&H.hlen[common], (uint32_t)__popc(same));
+    else if (fin >= 0 && fin != common) atomicAdd(&H.hlen[fin], 1u);
+    const uint32_t s1 = __reduce_add_sync(0xffffffffu, p1);
+    const uint32_t s2 = __reduce_add_sync(0xffffffffu, p2);
+    const uint32_t s3 = __reduce_add_sync(0xffffffffu, p3);
+    // lane L adds scalar L of the warp to the CTA's counters (no register held across the tile loop):
+    // reads, matches, bases, quality-trimmed, adapter bases, adjacent x 5
+    uint32_t mine_add = 0;
+    switch (lane) {
+    case 0: mine_add = (s2 >> 16) & 63u; break;
+    case 1: mine_add = s2 >> 22; break;
+    case 2: mine_add = s1 & 0xffffu; break;
+    case 3: mine_add = s1 >> 16; break;
+    case 4: mine_add = s2 & 0xffffu; break;
+    default: if (lane < 10) mine_add = (s3 >> (6 * (lane - 5))) & 63u; break;
+    }
+    if (mine_add) {
+        if (lane < 5) atomicAdd(&H.scal[lane], (unsigned long long)mine_add);
+        else atomicAdd(&H.hadj[lane - 5], mine_add);
+    }
+}
+// The CTA's counters into the vector (one adapter: lengths, then its 5' block and its 3' block); after a __syncthreads.
+__device__ __forceinline__ void stats_cta_flush(const StatsSmem &H, int max_len, int kmax, int cols, unsigned long long *stats)
+{
+    // reads, matches, bases, quality-trimmed, adapter bases -> stats[0, 2, 1, 3, 4]
+    if (threadIdx.x < 5 && H.scal[threadIdx.x])
+        atomicAdd(&stats[threadIdx.x == 1 ? 2 : (threadIdx.x == 2 ? 1 : threadIdx.x)], H.scal[threadIdx.x]);
+    unsigned long long *hist = stats + CG_STATS_SCALARS;
+    const long long end_size = cg_stats_end_size(max_len, kmax);
+    for (int i = threadIdx.x; i <= max_len; i += CG_NT) {
+        const uint32_t v = H.hlen[i];
+        if (v) atomicAdd(&hist[i], (unsigned long long)v);
+    }
+    for (int i = threadIdx.x; i < 2 * cols * (max_len + 1); i += CG_NT) {
+        const uint32_t w = H.hrem[i];
+        const int kind = i / (cols * (max_len + 1)), j = i - kind * cols * (max_len + 1);
+        if (w) atomicAdd(&hist[(max_len + 1) + kind * end_size + CG_STATS_ADJ + (long long)(j / cols) * (kmax + 1) + j % cols],
+                         (unsigned long long)w);
+    }
+    if (threadIdx.x < 8 && H.hadj[threadIdx.x])
+        atomicAdd(&hist[(max_len + 1) + end_size + threadIdx.x], (unsigned long long)H.hadj[threadIdx.x]);
+}
+
+// stats_max_len >= 0: room for the per-CTA histograms of the fused statistics, removed lengths at 0 errors only
 __host__ __device__ inline ScanSmem pscan_smem_layout(uint32_t blob_bytes, int mini_cap, bool has_qual, int stats_max_len = -1)
 {
     ScanSmem L;
@@ -41,7 +123,7 @@ __host__ __device__ inline ScanSmem pscan_smem_layout(uint32_t blob_bytes, int m
     L.blob_off = o; o += cg_align_up(blob_bytes, 16);
     L.enc_off = o; o += 768;
     L.stats_off = o;
-    if (stats_max_len >= 0) o += cg_align_up((size_t)(3 * (stats_max_len + 1) + 8) * sizeof(uint32_t), 8) + 8 * sizeof(unsigned long long);
+    if (stats_max_len >= 0) o += stats_smem_bytes(stats_max_len, 1);
     o = cg_align_up(o, 128);
     L.warp_off = o;
     size_t w = 0;
@@ -144,19 +226,15 @@ __device__ __forceinline__ void cg_pscan_body(const CgKernelArgs &a)
     uint64_t *bars = (uint64_t *)(wbase + L.bar_rel);
     uint8_t *s_seq = wbase + L.seq_rel;
     uint8_t *s_qual = wbase + L.qual_rel;
-    // fused statistics: per-CTA histograms, flushed at the end (layout: cg_types.h, stats_read_core).  Everything is
-    // re-derived from the kernel arguments where it is used: nothing of it may occupy a register across the plane code.
+    // fused statistics: per-CTA histograms, flushed at the end (stats_smem_view; the reads settled here have 0 errors).
+    // Everything is re-derived from the kernel arguments where it is used: nothing of it may occupy a register across
+    // the plane code.
 #define CG_PSCAN_STATS_VIEW                                                                                              \
     const int st_len = a.stats_max_len;                                                                                  \
-    uint32_t *s_hlen = (uint32_t *)(smem + pscan_smem_layout(a.blob_bytes, a.mini_cap, HAS_QUAL, st_len).stats_off);     \
-    uint32_t *s_hrem = s_hlen + (st_len + 1);   /* removed lengths at 0 errors: 5' matches, then 3' matches */           \
-    uint32_t *s_hadj = s_hrem + 2 * (st_len + 1);                                                                        \
-    unsigned long long *s_scal = (unsigned long long *)((uint8_t *)s_hlen + cg_align_up((size_t)(3 * (st_len + 1) + 8) * sizeof(uint32_t), 8));
+    const StatsSmem H = stats_smem_view(smem + pscan_smem_layout(a.blob_bytes, a.mini_cap, HAS_QUAL, st_len).stats_off, st_len, 1);
     if (STATS && a.stats) {
         CG_PSCAN_STATS_VIEW
-        (void)s_hrem; (void)s_hadj;
-        for (int i = threadIdx.x; i < 3 * (st_len + 1) + 8; i += CG_NT) s_hlen[i] = 0;
-        if (threadIdx.x < 8) s_scal[threadIdx.x] = 0;     // reads, bases, with adapters, quality-trimmed, adapter bases
+        stats_smem_zero(H, st_len, 1);
     }
     for (uint32_t i = tid; i < a.blob_bytes / 16; i += CG_NT) ((uint4 *)s_blob)[i] = ((const uint4 *)a.blob)[i];
     for (uint32_t i = tid; i < 768 / 16; i += CG_NT) ((uint4 *)s_enc)[i] = ((const uint4 *)a.enc)[i];
@@ -256,11 +334,8 @@ __device__ __forceinline__ void cg_pscan_body(const CgKernelArgs &a)
                 else if (cls == CG_PLANE_OVERLAP) hit_end_overlap(A, nn, s0, hit);
                 store_hit(a.out + (size_t)r * a.slots, hit, 0, nn);
                 if (STATS && a.stats) {
-                    // what stats_read_core adds for this read (one round, one slot), packed for three warp sums:
-                    // p1 = bases | quality-trimmed bases << 16, p2 = adapter bases | read << 16 | match << 22,
-                    // p3 = one 6-bit count per adjacent-base class
+                    // what stats_read_core adds for this read (one round, one slot), packed as stats_warp_add takes it
                     CG_PSCAN_STATS_VIEW
-                    (void)s_hlen; (void)s_scal; (void)s_hadj;
                     st_p1 = (uint32_t)n | ((a.quality_trim && a.qtrim) ? (uint32_t)(n - nn) << 16 : 0u);
                     st_p2 = 1u << 16;
                     int fin = nn;
@@ -271,7 +346,7 @@ __device__ __forceinline__ void cg_pscan_body(const CgKernelArgs &a)
                         int removed = after ? nn - hit.rstart : hit.rstop;
                         removed = removed < 0 ? 0 : removed;
                         st_p2 |= (uint32_t)removed | (1u << 22);
-                        atomicAdd(&s_hrem[(after ? st_len + 1 : 0) + (removed > st_len ? st_len : removed)], 1u);
+                        atomicAdd(&H.hrem[(after ? st_len + 1 : 0) + (removed > st_len ? st_len : removed)], 1u);
                         if (after) {
                             int k = 4;
                             if (hit.rstart > 0) {
@@ -290,35 +365,7 @@ __device__ __forceinline__ void cg_pscan_body(const CgKernelArgs &a)
         }
         if (STATS && a.stats) {
             CG_PSCAN_STATS_VIEW
-            (void)s_hrem;
-            // most reads of a tile end in the same length bin: one shared-memory atomic for the bin of the first
-            // counted lane and its peers, one each for the others
-            const uint32_t counted = __ballot_sync(0xffffffffu, st_fin >= 0);
-            if (counted) {
-                const int leader = __ffs(counted) - 1;
-                const int common = __shfl_sync(0xffffffffu, st_fin, leader);
-                const uint32_t same = __ballot_sync(0xffffffffu, st_fin == common);
-                if (lane == leader) atomicAdd(&s_hlen[common], (uint32_t)__popc(same));
-                else if (st_fin >= 0 && st_fin != common) atomicAdd(&s_hlen[st_fin], 1u);
-                const uint32_t s1 = __reduce_add_sync(0xffffffffu, st_p1);
-                const uint32_t s2 = __reduce_add_sync(0xffffffffu, st_p2);
-                const uint32_t s3 = __reduce_add_sync(0xffffffffu, st_p3);
-                // lane L adds scalar L of the warp to the CTA's counters (no register held across the tile loop):
-                // reads, matches, bases, quality-trimmed, adapter bases, adjacent x 5
-                uint32_t mine_add = 0;
-                switch (lane) {
-                case 0: mine_add = (s2 >> 16) & 63u; break;
-                case 1: mine_add = s2 >> 22; break;
-                case 2: mine_add = s1 & 0xffffu; break;
-                case 3: mine_add = s1 >> 16; break;
-                case 4: mine_add = s2 & 0xffffu; break;
-                default: if (lane < 10) mine_add = (s3 >> (6 * (lane - 5))) & 63u; break;
-                }
-                if (mine_add) {
-                    if (lane < 5) atomicAdd(&s_scal[lane], (unsigned long long)mine_add);
-                    else atomicAdd(&s_hadj[lane - 5], mine_add);
-                }
-            }
+            stats_warp_add(H, st_fin, st_p1, st_p2, st_p3);
         }
         const bool slow = mine && cls == CG_PLANE_SLOW;
         // two lists: reads with locator hits (and everything the planes could not look at) from the front, reads
@@ -367,23 +414,7 @@ __device__ __forceinline__ void cg_pscan_body(const CgKernelArgs &a)
     if (STATS && a.stats) {
         CG_PSCAN_STATS_VIEW
         __syncthreads();
-        // reads, matches, bases, quality-trimmed, adapter bases -> stats[0, 2, 1, 3, 4]
-        if (threadIdx.x < 5 && s_scal[threadIdx.x])
-            atomicAdd(&a.stats[threadIdx.x == 1 ? 2 : (threadIdx.x == 2 ? 1 : threadIdx.x)], s_scal[threadIdx.x]);
-        // one adapter: lengths, then its 5' block and its 3' block (adjacent bases, removed length x errors)
-        unsigned long long *hist = a.stats + CG_STATS_SCALARS;
-        const long long end_size = cg_stats_end_size(st_len, a.stats_kmax);
-        for (int i = threadIdx.x; i <= st_len; i += CG_NT) {
-            const uint32_t v = s_hlen[i];
-            if (v) atomicAdd(&hist[i], (unsigned long long)v);
-            for (int kind = 0; kind < 2; ++kind) {
-                const uint32_t w = s_hrem[kind * (st_len + 1) + i];
-                if (w) atomicAdd(&hist[(st_len + 1) + kind * end_size + CG_STATS_ADJ + (long long)i * (a.stats_kmax + 1)],
-                                 (unsigned long long)w);
-            }
-        }
-        if (threadIdx.x < 8 && s_hadj[threadIdx.x])
-            atomicAdd(&hist[(st_len + 1) + end_size + threadIdx.x], (unsigned long long)s_hadj[threadIdx.x]);
+        stats_cta_flush(H, st_len, a.stats_kmax, 1, a.stats);
     }
 }
 
