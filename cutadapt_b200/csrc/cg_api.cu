@@ -12,7 +12,9 @@
 #include <algorithm>
 #include <chrono>
 #include <map>
+#include <memory>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/cutadapt_b200.h"
@@ -52,38 +54,48 @@ extern "C" int cg_version(void) { return CG_ABI_VERSION; }
 extern "C" const char *cg_last_error(void) { return g_err.c_str(); }
 
 // ------------------------------------------------------------------------------------------
-template <class T> struct DevBuf {
+// A growing device (DevBuf) or pinned host (PinBuf) buffer.  It owns its memory: freed when the buffer is destroyed or
+// assigned to, handed over by moves, never copied.
+template <class T, bool Pinned> class GrowBuf {
+  public:
     T *p = nullptr;
     size_t cap = 0;
+    GrowBuf() = default;
+    GrowBuf(const GrowBuf &) = delete;
+    GrowBuf &operator=(const GrowBuf &) = delete;
+    GrowBuf(GrowBuf &&o) noexcept : p(o.p), cap(o.cap) { o.p = nullptr; o.cap = 0; }
+    GrowBuf &operator=(GrowBuf &&o) noexcept
+    {
+        if (this != &o) {
+            release();
+            p = o.p; cap = o.cap;
+            o.p = nullptr; o.cap = 0;
+        }
+        return *this;
+    }
+    ~GrowBuf() { release(); }
     int ensure(size_t n)
     {
         if (n <= cap) return CG_OK;
-        if (p) cudaFree(p);
-        p = nullptr; cap = 0;
+        release();
         size_t want = n + n / 4 + 64;
-        cudaError_t e = cudaMalloc((void **)&p, want * sizeof(T));
-        if (e != cudaSuccess) return cuda_fail(e, "cudaMalloc");
+        cudaError_t e = Pinned ? cudaMallocHost((void **)&p, want * sizeof(T)) : cudaMalloc((void **)&p, want * sizeof(T));
+        if (e != cudaSuccess) return cuda_fail(e, Pinned ? "cudaMallocHost" : "cudaMalloc");
         cap = want;
         return CG_OK;
     }
-    void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
-};
-template <class T> struct PinBuf {
-    T *p = nullptr;
-    size_t cap = 0;
-    int ensure(size_t n)
+
+  private:
+    void release()
     {
-        if (n <= cap) return CG_OK;
-        if (p) cudaFreeHost(p);
+        if (p) Pinned ? cudaFreeHost(p) : cudaFree(p);
         p = nullptr; cap = 0;
-        size_t want = n + n / 4 + 64;
-        cudaError_t e = cudaMallocHost((void **)&p, want * sizeof(T));
-        if (e != cudaSuccess) return cuda_fail(e, "cudaMallocHost");
-        cap = want;
-        return CG_OK;
     }
-    void release() { if (p) cudaFreeHost(p); p = nullptr; cap = 0; }
 };
+template <class T> using DevBuf = GrowBuf<T, false>;
+template <class T> using PinBuf = GrowBuf<T, true>;
+static_assert(!std::is_copy_constructible<DevBuf<uint8_t>>::value && !std::is_copy_constructible<PinBuf<uint8_t>>::value,
+              "buffers own their memory: move them");
 
 #define CG_N_LANES 3
 struct Lane {
@@ -138,8 +150,8 @@ struct FastqSlot {
     // interleaved input (cg_fastq_submit_interleaved): 0 = a chunk of its own, 1 / 2 = mate 1 / 2 of the chunk uploaded to
     // mate 1's slot, split when the pair is collected; ilv_peer = the other mate's slot, ilv_format = input format
     int ilv = 0, ilv_peer = -1, ilv_format = 0;
-    unsigned long long *d_counters = nullptr;   // [0] newline total, [1..] CG_FQ_COUNTERS
-    int *d_err = nullptr;                       // [0] code, [1] record
+    DevBuf<unsigned long long> d_counters;      // [0] newline total, [1..] CG_FQ_COUNTERS
+    DevBuf<int> d_err;                          // [0] code, [1] record
     PinBuf<uint8_t> h_in, h_out;
     PinBuf<unsigned long long> h_counters;
 };
@@ -171,16 +183,7 @@ struct GzinStream {
     DevBuf<uint16_t> d_sym;
     DevBuf<int32_t> d_redo;
     DevBuf<uint32_t> d_part;
-    void release()
-    {
-        d_gz.release(); d_plain.release(); h_gz.release(); d_counts.release(); d_cand.release(); d_members.release();
-        d_flag.release(); d_offs.release(); d_res.release(); d_moff.release(); d_scan.release(); d_small.release();
-        d_tiles.release(); d_nl.release();
-        d_win.release(); d_pwin.release(); d_wins.release(); d_ch.release(); d_coff.release(); d_room.release();
-        d_sym.release(); d_redo.release(); d_part.release();
-        if (done) cudaEventDestroy(done);
-        done = nullptr;
-    }
+    ~GzinStream() { if (done) cudaEventDestroy(done); }   // not copyable, as its buffers are not
 };
 
 // A statistics accumulator of the FASTQ path (cg_fastq_stats_create): the vector of cg_fastq_stats_read at
@@ -281,7 +284,8 @@ extern "C" int cg_ctx_create(int device, void *stream, cg_ctx **out)
                                   "); cutadapt_b200 has no CPU fallback");
     if (device < 0 || device >= count) return fail(CG_EINVAL, "cg_ctx_create: device ordinal out of range");
     CU(cudaSetDevice(device));
-    cg_ctx *c = new cg_ctx();
+    // until it is complete, a failed step destroys what has been built
+    std::unique_ptr<cg_ctx, decltype(&cg_ctx_destroy)> c(new cg_ctx(), cg_ctx_destroy);
     c->device = device;
     cudaDeviceProp prop;
     CU(cudaGetDeviceProperties(&prop, device));
@@ -305,7 +309,7 @@ extern "C" int cg_ctx_create(int device, void *stream, cg_ctx **out)
         CU(cudaMalloc((void **)&c->d_phred, sizeof phred));
         CU(cudaMemcpy(c->d_phred, phred, sizeof phred, cudaMemcpyHostToDevice));
     }
-    *out = c;
+    *out = c.release();
     return CG_OK;
 }
 
@@ -331,38 +335,17 @@ extern "C" int cg_ctx_destroy(cg_ctx *c)
     for (auto ev : c->event_pool) cudaEventDestroy(ev);
     delete c->pool;
     c->pool = nullptr;
-    for (int i = 0; i < CG_N_LANES; ++i) {
-        Lane &l = c->lanes[i];
-        l.d_pack.release(); l.d_exc.release(); l.h_pack.release(); l.h_exc.release();
-        l.d_seq.release(); l.d_qual.release(); l.d_offs.release(); l.d_out.release(); l.d_qtrim.release();
-        l.h_seq.release(); l.h_qual.release(); l.h_offs.release(); l.h_out.release(); l.h_qtrim.release();
+    for (Lane &l : c->lanes)
         if (l.stream) cudaStreamDestroy(l.stream);
-    }
-    c->scratch_p.release(); c->scratch_w.release(); c->tasks.release(); c->tasks2.release(); c->tasks3.release(); c->stat_ents.release();
-    c->pass_tmp.release(); c->view_base.release(); c->view_back.release();
-    for (FastqSlot &f : c->fq) {
-        f.d_in.release(); f.d_out.release(); f.d_seq.release(); f.d_qual.release(); f.d_tiles.release(); f.d_nl.release();
-        f.d_rec.release(); f.d_len.release(); f.d_mask.release(); f.d_adest.release(); f.d_dmbytes.release();
-        f.d_dmbase.release(); f.d_keep.release(); f.d_interval.release(); f.d_outlen.release(); f.d_qtrim.release();
-        f.d_offs.release(); f.d_outoff.release(); f.d_scan.release(); f.d_matches.release(); f.d_matches_rc.release();
-        f.d_isrc.release(); f.d_dest.release(); f.d_pairkey.release(); f.d_destkeep.release(); f.d_origin.release();
-        f.d_names.release(); f.d_infoout.release(); f.d_nameoff.release(); f.d_inforow.release(); f.d_infooff.release();
-        f.d_norm.release(); f.d_faline.release(); f.d_faoff.release();
-        f.d_fqstats.release(); f.d_polya.release(); f.h_fqstats.release();
-        f.d_gzpieces.release(); f.d_gzslots.release(); f.d_gzout.release(); f.d_gzsizes.release(); f.d_gzoff.release();
-        f.h_in.release(); f.h_out.release(); f.h_counters.release();
-        if (f.d_counters) cudaFree(f.d_counters);
-        if (f.d_err) cudaFree(f.d_err);
+    for (FastqSlot &f : c->fq)
         if (f.stream) cudaStreamDestroy(f.stream);
-    }
-    for (auto &kv : c->gzin) kv.second.release();
     if (c->scratch_ev) cudaEventDestroy(c->scratch_ev);
     if (c->d_task_count) cudaFree(c->d_task_count);
     if (c->d_err) cudaFree(c->d_err);
     if (c->d_enc) cudaFree(c->d_enc);
     if (c->d_phred) cudaFree(c->d_phred);
     if (c->own_stream && c->stream) cudaStreamDestroy(c->stream);
-    delete c;
+    delete c;                                   // the buffers and the gzip input streams free themselves
     return CG_OK;
 }
 
@@ -944,10 +927,6 @@ extern "C" int cg_locate_debug(cg_ctx *c, const cg_adapter_desc *adapter, const 
     DevBuf<uint8_t> d_blob, d_query;
     DevBuf<int> d_scratch;
     DevBuf<int32_t> d_mat, d_res;
-    struct Free {
-        DevBuf<uint8_t> &a, &b; DevBuf<int> &s; DevBuf<int32_t> &m, &r;
-        ~Free() { a.release(); b.release(); s.release(); m.release(); r.release(); }
-    } free_all{d_blob, d_query, d_scratch, d_mat, d_res};
     if ((rc = d_blob.ensure(set.blob.size())) != CG_OK || (rc = d_query.ensure((size_t)n + 16)) != CG_OK ||
         (rc = d_scratch.ensure(3 * ((size_t)m + 2))) != CG_OK || (rc = d_mat.ensure(2 * cells)) != CG_OK ||
         (rc = d_res.ensure(8)) != CG_OK)
@@ -1694,17 +1673,16 @@ static int fastq_slot_init(cg_ctx *c, FastqSlot &f)
 {
     f.ilv = 0;
     if (!f.stream) CU(cudaStreamCreateWithFlags(&f.stream, cudaStreamNonBlocking));
-    if (!f.d_counters) CU(cudaMalloc((void **)&f.d_counters, (1 + CG_FQ_COUNTERS) * sizeof(unsigned long long)));
-    if (!f.d_err) CU(cudaMalloc((void **)&f.d_err, 2 * sizeof(int)));
+    int rc;
+    if ((rc = f.d_counters.ensure(1 + CG_FQ_COUNTERS)) != CG_OK || (rc = f.d_err.ensure(2)) != CG_OK) return rc;
     if (!c->pool) {
         c->pool = new CgHostPool(cg_host_threads_default());
         c->exc_scratch.resize((size_t)c->pool->size());
     }
-    int rc;
     if ((rc = f.h_counters.ensure(1 + CG_FQ_COUNTERS)) != CG_OK) return rc;
-    CU(cudaMemsetAsync(f.d_counters, 0, (1 + CG_FQ_COUNTERS) * sizeof(unsigned long long), f.stream));
+    CU(cudaMemsetAsync(f.d_counters.p, 0, (1 + CG_FQ_COUNTERS) * sizeof(unsigned long long), f.stream));
     const int err_init[2] = {0, 0x7FFFFFFF};
-    CU(cudaMemcpyAsync(f.d_err, err_init, sizeof err_init, cudaMemcpyHostToDevice, f.stream));
+    CU(cudaMemcpyAsync(f.d_err.p, err_init, sizeof err_init, cudaMemcpyHostToDevice, f.stream));
     return CG_OK;
 }
 
@@ -1715,10 +1693,10 @@ static int fastq_slot_count(cg_ctx *c, FastqSlot &f, int64_t n_bytes)
     if ((rc = f.d_tiles.ensure((size_t)cg_fastq_tiles(n_bytes) + 1)) != CG_OK) return rc;
     f.n_bytes = n_bytes;
     if (n_bytes) {
-        CU(cg_launch_fastq_index(f.d_in.p, n_bytes, f.d_tiles.p, f.d_counters, nullptr, 0, f.stream));
+        CU(cg_launch_fastq_index(f.d_in.p, n_bytes, f.d_tiles.p, f.d_counters.p, nullptr, 0, f.stream));
         c->launches += 2;
     }
-    CU(cudaMemcpyAsync(f.h_counters.p, f.d_counters, sizeof(unsigned long long), cudaMemcpyDeviceToHost, f.stream));
+    CU(cudaMemcpyAsync(f.h_counters.p, f.d_counters.p, sizeof(unsigned long long), cudaMemcpyDeviceToHost, f.stream));
     return CG_OK;
 }
 
@@ -1741,44 +1719,72 @@ static int fastq_slot_upload(cg_ctx *c, FastqSlot &f, const uint8_t *fastq, int6
     return fastq_slot_count(c, f, n_bytes);
 }
 
+// The argument checks of a submit: `ok` holds the caller's own, then up to two byte buffers and the format; `what` names
+// a buffer in the size message.
+static int submit_check(const char *who, bool ok, int32_t format, const char *what, const uint8_t *p1, int64_t n1,
+                        const uint8_t *p2 = nullptr, int64_t n2 = 0)
+{
+    if (!ok || n1 < 0 || n2 < 0 || (n1 && !p1) || (n2 && !p2) || format < CG_FORMAT_FASTQ ||
+        format > CG_FORMAT_FASTQ_TO_FASTA)
+        return fail(CG_EINVAL, std::string(who) + ": bad argument");
+    if (n1 >= (1LL << 31) || n2 >= (1LL << 31))
+        return fail(CG_EINVAL, std::string(who) + ": a " + what + " must be smaller than 2 GiB");
+    return CG_OK;
+}
+
+// The n (1 or 2) slots a submission gets, from fq_next on; *s1 the first.  `busy`: the message when one is in flight.
+static int fq_find(cg_ctx *c, int n, const char *busy, int *s1)
+{
+    *s1 = c->fq_next;
+    for (int i = 0; i < n; ++i)
+        if (c->fq[(*s1 + i) % CG_FQ_SLOTS].busy) return fail(CG_EINVAL, busy);
+    return CG_OK;
+}
+
+// Hand out the slots fq_find found: one (slot2 == nullptr) or two, busy until collected.  ilv_format >= 0: the two are
+// the mates of one interleaved chunk in that input format (FastqSlot::ilv).
+static void fq_take(cg_ctx *c, int s1, int32_t *slot1, int32_t *slot2 = nullptr, int ilv_format = -1)
+{
+    const int s2 = (s1 + 1) % CG_FQ_SLOTS;
+    c->fq[s1].busy = true;
+    *slot1 = s1;
+    c->fq_next = s2;
+    if (!slot2) return;
+    c->fq[s2].busy = true;
+    *slot2 = s2;
+    c->fq_next = (s2 + 1) % CG_FQ_SLOTS;
+    if (ilv_format < 0) return;
+    FastqSlot &f1 = c->fq[s1], &f2 = c->fq[s2];
+    f1.ilv = 1; f1.ilv_peer = s2;
+    f2.ilv = 2; f2.ilv_peer = s1;
+    f1.ilv_format = f2.ilv_format = ilv_format == CG_FORMAT_FASTA ? CG_FORMAT_FASTA : CG_FORMAT_FASTQ;
+}
+
 extern "C" int cg_fastq_submit(cg_ctx *c, const uint8_t *fastq, int64_t n_bytes, int32_t *slot_out)
 {
-    if (!c || !slot_out || n_bytes < 0 || (n_bytes && !fastq)) return fail(CG_EINVAL, "cg_fastq_submit: bad argument");
-    if (n_bytes >= (1LL << 31)) return fail(CG_EINVAL, "cg_fastq_submit: a chunk must be smaller than 2 GiB");
-    CU(cudaSetDevice(c->device));
-    const int si = c->fq_next;
-    FastqSlot &f = c->fq[si];
-    if (f.busy) return fail(CG_EINVAL, "cg_fastq_submit: all slots are in flight, collect one first");
-    c->fq_next = (si + 1) % CG_FQ_SLOTS;
-    const int rc = fastq_slot_upload(c, f, fastq, n_bytes);
+    int rc = submit_check("cg_fastq_submit", c && slot_out, CG_FORMAT_FASTQ, "chunk", fastq, n_bytes);
     if (rc != CG_OK) return rc;
-    f.busy = true;
-    *slot_out = si;
+    CU(cudaSetDevice(c->device));
+    int si;
+    if ((rc = fq_find(c, 1, "cg_fastq_submit: all slots are in flight, collect one first", &si)) != CG_OK) return rc;
+    if ((rc = fastq_slot_upload(c, c->fq[si], fastq, n_bytes)) != CG_OK) return rc;
+    fq_take(c, si, slot_out);
     return CG_OK;
 }
 
 extern "C" int cg_fastq_submit_interleaved(cg_ctx *c, const uint8_t *chunk, int64_t n_bytes, int32_t format, int32_t *slot1,
                                            int32_t *slot2)
 {
-    if (!c || !slot1 || !slot2 || n_bytes < 0 || (n_bytes && !chunk) || format < CG_FORMAT_FASTQ ||
-        format > CG_FORMAT_FASTQ_TO_FASTA)
-        return fail(CG_EINVAL, "cg_fastq_submit_interleaved: bad argument");
-    if (n_bytes >= (1LL << 31)) return fail(CG_EINVAL, "cg_fastq_submit_interleaved: a chunk must be smaller than 2 GiB");
+    int rc = submit_check("cg_fastq_submit_interleaved", c && slot1 && slot2, format, "chunk", chunk, n_bytes);
+    if (rc != CG_OK) return rc;
     CU(cudaSetDevice(c->device));
-    const int s1 = c->fq_next, s2 = (s1 + 1) % CG_FQ_SLOTS;
-    FastqSlot &f1 = c->fq[s1], &f2 = c->fq[s2];
-    if (f1.busy || f2.busy)
-        return fail(CG_EINVAL, "cg_fastq_submit_interleaved: two free slots are needed, collect one first");
-    c->fq_next = (s2 + 1) % CG_FQ_SLOTS;
-    int rc;
-    if ((rc = fastq_slot_upload(c, f1, chunk, n_bytes)) != CG_OK) return rc;
-    if ((rc = fastq_slot_upload(c, f2, nullptr, 0)) != CG_OK) return rc;     // its chunk comes from the split
-    f1.ilv = 1; f1.ilv_peer = s2;
-    f2.ilv = 2; f2.ilv_peer = s1;
-    f1.ilv_format = f2.ilv_format = format == CG_FORMAT_FASTA ? CG_FORMAT_FASTA : CG_FORMAT_FASTQ;
-    f1.busy = f2.busy = true;
-    *slot1 = s1;
-    *slot2 = s2;
+    int s1;
+    if ((rc = fq_find(c, 2, "cg_fastq_submit_interleaved: two free slots are needed, collect one first", &s1)) != CG_OK)
+        return rc;
+    if ((rc = fastq_slot_upload(c, c->fq[s1], chunk, n_bytes)) != CG_OK) return rc;
+    // its chunk comes from the split
+    if ((rc = fastq_slot_upload(c, c->fq[(s1 + 1) % CG_FQ_SLOTS], nullptr, 0)) != CG_OK) return rc;
+    fq_take(c, s1, slot1, slot2, format);
     return CG_OK;
 }
 
@@ -1807,7 +1813,6 @@ extern "C" int cg_gzin_create_ex(cg_ctx *c, int32_t flags, int32_t *handle)
         // CUTADAPT_B200_GZIN_STRIDE (cutadapt_b200.h): the stride sweep of tools/measure_fastq.py --gzip-input
         if (const char *e = getenv("CUTADAPT_B200_GZIN_STRIDE")) g.stride = std::max(32768LL, atoll(e));
         if ((rc = g.d_win.ensure(GU_WIN)) != CG_OK || (rc = g.d_pwin.ensure(GU_WIN)) != CG_OK) {
-            g.release();
             c->gzin.erase(h);
             return rc;
         }
@@ -1826,7 +1831,6 @@ extern "C" int cg_gzin_destroy(cg_ctx *c, int32_t handle)
     if (it == c->gzin.end()) return fail(CG_EINVAL, "cg_gzin_destroy: unknown handle");
     CU(cudaSetDevice(c->device));
     if (it->second.done) CU(cudaEventSynchronize(it->second.done));
-    it->second.release();
     c->gzin.erase(it);
     return CG_OK;
 }
@@ -1840,8 +1844,7 @@ static int gzin_plain_room(GzinStream &g, long long keep, long long total, cudaS
     if ((rc = nb.ensure((size_t)total + 64)) != CG_OK) return rc;
     if (keep) CU(cudaMemcpyAsync(nb.p, g.d_plain.p, (size_t)keep, cudaMemcpyDeviceToDevice, st));
     CU(cudaStreamSynchronize(st));
-    g.d_plain.release();
-    g.d_plain = nb;
+    g.d_plain = std::move(nb);
     return CG_OK;
 }
 
@@ -1954,8 +1957,7 @@ static int gzin_blocks(cg_ctx *c, GzinStream &g, long long n, long long bound, l
             if ((rc = nb.ensure((size_t)arena)) != CG_OK) return rc;
             CU(cudaMemcpyAsync(nb.p, g.d_sym.p, (size_t)old_arena * sizeof(uint16_t), cudaMemcpyDeviceToDevice, st));
             CU(cudaStreamSynchronize(st));
-            g.d_sym.release();
-            g.d_sym = nb;
+            g.d_sym = std::move(nb);
             CU(cudaMemcpyAsync(g.d_coff.p, off.data(), K * sizeof(long long), cudaMemcpyHostToDevice, st));
             CU(cudaMemcpyAsync(g.d_room.p, room.data(), K * sizeof(long long), cudaMemcpyHostToDevice, st));
         }
@@ -2242,19 +2244,16 @@ static GzinStream *gzin_lookup(cg_ctx *c, int32_t handle)
 extern "C" int cg_fastq_submit_gzip(cg_ctx *c, int32_t handle, const uint8_t *gz, int64_t n_bytes, int32_t format,
                                     int32_t final, int32_t *slot, cg_gzin_result *res)
 {
-    if (!c || !slot || !res || n_bytes < 0 || (n_bytes && !gz) || format < CG_FORMAT_FASTQ ||
-        format > CG_FORMAT_FASTQ_TO_FASTA)
-        return fail(CG_EINVAL, "cg_fastq_submit_gzip: bad argument");
-    if (n_bytes >= (1LL << 31)) return fail(CG_EINVAL, "cg_fastq_submit_gzip: a submission must be smaller than 2 GiB");
+    int rc = submit_check("cg_fastq_submit_gzip", c && slot && res, format, "submission", gz, n_bytes);
+    if (rc != CG_OK) return rc;
     GzinStream *g = gzin_lookup(c, handle);
     if (!g) return fail(CG_EINVAL, "cg_fastq_submit_gzip: unknown handle");
     CU(cudaSetDevice(c->device));
     *slot = -1;
     memset(res, 0, sizeof *res);
-    const int si = c->fq_next;
+    int si;
+    if ((rc = fq_find(c, 1, "cg_fastq_submit_gzip: all slots are in flight, collect one first", &si)) != CG_OK) return rc;
     FastqSlot &f = c->fq[si];
-    if (f.busy) return fail(CG_EINVAL, "cg_fastq_submit_gzip: all slots are in flight, collect one first");
-    int rc;
     bool fin = false;
     if ((rc = fastq_slot_init(c, f)) != CG_OK) return rc;
     if ((rc = gzin_inflate(c, *g, gz, n_bytes, final != 0, f.stream, res, &fin)) != CG_OK) return rc;
@@ -2265,11 +2264,7 @@ extern "C" int cg_fastq_submit_gzip(cg_ctx *c, int32_t handle, const uint8_t *gz
     else if ((rc = gzin_cut(c, *g, k, gu_select_single(k.fasta, k.F, k.b0, 0), f.stream, &cut, &n_records)) != CG_OK)
         return rc;
     if ((rc = gzin_commit(c, *g, cut ? &f : nullptr, cut, n_records, f.stream, res)) != CG_OK) return rc;
-    if (cut) {
-        c->fq_next = (si + 1) % CG_FQ_SLOTS;
-        f.busy = true;
-        *slot = si;
-    }
+    if (cut) fq_take(c, si, slot);
     return CG_OK;
 }
 
@@ -2292,21 +2287,17 @@ extern "C" int cg_fastq_submit_gzip_interleaved(cg_ctx *c, int32_t handle, const
                                                 int32_t format, int32_t final, int32_t *slot1, int32_t *slot2,
                                                 cg_gzin_result *res)
 {
-    if (!c || !slot1 || !slot2 || !res || n_bytes < 0 || (n_bytes && !gz) || format < CG_FORMAT_FASTQ ||
-        format > CG_FORMAT_FASTQ_TO_FASTA)
-        return fail(CG_EINVAL, "cg_fastq_submit_gzip_interleaved: bad argument");
-    if (n_bytes >= (1LL << 31))
-        return fail(CG_EINVAL, "cg_fastq_submit_gzip_interleaved: a submission must be smaller than 2 GiB");
+    int rc = submit_check("cg_fastq_submit_gzip_interleaved", c && slot1 && slot2 && res, format, "submission", gz, n_bytes);
+    if (rc != CG_OK) return rc;
     GzinStream *g = gzin_lookup(c, handle);
     if (!g) return fail(CG_EINVAL, "cg_fastq_submit_gzip_interleaved: unknown handle");
     CU(cudaSetDevice(c->device));
     *slot1 = *slot2 = -1;
     memset(res, 0, sizeof *res);
-    const int s1 = c->fq_next, s2 = (s1 + 1) % CG_FQ_SLOTS;
-    FastqSlot &f1 = c->fq[s1], &f2 = c->fq[s2];
-    if (f1.busy || f2.busy)
-        return fail(CG_EINVAL, "cg_fastq_submit_gzip_interleaved: two free slots are needed, collect one first");
-    int rc;
+    int s1;
+    if ((rc = fq_find(c, 2, "cg_fastq_submit_gzip_interleaved: two free slots are needed, collect one first", &s1)) != CG_OK)
+        return rc;
+    FastqSlot &f1 = c->fq[s1], &f2 = c->fq[(s1 + 1) % CG_FQ_SLOTS];
     bool fin = false;
     if ((rc = fastq_slot_init(c, f1)) != CG_OK) return rc;
     if ((rc = gzin_inflate(c, *g, gz, n_bytes, final != 0, f1.stream, res, &fin)) != CG_OK) return rc;
@@ -2320,13 +2311,7 @@ extern "C" int cg_fastq_submit_gzip_interleaved(cg_ctx *c, int32_t handle, const
     if (!cut) return CG_OK;
     if ((rc = fastq_slot_init(c, f2)) != CG_OK) return rc;          // its chunk comes from the split
     if ((rc = fastq_slot_count(c, f2, 0)) != CG_OK) return rc;
-    f1.ilv = 1; f1.ilv_peer = s2;
-    f2.ilv = 2; f2.ilv_peer = s1;
-    f1.ilv_format = f2.ilv_format = format == CG_FORMAT_FASTA ? CG_FORMAT_FASTA : CG_FORMAT_FASTQ;
-    f1.busy = f2.busy = true;
-    c->fq_next = (s2 + 1) % CG_FQ_SLOTS;
-    *slot1 = s1;
-    *slot2 = s2;
+    fq_take(c, s1, slot1, slot2, format);
     return CG_OK;
 }
 
@@ -2335,22 +2320,19 @@ extern "C" int cg_fastq_submit_gzip_paired(cg_ctx *c, int32_t handle1, int32_t h
                                            int32_t final, int32_t *slot1, int32_t *slot2, cg_gzin_result *res1,
                                            cg_gzin_result *res2)
 {
-    if (!c || !slot1 || !slot2 || !res1 || !res2 || n_bytes1 < 0 || n_bytes2 < 0 || (n_bytes1 && !gz1) ||
-        (n_bytes2 && !gz2) || format < CG_FORMAT_FASTQ || format > CG_FORMAT_FASTQ_TO_FASTA || handle1 == handle2)
-        return fail(CG_EINVAL, "cg_fastq_submit_gzip_paired: bad argument");
-    if (n_bytes1 >= (1LL << 31) || n_bytes2 >= (1LL << 31))
-        return fail(CG_EINVAL, "cg_fastq_submit_gzip_paired: a submission must be smaller than 2 GiB");
+    int rc = submit_check("cg_fastq_submit_gzip_paired", c && slot1 && slot2 && res1 && res2 && handle1 != handle2, format,
+                          "submission", gz1, n_bytes1, gz2, n_bytes2);
+    if (rc != CG_OK) return rc;
     GzinStream *g1 = gzin_lookup(c, handle1), *g2 = gzin_lookup(c, handle2);
     if (!g1 || !g2) return fail(CG_EINVAL, "cg_fastq_submit_gzip_paired: unknown handle");
     CU(cudaSetDevice(c->device));
     *slot1 = *slot2 = -1;
     memset(res1, 0, sizeof *res1);
     memset(res2, 0, sizeof *res2);
-    const int s1 = c->fq_next, s2 = (s1 + 1) % CG_FQ_SLOTS;
-    FastqSlot &f1 = c->fq[s1], &f2 = c->fq[s2];
-    if (f1.busy || f2.busy)
-        return fail(CG_EINVAL, "cg_fastq_submit_gzip_paired: two free slots are needed, collect one first");
-    int rc;
+    int s1;
+    if ((rc = fq_find(c, 2, "cg_fastq_submit_gzip_paired: two free slots are needed, collect one first", &s1)) != CG_OK)
+        return rc;
+    FastqSlot &f1 = c->fq[s1], &f2 = c->fq[(s1 + 1) % CG_FQ_SLOTS];
     bool fin1 = false, fin2 = false;
     if ((rc = fastq_slot_init(c, f1)) != CG_OK) return rc;
     if ((rc = fastq_slot_init(c, f2)) != CG_OK) return rc;
@@ -2380,10 +2362,7 @@ extern "C" int cg_fastq_submit_gzip_paired(cg_ctx *c, int32_t handle1, int32_t h
     // a mate without bytes (the other file's last records) gets an empty chunk
     if (!cut1 && (rc = fastq_slot_count(c, f1, 0)) != CG_OK) return rc;
     if (!cut2 && (rc = fastq_slot_count(c, f2, 0)) != CG_OK) return rc;
-    f1.busy = f2.busy = true;
-    c->fq_next = (s2 + 1) % CG_FQ_SLOTS;
-    *slot1 = s1;
-    *slot2 = s2;
+    fq_take(c, s1, slot1, slot2);
     return CG_OK;
 }
 
@@ -2445,12 +2424,12 @@ static int fasta_stage_normalise(cg_ctx *c, FastqSlot &f, const cg_fastq_params 
     if ((rc = f.d_len.ensure((size_t)n + 1)) != CG_OK) return rc;
     if ((rc = f.d_origin.ensure((size_t)n * 2 + 2)) != CG_OK) return rc;
     CU(cg_launch_fasta_scatter(f.d_in.p, n_bytes, f.d_nl.p, g.n_nl, n_lines, d_off, d_idx, d_first, f.d_norm.p, f.d_rec.p,
-                               f.d_err, st));
-    CU(cg_launch_fasta_records(f.d_rec.p, n, n_norm, fp->cut_front, fp->cut_back, f.d_len.p, f.d_origin.p, f.d_counters + 1,
+                               f.d_err.p, st));
+    CU(cg_launch_fasta_records(f.d_rec.p, n, n_norm, fp->cut_front, fp->cut_back, f.d_len.p, f.d_origin.p, f.d_counters.p + 1,
                                st));
     c->launches += 2;
     int fa_err[2];
-    CU(cudaMemcpyAsync(fa_err, f.d_err, sizeof fa_err, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(fa_err, f.d_err.p, sizeof fa_err, cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
     if (fa_err[0]) return fastq_format_error(fa_err);
     std::swap(f.d_in, f.d_norm);                // every later kernel reads the normalised chunk
@@ -2572,13 +2551,13 @@ static int fastq_split_interleaved(cg_ctx *c, FastqSlot &f1, FastqSlot &f2, cuda
     const int err_init[2] = {0, 0x7FFFFFFF};
     for (FastqSlot *f : {&f1, &f2}) {
         if ((rc = f->d_tiles.ensure((size_t)cg_fastq_tiles(f->n_bytes) + 1)) != CG_OK) return rc;
-        CU(cudaMemsetAsync(f->d_counters, 0, (1 + CG_FQ_COUNTERS) * sizeof(unsigned long long), st));
-        CU(cudaMemcpyAsync(f->d_err, err_init, sizeof err_init, cudaMemcpyHostToDevice, st));
+        CU(cudaMemsetAsync(f->d_counters.p, 0, (1 + CG_FQ_COUNTERS) * sizeof(unsigned long long), st));
+        CU(cudaMemcpyAsync(f->d_err.p, err_init, sizeof err_init, cudaMemcpyHostToDevice, st));
         if (f->n_bytes) {
-            CU(cg_launch_fastq_index(f->d_in.p, f->n_bytes, f->d_tiles.p, f->d_counters, nullptr, 0, st));
+            CU(cg_launch_fastq_index(f->d_in.p, f->n_bytes, f->d_tiles.p, f->d_counters.p, nullptr, 0, st));
             c->launches += 2;
         }
-        CU(cudaMemcpyAsync(f->h_counters.p, f->d_counters, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+        CU(cudaMemcpyAsync(f->h_counters.p, f->d_counters.p, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
     }
     CU(cudaStreamSynchronize(st));
     return CG_OK;
@@ -2639,7 +2618,7 @@ static int fastq_stage_records(cg_ctx *c, FastqSlot &f, const cg_fastq_params *f
     if (!fasta) {
         CU(cg_launch_fastq_index(f.d_in.p, n_bytes, f.d_tiles.p, nullptr, f.d_nl.p, 1, st));
         CU(cg_launch_fastq_records(f.d_in.p, n_bytes, f.d_nl.p, g.n_nl, n, fp->cut_front, fp->cut_back, f.d_rec.p, f.d_len.p,
-                                   f.d_origin.p, f.d_counters + 1, f.d_err, st));
+                                   f.d_origin.p, f.d_counters.p + 1, f.d_err.p, st));
         c->launches += 2;
     }
     g.d_qtrim = g.want_q ? f.d_qtrim.p : nullptr;
@@ -2662,7 +2641,7 @@ static int fastq_stage_fold_qtrim(cg_ctx *c, FastqSlot &f, const cg_params *p, c
     if (!g.want_q) return CG_OK;
     int rc = fastq_stage_pretrim(c, f, p, st, g);
     if (rc != CG_OK) return rc;
-    CU(cg_launch_fastq_fold_qtrim(f.d_rec.p, f.d_len.p, g.d_qtrim, g.n, f.d_origin.p, f.d_counters + 1, st));
+    CU(cg_launch_fastq_fold_qtrim(f.d_rec.p, f.d_len.p, g.d_qtrim, g.n, f.d_origin.p, f.d_counters.p + 1, st));
     c->launches += 1;
     g.d_qtrim = nullptr;
     g.want_q = false;
@@ -2691,7 +2670,7 @@ static int fastq_stage_pack(cg_ctx *c, FastqSlot &f, cudaStream_t st, FqStage &g
     c->launches += 1;
     int fq_err[2];
     CU(cudaMemcpyAsync(&g.max_len, c->d_err + 1, sizeof(int), cudaMemcpyDeviceToHost, st));
-    CU(cudaMemcpyAsync(fq_err, f.d_err, sizeof fq_err, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(fq_err, f.d_err.p, sizeof fq_err, cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
     if (fq_err[0]) return fastq_format_error(fq_err, f.ilv);
     return CG_OK;
@@ -2721,7 +2700,7 @@ static int fastq_stage_verdict(cg_ctx *c, FastqSlot &f, const cg_fastq_params *f
     flt.discard_casava = fp->discard_casava;
     flt.action = g.action;
     CU(cg_launch_fastq_evaluate(f.d_in.p, f.d_rec.p, f.d_len.p, g.n, g.d_matches, g.times, g.slots, g.d_qtrim, flt,
-                                c->d_phred, g.d_is_rc, f.d_interval.p, f.d_keep.p, f.d_mask.p, f.d_counters + 1, f.d_err,
+                                c->d_phred, g.d_is_rc, f.d_interval.p, f.d_keep.p, f.d_mask.p, f.d_counters.p + 1, f.d_err.p,
                                 st, d_poly_a));
     c->launches += 1;
     return CG_OK;
@@ -2864,7 +2843,7 @@ static int fastq_stage_evaluate(cg_ctx *c, FastqSlot &f, const cg_adapterset *s,
         rc = launch_trim(c, s, f.d_seq.p, nullptr, f.d_offs.p, n, g.max_len, &pt, f.d_matches_rc.p, nullptr, st, true);
         if (rc != CG_OK) return rc;
         CU(cg_launch_fastq_revcomp_commit(f.d_in.p, f.d_rec.p, f.d_len.p, f.d_origin.p, n, f.d_matches.p, f.d_matches_rc.p, (int)per_read,
-                                          f.d_isrc.p, f.d_counters + 1, st, g.has_qual() ? 1 : 0));
+                                          f.d_isrc.p, f.d_counters.p + 1, st, g.has_qual() ? 1 : 0));
         c->launches += 1;
         g.d_matches = f.d_matches.p;
         g.d_is_rc = f.d_isrc.p;
@@ -2950,8 +2929,8 @@ static int split_check(const FqSplit &sp, const cg_fastq_params *fp, const char 
 static int fastq_stage_result(FastqSlot &f, const FqStage &g, cudaStream_t st, cg_fastq_result *res)
 {
     int fq_err[2];
-    CU(cudaMemcpyAsync(fq_err, f.d_err, sizeof fq_err, cudaMemcpyDeviceToHost, st));
-    CU(cudaMemcpyAsync(f.h_counters.p, f.d_counters, (1 + CG_FQ_COUNTERS) * sizeof(unsigned long long),
+    CU(cudaMemcpyAsync(fq_err, f.d_err.p, sizeof fq_err, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(f.h_counters.p, f.d_counters.p, (1 + CG_FQ_COUNTERS) * sizeof(unsigned long long),
                        cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
     if (fq_err[0]) return fastq_format_error(fq_err, f.ilv);
@@ -3062,63 +3041,100 @@ static int gzip_check(const cg_fastq_params *fp, const char *who)
     return CG_OK;
 }
 
-// sizes -> offsets -> formatted records -> host; counters.  segments (host, n_dest + 1 values): where each destination
-// starts in `out`.
-static int fastq_stage_output(cg_ctx *c, FastqSlot &f, const FqStage &g, cudaStream_t st, uint8_t *out,
-                              int64_t out_capacity, cg_fastq_result *res, const FqDemux *dm = nullptr,
-                              int64_t *segments = nullptr, const FqSplit *sp = nullptr, int gzip_outputs = 0)
+// A mate of a collect: its slot and stage, its parameters and the caller's output for it
+struct FqMate {
+    FastqSlot *f = nullptr;
+    FqStage *g = nullptr;
+    const cg_fastq_params *fp = nullptr;
+    uint8_t *out = nullptr;
+    int64_t capacity = 0;
+    cg_fastq_result *res = nullptr;
+    int64_t *segments = nullptr;          // host, or null: where each destination starts in out
+};
+
+// The formatted records of a collect to the callers' outputs.  write(d_out) fills the device buffer; bounds (host) are
+// its destinations, the n_out (1 or 2) outputs m[i] take an equal share of them in order.  With gzip (the caller asked
+// for gzip outputs) the records go through fastq_gzip, destination d compressed when gz[d], before the capacity checks;
+// bounds, out_bytes and segments then describe the packed bytes.  Without, the checks come before the records are
+// written.  The scratch and the bounce buffer are slot f's.
+template <class Write>
+static int fastq_emit(cg_ctx *c, FastqSlot &f, std::vector<int64_t> &bounds, const std::vector<char> &gz, bool gzip,
+                      const FqMate *m, int n_out, const char *who, cudaStream_t st, Write write)
 {
+    const size_t per = (bounds.size() - 1) / (size_t)n_out;
+    const bool pack = gzip && bounds.back() > 0;
+    int rc;
+    if (pack) {
+        if ((rc = f.d_out.ensure((size_t)bounds.back() + 64)) != CG_OK) return rc;
+        if ((rc = write(f.d_out.p)) != CG_OK) return rc;
+        long long packed = 0;
+        if ((rc = fastq_gzip(c, f, f.d_out.p, bounds, gz, &packed, st)) != CG_OK) return rc;
+        for (int i = 0; i < n_out; ++i) m[i].res->out_bytes = bounds[(i + 1) * per] - bounds[i * per];
+    }
+    std::string need;
+    bool small = false, null = false;
+    for (int i = 0; i < n_out; ++i) {
+        const int64_t bytes = bounds[(i + 1) * per] - bounds[i * per];
+        need += (i ? " and " : "") + std::to_string(bytes);
+        small |= bytes > m[i].capacity;
+        null |= bytes && !m[i].out;
+    }
+    if (small) return fail(CG_EINVAL, std::string(who) + ": output buffer too small (" + need + " bytes needed)");
+    if (null) return fail(CG_EINVAL, std::string(who) + ": out is NULL");
+    if (pack) {
+        for (int i = 0; i < n_out; ++i)
+            if (m[i].segments)
+                for (size_t d = 0; d <= per; ++d) m[i].segments[d] = bounds[i * per + d] - bounds[i * per];
+    } else {
+        if (bounds.back() == 0) return CG_OK;
+        if ((rc = f.d_out.ensure((size_t)bounds.back() + 64)) != CG_OK) return rc;
+        if ((rc = write(f.d_out.p)) != CG_OK) return rc;
+    }
+    const uint8_t *d_src = pack ? f.d_gzout.p : f.d_out.p;
+    for (int i = 0; i < n_out; ++i)
+        if ((rc = fastq_copy_out(c, f, m[i].out, d_src + bounds[i * per], bounds[(i + 1) * per] - bounds[i * per], st)) !=
+            CG_OK)
+            return rc;
+    return CG_OK;
+}
+
+// sizes -> offsets -> formatted records -> host; counters.  m.segments (n_dest + 1 values): where each destination
+// starts in m.out.
+static int fastq_stage_output(cg_ctx *c, const FqMate &m, cudaStream_t st, const FqDemux *dm, const FqSplit *sp)
+{
+    FastqSlot &f = *m.f;
+    const FqStage &g = *m.g;
     const long long n = g.n;
     int rc;
     long long total = 0;
     if (dm || sp) {
         rc = fastq_partition(c, f, n, dm ? dm->n_dest() : FqSplit::n_dest, f.d_outlen.p, dm ? dm->d_dest : sp->d_route,
-                             segments, &total, st);
+                             m.segments, &total, st);
         if (rc != CG_OK) return rc;
     } else {
         CU(cg_launch_scan_i32(f.d_outlen.p, n, f.d_scan.p, f.d_outoff.p, st));
         c->launches += 3;
         CU(cudaMemcpyAsync(&total, f.d_outoff.p + n, sizeof total, cudaMemcpyDeviceToHost, st));
     }
-    if ((rc = fastq_stage_result(f, g, st, res)) != CG_OK) return rc;
-    res->out_bytes = res->out_bytes_plain = total;
-    if (gzip_outputs && total > 0) {
-        const int n_dest = dm ? dm->n_dest() : sp ? FqSplit::n_dest : 1;
-        std::vector<int64_t> bounds{0, (int64_t)total};
-        if (segments) bounds.assign(segments, segments + n_dest + 1);
-        std::vector<char> gz((size_t)n_dest);
-        for (int d = 0; d < n_dest; ++d) gz[(size_t)d] = gzip_dest(gzip_outputs, dm != nullptr, d);
-        if ((rc = f.d_out.ensure((size_t)total + 64)) != CG_OK) return rc;
-        if ((rc = fastq_write_records(c, f, g, f.d_out.p, sp, segments, st)) != CG_OK) return rc;
-        long long packed = 0;
-        if ((rc = fastq_gzip(c, f, f.d_out.p, bounds, gz, &packed, st)) != CG_OK) return rc;
-        res->out_bytes = packed;
-        if (packed > out_capacity)
-            return fail(CG_EINVAL, "cg_fastq_collect: output buffer too small (" + std::to_string(packed) + " bytes needed)");
-        if (!out) return fail(CG_EINVAL, "cg_fastq_collect: out is NULL");
-        if (segments) std::copy(bounds.begin(), bounds.end(), segments);
-        return fastq_copy_out(c, f, out, f.d_gzout.p, packed, st);
-    }
-    if (total > out_capacity)
-        return fail(CG_EINVAL, "cg_fastq_collect: output buffer too small (" + std::to_string(total) + " bytes needed)");
-    if (total > 0) {
-        if (!out) return fail(CG_EINVAL, "cg_fastq_collect: out is NULL");
-        if ((rc = f.d_out.ensure((size_t)total + 64)) != CG_OK) return rc;
-        if ((rc = fastq_write_records(c, f, g, f.d_out.p, sp, segments, st)) != CG_OK) return rc;
-        if ((rc = fastq_copy_out(c, f, out, f.d_out.p, total, st)) != CG_OK) return rc;
-    }
-    return CG_OK;
+    if ((rc = fastq_stage_result(f, g, st, m.res)) != CG_OK) return rc;
+    m.res->out_bytes = m.res->out_bytes_plain = total;
+    const int n_dest = dm ? dm->n_dest() : sp ? FqSplit::n_dest : 1;
+    std::vector<int64_t> bounds{0, (int64_t)total};
+    if (m.segments) bounds.assign(m.segments, m.segments + n_dest + 1);
+    std::vector<char> gz((size_t)n_dest);
+    for (int d = 0; d < n_dest; ++d) gz[(size_t)d] = gzip_dest(m.fp->gzip_outputs, dm != nullptr, d);
+    return fastq_emit(c, f, bounds, gz, m.fp->gzip_outputs != 0, &m, 1, "cg_fastq_collect", st,
+                      [&](uint8_t *d_out) { return fastq_write_records(c, f, g, d_out, sp, m.segments, st); });
 }
 
 // Interleaved outputs (cg_fastq_collect_paired_interleaved): bit d of sp.ilv_dests = destination d gets both mates in
 // out1, R1 then R2 per pair.  The pair's sizes are folded into mate 1 for the partition, mate 2 then follows its mate 1
-// (off1 + len1); both mates go through the writer into one device buffer, mate 1's region (total1 bytes) then mate 2's,
-// which two copies return.
-static int fastq_stage_output_interleaved(cg_ctx *c, FastqSlot &f1, const FqStage &g1, FastqSlot &f2, const FqStage &g2,
-                                          cudaStream_t st, uint8_t *out1, int64_t out_capacity1, uint8_t *out2,
-                                          int64_t out_capacity2, cg_fastq_result *res1, cg_fastq_result *res2,
-                                          int64_t *segments1, int64_t *segments2, const FqSplit &sp, int gzip1, int gzip2)
+// (off1 + len1); both mates go through the writer into one device buffer, mate 1's region (total1 bytes) then mate 2's.
+static int fastq_stage_output_interleaved(cg_ctx *c, const FqMate *m, const FqSplit &sp, cudaStream_t st)
 {
+    FastqSlot &f1 = *m[0].f, &f2 = *m[1].f;
+    const FqStage &g1 = *m[0].g, &g2 = *m[1].g;
+    int64_t *segments1 = m[0].segments, *segments2 = m[1].segments;
     const long long n = g1.n;
     int rc;
     if ((rc = f1.d_fold.ensure((size_t)n)) != CG_OK) return rc;
@@ -3132,51 +3148,27 @@ static int fastq_stage_output_interleaved(cg_ctx *c, FastqSlot &f1, const FqStag
     CU(cg_launch_fastq_interleave(1, n, sp.d_route, sp.ilv_dests, f1.d_outlen.p, f2.d_outlen.p, nullptr, nullptr,
                                   f1.d_outoff.p, f2.d_outoff.p, f1.d_dmbase.p + cg_demux_tiles(n) * FqSplit::n_dest, st));
     c->launches += 1;
-    if ((rc = fastq_stage_result(f1, g1, st, res1)) != CG_OK) return rc;
-    if ((rc = fastq_stage_result(f2, g2, st, res2)) != CG_OK) return rc;
-    res1->out_bytes = res1->out_bytes_plain = total1;
-    res2->out_bytes = res2->out_bytes_plain = total2;
-    if ((gzip1 || gzip2) && total1 + total2 > 0) {
-        // out1's four destinations, then out2's, in the one buffer the writer fills
-        std::vector<int64_t> bounds(2 * FqSplit::n_dest + 1);
-        std::vector<char> gz(2 * FqSplit::n_dest);
-        for (int d = 0; d < FqSplit::n_dest; ++d) {
-            bounds[d] = segments1[d];
-            bounds[FqSplit::n_dest + d] = total1 + segments2[d];
-            gz[d] = gzip_dest(gzip1, false, d);
-            gz[FqSplit::n_dest + d] = gzip_dest(gzip2, false, d);
-        }
-        bounds[2 * FqSplit::n_dest] = total1 + total2;
-        if ((rc = f1.d_out.ensure((size_t)(total1 + total2) + 64)) != CG_OK) return rc;
-        if ((rc = fastq_write_records(c, f1, g1, f1.d_out.p, &sp, segments1, st)) != CG_OK) return rc;
-        if ((rc = fastq_write_records(c, f2, g2, f1.d_out.p, &sp, segments1, st)) != CG_OK) return rc;
-        long long packed = 0;
-        if ((rc = fastq_gzip(c, f1, f1.d_out.p, bounds, gz, &packed, st)) != CG_OK) return rc;
-        const int64_t packed1 = bounds[FqSplit::n_dest], packed2 = packed - packed1;
-        res1->out_bytes = packed1;
-        res2->out_bytes = packed2;
-        if (packed1 > out_capacity1 || packed2 > out_capacity2)
-            return fail(CG_EINVAL, "cg_fastq_collect_paired_interleaved: output buffer too small (" + std::to_string(packed1) +
-                                       " and " + std::to_string(packed2) + " bytes needed)");
-        if ((packed1 && !out1) || (packed2 && !out2)) return fail(CG_EINVAL, "cg_fastq_collect_paired_interleaved: out is NULL");
-        for (int d = 0; d <= FqSplit::n_dest; ++d) {
-            segments1[d] = bounds[d];
-            segments2[d] = bounds[FqSplit::n_dest + d] - packed1;
-        }
-        if ((rc = fastq_copy_out(c, f1, out1, f1.d_gzout.p, packed1, st)) != CG_OK) return rc;
-        return fastq_copy_out(c, f2, out2, f1.d_gzout.p + packed1, packed2, st);
+    if ((rc = fastq_stage_result(f1, g1, st, m[0].res)) != CG_OK) return rc;
+    if ((rc = fastq_stage_result(f2, g2, st, m[1].res)) != CG_OK) return rc;
+    m[0].res->out_bytes = m[0].res->out_bytes_plain = total1;
+    m[1].res->out_bytes = m[1].res->out_bytes_plain = total2;
+    // out1's four destinations, then out2's, in the one buffer the writer fills
+    std::vector<int64_t> bounds(2 * FqSplit::n_dest + 1);
+    std::vector<char> gz(2 * FqSplit::n_dest);
+    for (int d = 0; d < FqSplit::n_dest; ++d) {
+        bounds[d] = segments1[d];
+        bounds[FqSplit::n_dest + d] = total1 + segments2[d];
+        gz[d] = gzip_dest(m[0].fp->gzip_outputs, false, d);
+        gz[FqSplit::n_dest + d] = gzip_dest(m[1].fp->gzip_outputs, false, d);
     }
-    if (total1 > out_capacity1 || total2 > out_capacity2)
-        return fail(CG_EINVAL, "cg_fastq_collect_paired_interleaved: output buffer too small (" + std::to_string(total1) +
-                                   " and " + std::to_string(total2) + " bytes needed)");
-    if ((total1 && !out1) || (total2 && !out2)) return fail(CG_EINVAL, "cg_fastq_collect_paired_interleaved: out is NULL");
-    if (total1 + total2 == 0) return CG_OK;
-    if ((rc = f1.d_out.ensure((size_t)(total1 + total2) + 64)) != CG_OK) return rc;
-    // a pair has bytes in a destination for both mates or for neither: segments1 says which formats mate 2 needs too
-    if ((rc = fastq_write_records(c, f1, g1, f1.d_out.p, &sp, segments1, st)) != CG_OK) return rc;
-    if ((rc = fastq_write_records(c, f2, g2, f1.d_out.p, &sp, segments1, st)) != CG_OK) return rc;
-    if ((rc = fastq_copy_out(c, f1, out1, f1.d_out.p, total1, st)) != CG_OK) return rc;
-    return fastq_copy_out(c, f2, out2, f1.d_out.p + total1, total2, st);
+    bounds[2 * FqSplit::n_dest] = total1 + total2;
+    return fastq_emit(c, f1, bounds, gz, m[0].fp->gzip_outputs || m[1].fp->gzip_outputs, m, 2,
+                      "cg_fastq_collect_paired_interleaved", st, [&](uint8_t *d_out) {
+                          // a pair has bytes in a destination for both mates or for neither: segments1 says which formats
+                          // mate 2 needs too
+                          int rc2 = fastq_write_records(c, f1, g1, d_out, &sp, segments1, st);
+                          return rc2 != CG_OK ? rc2 : fastq_write_records(c, f2, g2, d_out, &sp, segments1, st);
+                      });
 }
 
 // --info-file rows of a chunk, an extra output of a collect
@@ -3227,6 +3219,51 @@ static int fastq_stage_info(cg_ctx *c, FastqSlot &f, const FqStage &g, const cg_
     return CG_OK;
 }
 
+// The part of a collect after the evaluation, for one mate (n_mates 1) or a pair, on stream st: the routes, the finish
+// kernel, the statistics, the output, the error flag and the statistics commit.  Both mates share one route per pair,
+// held by mate 1's slot.
+static int fastq_collect_finish(cg_ctx *c, const FqMate *m, int n_mates, FqDemux *dm, FqSplit *sp, int pair_filter_mode,
+                                int mode_untrimmed, cudaStream_t st)
+{
+    const long long n = m[0].g->n;
+    FastqSlot *f[2] = {};
+    const CgFastqRecord *rec[2] = {};
+    const int32_t *interval[2] = {}, *mask[2] = {};
+    int32_t *outlen[2] = {};
+    unsigned long long *counters[2] = {};
+    int enabled[2] = {};
+    for (int i = 0; i < n_mates; ++i) {
+        f[i] = m[i].f;
+        rec[i] = f[i]->d_rec.p; interval[i] = f[i]->d_interval.p; mask[i] = f[i]->d_mask.p; outlen[i] = f[i]->d_outlen.p;
+        counters[i] = f[i]->d_counters.p + 1;
+        enabled[i] = fastq_enabled_filters(m[i].fp);
+    }
+    int rc;
+    if (dm && (rc = fastq_stage_route(c, *f[0], f[1], n, *dm, st)) != CG_OK) return rc;
+    if (sp) {
+        if ((rc = f[0]->d_dest.ensure((size_t)n)) != CG_OK) return rc;
+        sp->d_route = f[0]->d_dest.p;
+        for (int i = 0; i < n_mates; ++i) enabled[i] = fq_route_enabled(enabled[i], sp->redirect);
+    }
+    CU(cg_launch_fastq_finish(n, rec[0], interval[0], mask[0], enabled[0], outlen[0], counters[0], rec[1], interval[1],
+                              mask[1], enabled[1], outlen[1], counters[1], pair_filter_mode, mode_untrimmed,
+                              m[0].g->rc_suffix, dm ? dm->d_dest : nullptr, dm ? dm->d_dest_keep : nullptr, st,
+                              m[0].g->fasta_out() ? 1 : 0, sp ? sp->redirect : 0, sp ? sp->fasta_dests : 0,
+                              sp ? sp->d_route : nullptr));
+    c->launches += 1;
+    for (int i = 0; i < n_mates; ++i)
+        if ((rc = fastq_stage_stats_tail(c, *f[i], *m[i].g, st, sp ? sp->d_route : nullptr)) != CG_OK) return rc;
+    if (sp && sp->interleaved) {
+        if ((rc = fastq_stage_output_interleaved(c, m, *sp, st)) != CG_OK) return rc;
+    } else {
+        for (int i = 0; i < n_mates; ++i)
+            if ((rc = fastq_stage_output(c, m[i], st, dm, sp)) != CG_OK) return rc;
+    }
+    if ((rc = check_err_flag(c)) != CG_OK) return rc;
+    for (int i = 0; i < n_mates; ++i) fastq_stats_commit(*f[i], *m[i].g, m[i].fp, *m[i].res);
+    return CG_OK;
+}
+
 static int fastq_collect_impl(cg_ctx *c, int32_t slot, const cg_adapterset *s, const cg_fastq_params *fp,
                               uint8_t *out, int64_t out_capacity, cg_fastq_result *res, FqDemux *dm, int64_t *segments,
                               const FqInfo *info = nullptr, FqSplit *sp = nullptr)
@@ -3248,24 +3285,9 @@ static int fastq_collect_impl(cg_ctx *c, int32_t slot, const cg_adapterset *s, c
     rc = fastq_stage_evaluate(c, f, s, fp, 1, f.stream, g);
     if (rc != CG_OK || g.n == 0) return rc;
     if (info && (rc = fastq_stage_info(c, f, g, fp, *info, f.stream)) != CG_OK) return rc;
-    if (dm && (rc = fastq_stage_route(c, f, nullptr, g.n, *dm, f.stream)) != CG_OK) return rc;
-    int enabled = fastq_enabled_filters(fp);
-    if (sp) {
-        if ((rc = f.d_dest.ensure((size_t)g.n)) != CG_OK) return rc;
-        sp->d_route = f.d_dest.p;
-        enabled = fq_route_enabled(enabled, sp->redirect);
-    }
-    CU(cg_launch_fastq_finish(g.n, f.d_rec.p, f.d_interval.p, f.d_mask.p, enabled, f.d_outlen.p,
-                              f.d_counters + 1, nullptr, nullptr, nullptr, 0, nullptr, nullptr, 0, 0, g.rc_suffix,
-                              dm ? dm->d_dest : nullptr, dm ? dm->d_dest_keep : nullptr, f.stream, g.fasta_out() ? 1 : 0,
-                              sp ? sp->redirect : 0, sp ? sp->fasta_dests : 0, sp ? sp->d_route : nullptr));
-    c->launches += 1;
-    if ((rc = fastq_stage_stats_tail(c, f, g, f.stream, sp ? sp->d_route : nullptr)) != CG_OK) return rc;
-    if ((rc = fastq_stage_output(c, f, g, f.stream, out, out_capacity, res, dm, segments, sp, fp->gzip_outputs)) != CG_OK)
-        return rc;
-    if ((rc = check_err_flag(c)) != CG_OK) return rc;
-    fastq_stats_commit(f, g, fp, *res);
-    return CG_OK;
+    FqMate m;
+    m.f = &f; m.g = &g; m.fp = fp; m.out = out; m.capacity = out_capacity; m.res = res; m.segments = segments;
+    return fastq_collect_finish(c, &m, 1, dm, sp, 0, 0, f.stream);
 }
 
 extern "C" int cg_fastq_collect(cg_ctx *c, int32_t slot, const cg_adapterset *s, const cg_fastq_params *fp,
@@ -3435,95 +3457,60 @@ static int fastq_collect_paired_impl(cg_ctx *c, int32_t slot1, int32_t slot2, co
                                "slots go in the order cg_fastq_submit_interleaved gave them)");
     CU(cudaSetDevice(c->device));
     f1.busy = f2.busy = false;
+    // The slots are free again: every exit waits until mate 2's upload, on its own stream, is done with the caller's
+    // buffer and the slot's.  Everything after it runs on mate 1's stream.
+    struct StreamWait {
+        cudaStream_t s;
+        ~StreamWait() { cudaStreamSynchronize(s); }
+    } wait_mate2{f2.stream};
     if (fp1->format != fp2->format) return fail(CG_EINVAL, "cg_fastq_collect_paired: both mates must have the same format");
     memset(res1, 0, sizeof *res1);
     memset(res2, 0, sizeof *res2);
-    // after its upload everything of the second mate runs on the first mate's stream
     cudaStream_t st = f1.stream;
     FqStage g1, g2;
     int rc;
     if (f1.ilv) {
-        if ((fp1->format == CG_FORMAT_FASTA) != (f1.ilv_format == CG_FORMAT_FASTA)) {
-            cudaStreamSynchronize(f2.stream);
+        if ((fp1->format == CG_FORMAT_FASTA) != (f1.ilv_format == CG_FORMAT_FASTA))
             return fail(CG_EINVAL, "cg_fastq_collect_paired: the input format of the parameters is not the one the "
                                    "interleaved chunk was submitted with");
-        }
         if ((rc = fastq_split_interleaved(c, f1, f2, st)) != CG_OK) return rc;
     }
     // one statistics accumulator per mate, as the reference keeps per-mate statistics (report.py:162-208)
-    if (fp1->stats != 0 && fp1->stats == fp2->stats) {
-        cudaStreamSynchronize(f2.stream);
+    if (fp1->stats != 0 && fp1->stats == fp2->stats)
         return fail(CG_EINVAL, "cg_fastq_collect_paired: the two mates need different statistics handles");
-    }
     if (sp && ((rc = split_check(*sp, fp1, "cg_fastq_collect_paired_split")) != CG_OK ||
-               (rc = split_check(*sp, fp2, "cg_fastq_collect_paired_split")) != CG_OK)) {
-        cudaStreamSynchronize(f2.stream);
+               (rc = split_check(*sp, fp2, "cg_fastq_collect_paired_split")) != CG_OK))
         return rc;
-    }
-    if ((rc = gzip_check(fp1, "cg_fastq_collect_paired")) != CG_OK || (rc = gzip_check(fp2, "cg_fastq_collect_paired")) != CG_OK) {
-        cudaStreamSynchronize(f2.stream);
+    if ((rc = gzip_check(fp1, "cg_fastq_collect_paired")) != CG_OK || (rc = gzip_check(fp2, "cg_fastq_collect_paired")) != CG_OK)
         return rc;
-    }
     if (sp && sp->interleaved) {
         // an interleaved destination holds both mates: both must agree on compressing it
         const int ilv_bits = ((sp->ilv_dests & 1) ? CG_GZIP_MAIN : 0) | (sp->ilv_dests >> 1);
-        if ((fp1->gzip_outputs ^ fp2->gzip_outputs) & ilv_bits) {
-            cudaStreamSynchronize(f2.stream);
+        if ((fp1->gzip_outputs ^ fp2->gzip_outputs) & ilv_bits)
             return fail(CG_EINVAL, "cg_fastq_collect_paired_interleaved: an interleaved output must have its gzip_outputs bit "
                                    "set alike in both mates' parameters");
-        }
     }
     if ((rc = fqstats_lookup(c, fp1->stats, pa ? pa->n_pairs : (s1 ? s1->host.n_adapters : 0), &g1.acc)) != CG_OK ||
-        (rc = fqstats_lookup(c, fp2->stats, pa ? pa->n_pairs : (s2 ? s2->host.n_adapters : 0), &g2.acc)) != CG_OK) {
-        cudaStreamSynchronize(f2.stream);
+        (rc = fqstats_lookup(c, fp2->stats, pa ? pa->n_pairs : (s2 ? s2->host.n_adapters : 0), &g2.acc)) != CG_OK)
         return rc;
-    }
     if (pa) {
-        CU(cudaStreamSynchronize(f2.stream));
         if ((rc = fastq_stage_pair_adapters(c, f1, f2, *pa, fp1, fp2, st, g1, g2)) != CG_OK) return rc;
     } else {
-        rc = fastq_stage_evaluate(c, f1, s1, fp1, 1, st, g1);
-        if (rc != CG_OK) { cudaStreamSynchronize(f2.stream); return rc; }
+        if ((rc = fastq_stage_evaluate(c, f1, s1, fp1, 1, st, g1)) != CG_OK) return rc;
         if ((rc = fastq_stage_evaluate(c, f2, s2, fp2, 2, st, g2)) != CG_OK) return rc;
     }
     if (g1.n != g2.n)
         return fail(CG_EINVAL, "paired FASTQ chunks differ in their number of records (" + std::to_string(g1.n) + " vs " +
                                    std::to_string(g2.n) + ")");
     if (g1.n == 0) return CG_OK;
-    if (dm && (rc = fastq_stage_route(c, f1, &f2, g1.n, *dm, st)) != CG_OK) return rc;
     // --discard-untrimmed with adapters on one mate only tests "both" (cli.py:859-893)
     const int mode_untrimmed = (!pa && (!s1 || !s2)) ? 1 : pair_filter_mode;
-    int enabled1 = fastq_enabled_filters(fp1), enabled2 = fastq_enabled_filters(fp2);
-    if (sp) {
-        // both mates share one destination per pair (the first mate's slot holds it)
-        if ((rc = f1.d_dest.ensure((size_t)g1.n)) != CG_OK) return rc;
-        sp->d_route = f1.d_dest.p;
-        enabled1 = fq_route_enabled(enabled1, sp->redirect);
-        enabled2 = fq_route_enabled(enabled2, sp->redirect);
-    }
-    CU(cg_launch_fastq_finish(g1.n, f1.d_rec.p, f1.d_interval.p, f1.d_mask.p, enabled1, f1.d_outlen.p,
-                              f1.d_counters + 1, f2.d_rec.p, f2.d_interval.p, f2.d_mask.p, enabled2,
-                              f2.d_outlen.p, f2.d_counters + 1, pair_filter_mode, mode_untrimmed, 0,
-                              dm ? dm->d_dest : nullptr, dm ? dm->d_dest_keep : nullptr, st, g1.fasta_out() ? 1 : 0,
-                              sp ? sp->redirect : 0, sp ? sp->fasta_dests : 0, sp ? sp->d_route : nullptr));
-    c->launches += 1;
-    const int32_t *route = sp ? sp->d_route : nullptr;
-    if ((rc = fastq_stage_stats_tail(c, f1, g1, st, route)) != CG_OK) return rc;
-    if ((rc = fastq_stage_stats_tail(c, f2, g2, st, route)) != CG_OK) return rc;
-    if (sp && sp->interleaved) {
-        rc = fastq_stage_output_interleaved(c, f1, g1, f2, g2, st, out1, out_capacity1, out2, out_capacity2, res1, res2,
-                                            segments1, segments2, *sp, fp1->gzip_outputs, fp2->gzip_outputs);
-        if (rc != CG_OK) return rc;
-    } else {
-        if ((rc = fastq_stage_output(c, f1, g1, st, out1, out_capacity1, res1, dm, segments1, sp, fp1->gzip_outputs)) != CG_OK)
-            return rc;
-        if ((rc = fastq_stage_output(c, f2, g2, st, out2, out_capacity2, res2, dm, segments2, sp, fp2->gzip_outputs)) != CG_OK)
-            return rc;
-    }
-    if ((rc = check_err_flag(c)) != CG_OK) return rc;
-    fastq_stats_commit(f1, g1, fp1, *res1);
-    fastq_stats_commit(f2, g2, fp2, *res2);
-    return CG_OK;
+    FqMate m[2];
+    m[0].f = &f1; m[0].g = &g1; m[0].fp = fp1; m[0].out = out1; m[0].capacity = out_capacity1; m[0].res = res1;
+    m[0].segments = segments1;
+    m[1].f = &f2; m[1].g = &g2; m[1].fp = fp2; m[1].out = out2; m[1].capacity = out_capacity2; m[1].res = res2;
+    m[1].segments = segments2;
+    return fastq_collect_finish(c, m, 2, dm, sp, pair_filter_mode, mode_untrimmed, st);
 }
 
 extern "C" int cg_fastq_collect_paired(cg_ctx *c, int32_t slot1, int32_t slot2, const cg_adapterset *s1,

@@ -717,6 +717,14 @@ def read_interleaved_fastq_chunks(f, buffer_size: int = 4 * 1024 * 1024):
 
 def read_paired_fastq_chunks(f1, f2, buffer_size: int = 4 * 1024 * 1024):
     """Pairs of chunks with the same number of complete records each (``dnaio.read_paired_chunks``)."""
+    return _read_paired_chunks(f1, f2, buffer_size, lambda buf, end: buf.count(b"\n", 0, _fastq_head(buf, end)) // 4,
+                               _cut_records)
+
+
+def _read_paired_chunks(f1, f2, buffer_size: int, count, cut):
+    """Pairs of chunks with the same number of complete records each: count(buf, end) is the number of complete
+    records in buf[:end], cut(buf, end, n) the offset just behind the first n of them.  Whatever is left at the end of
+    the files is the last pair."""
     bufs = [bytearray(buffer_size), bytearray(buffer_size)]
     starts = [0, 0]
     files = (f1, f2)
@@ -731,10 +739,9 @@ def read_paired_fastq_chunks(f1, f2, buffer_size: int = 4 * 1024 * 1024):
             ends[k] = starts[k] + (n or 0)
         if eof[0] and eof[1]:
             break
-        heads = [_fastq_head(bufs[k], ends[k]) for k in (0, 1)]
-        records = min(bufs[k].count(b"\n", 0, heads[k]) // 4 for k in (0, 1))
+        records = min(count(bufs[k], ends[k]) for k in (0, 1))
         if records:
-            cuts = [_cut_records(bufs[k], ends[k], records) for k in (0, 1)]
+            cuts = [cut(bufs[k], ends[k], records) for k in (0, 1)]
             yield bytes(bufs[0][:cuts[0]]), bytes(bufs[1][:cuts[1]])
             for k in (0, 1):
                 bufs[k][0:ends[k] - cuts[k]] = bufs[k][cuts[k]:ends[k]]
@@ -787,31 +794,8 @@ def read_interleaved_fasta_chunks(f, buffer_size: int = 4 * 1024 * 1024):
 
 def read_paired_fasta_chunks(f1, f2, buffer_size: int = 4 * 1024 * 1024):
     """Pairs of FASTA chunks with the same number of complete records each (see read_fasta_chunks)."""
-    bufs = [bytearray(buffer_size), bytearray(buffer_size)]
-    starts = [0, 0]
-    files = (f1, f2)
-    eof = [False, False]
-    while True:
-        ends = list(starts)
-        for k in (0, 1):
-            if starts[k] == len(bufs[k]):
-                bufs[k].extend(bytes(len(bufs[k])))
-            n = 0 if eof[k] else files[k].readinto(memoryview(bufs[k])[starts[k]:])
-            eof[k] = eof[k] or not n
-            ends[k] = starts[k] + (n or 0)
-        if eof[0] and eof[1]:
-            break
-        records = min(_fasta_headers(bufs[k], _fasta_head(bufs[k], ends[k])) for k in (0, 1))
-        if records:
-            cuts = [_fasta_cut(bufs[k], ends[k], records) for k in (0, 1)]
-            yield bytes(bufs[0][:cuts[0]]), bytes(bufs[1][:cuts[1]])
-            for k in (0, 1):
-                bufs[k][0:ends[k] - cuts[k]] = bufs[k][cuts[k]:ends[k]]
-                starts[k] = ends[k] - cuts[k]
-        else:
-            starts = ends
-    if starts[0] or starts[1]:
-        yield bytes(bufs[0][:starts[0]]), bytes(bufs[1][:starts[1]])
+    return _read_paired_chunks(f1, f2, buffer_size, lambda buf, end: _fasta_headers(buf, _fasta_head(buf, end)),
+                               _fasta_cut)
 
 
 class DeviceChunk:
@@ -824,6 +808,30 @@ class DeviceChunk:
 
     def __len__(self) -> int:
         return self.size
+
+
+def _submit_chunk(ctx, chunk):
+    """(slot, chunk) for the trimmers' collects: bytes or a uint8 array are uploaded (``cg_fastq_submit``) and come back
+    as the array, which has to stay alive until the collect; a DeviceChunk is in its slot already."""
+    if isinstance(chunk, DeviceChunk):
+        return chunk.slot, chunk
+    buf = np.frombuffer(chunk, dtype=np.uint8) if not isinstance(chunk, np.ndarray) else chunk
+    slot = C.c_int32(-1)
+    _lib.check(_lib.lib().cg_fastq_submit(ctx.handle, buf.ctypes.data if buf.size else None, buf.size, C.byref(slot)))
+    return slot.value, buf
+
+
+def _one_in_flight(items, submit, collect):
+    """collect(submit(item)) of every item in order, item i+1 submitted before item i is collected: its upload
+    overlaps the work on item i."""
+    pending = None
+    for item in items:
+        ticket = submit(item)
+        if pending is not None:
+            yield collect(pending)
+        pending = ticket
+    if pending is not None:
+        yield collect(pending)
 
 
 class _GzipInput:
@@ -1144,13 +1152,8 @@ class FastqTrimmer:
         self._out_bufs, self._out_keep = {}, {}
 
     def _submit(self, chunk) -> Tuple[int, int, object]:
-        if isinstance(chunk, DeviceChunk):
-            return chunk.slot, chunk.size, chunk
-        buf = np.frombuffer(chunk, dtype=np.uint8) if not isinstance(chunk, np.ndarray) else chunk
-        slot = C.c_int32(-1)
-        _lib.check(_lib.lib().cg_fastq_submit(self.ctx.handle, buf.ctypes.data if buf.size else None, buf.size,
-                                              C.byref(slot)))
-        return slot.value, buf.size, buf    # buf is kept alive until collect
+        slot, buf = _submit_chunk(self.ctx, chunk)
+        return slot, buf.size, buf
 
     def _capacity(self, n_bytes: int, n_dest: int = 4, chunk=None) -> int:
         # a device chunk cannot be submitted again, so FASTA output with " rc" suffixes gets room for all of them
@@ -1233,14 +1236,7 @@ class FastqTrimmer:
 
     def process_chunks_split(self, chunks, copy: bool = True):
         """process_chunk_split over an iterable with one chunk in flight (see process_chunks)."""
-        pending = None
-        for chunk in chunks:
-            ticket = self._submit(chunk)
-            if pending is not None:
-                yield self._collect_split(pending, copy)
-            pending = ticket
-        if pending is not None:
-            yield self._collect_split(pending, copy)
+        yield from _one_in_flight(chunks, self._submit, lambda ticket: self._collect_split(ticket, copy))
 
     def _demux_names(self):
         return _demux_names(self.adapters)
@@ -1367,14 +1363,7 @@ class FastqTrimmer:
     def process_chunks(self, chunks, copy: bool = True):
         """copy=False yields uint8 array views into per-slot buffers: valid until the next-but-one result."""
         self._no_redirect("process_chunks")
-        pending = None
-        for chunk in chunks:
-            ticket = self._submit(chunk)
-            if pending is not None:
-                yield self._collect(pending, copy)
-            pending = ticket
-        if pending is not None:
-            yield self._collect(pending, copy)
+        yield from _one_in_flight(chunks, self._submit, lambda ticket: self._collect(ticket, copy))
 
 
 class PairedFastqTrimmer:
@@ -1500,19 +1489,10 @@ class PairedFastqTrimmer:
     def written_lengths(self):
         return tuple(written_lengths(v, max_len) for v, max_len, _ in self.statistics_vector())
 
-    def _submit(self, chunk):
-        if isinstance(chunk, DeviceChunk):
-            return chunk.slot, chunk
-        buf = np.frombuffer(chunk, dtype=np.uint8) if not isinstance(chunk, np.ndarray) else chunk
-        slot = C.c_int32(-1)
-        _lib.check(_lib.lib().cg_fastq_submit(self.ctx.handle, buf.ctypes.data if buf.size else None, buf.size,
-                                              C.byref(slot)))
-        return slot.value, buf
-
     def _submit_pair(self, chunk1, chunk2):
         """((slot1, chunk), (slot2, chunk)): two chunks, or one interleaved chunk (chunk2 None) split on the device."""
         if chunk2 is not None:
-            return self._submit(chunk1), self._submit(chunk2)
+            return _submit_chunk(self.ctx, chunk1), _submit_chunk(self.ctx, chunk2)
         if isinstance(chunk1, DeviceChunk):            # interleaved, already split into two slots
             return (chunk1.slot, chunk1), (chunk1.slot2, chunk1)
         buf = np.frombuffer(chunk1, dtype=np.uint8) if not isinstance(chunk1, np.ndarray) else chunk1
@@ -1573,15 +1553,9 @@ class PairedFastqTrimmer:
     def process_chunks_split(self, pairs):
         """process_chunk_split over an iterable of (chunk1, chunk2), or of interleaved chunks, with one pair in flight:
         the upload of pair i+1 overlaps the work on pair i."""
-        pending = None
-        for item in pairs:
-            chunk1, chunk2 = item if isinstance(item, (tuple, list)) else (item, None)
-            tickets = self._submit_pair(chunk1, chunk2)
-            if pending is not None:
-                yield self._collect_split(pending)
-            pending = tickets
-        if pending is not None:
-            yield self._collect_split(pending)
+        yield from _one_in_flight(
+            pairs, lambda item: self._submit_pair(*(item if isinstance(item, (tuple, list)) else (item, None))),
+            self._collect_split)
 
     def process_chunk(self, chunk1, chunk2=None) -> Tuple[bytes, bytes]:
         """(R1, R2) of one pair of chunks or of one interleaved chunk (chunk2 None); with "output" in
