@@ -45,6 +45,9 @@ CG_REDIRECT_TOO_LONG = 2         # --too-long-output (destination 2)
 CG_REDIRECT_UNTRIMMED = 4        # --untrimmed-output (destination 3)
 CG_INTERLEAVE_MAIN = 8           # cg_fastq_collect_paired_interleaved: the main output is interleaved
 CG_GZIP_MAIN = 8                 # cg_fastq_params.gzip_outputs: the main (every demultiplexed) output is gzip
+CG_ROWS_INFO = 0                 # cg_fastq_request_rows: --info-file rows
+CG_ROWS_REST = 1                 # --rest-file rows
+CG_ROWS_WILDCARD = 2             # --wildcard-file rows
 GZ_MEMBER = 65280                # plain bytes per gzip member of a gzip output ...
 GZ_OVERHEAD = 23                 # ... and the most a member adds to them
 
@@ -206,6 +209,8 @@ def _declare(lib) -> None:
                                           C.POINTER(cg_fastq_result), C.POINTER(i64)]
     lib.cg_fastq_collect_rows.argtypes = [vp, i32, vp, C.POINTER(cg_fastq_params), i32, C.c_char_p, vp, vp, i64, vp, i64,
                                           C.POINTER(cg_fastq_result), C.POINTER(i64)]
+    lib.cg_fastq_request_rows.argtypes = [vp, i32, i32, C.c_char_p, vp, i32, i32]
+    lib.cg_fastq_read_rows.argtypes = [vp, i32, i32, vp, i64, C.POINTER(i64), C.POINTER(i64)]
     lib.cg_fastq_collect_pair_adapters.argtypes = [vp, i32, i32, vp, vp, i32, C.POINTER(cg_fastq_params),
                                                    C.POINTER(cg_fastq_params), i32, vp, i64, vp, i64,
                                                    C.POINTER(cg_fastq_result), C.POINTER(cg_fastq_result)]

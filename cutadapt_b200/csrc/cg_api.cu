@@ -117,6 +117,22 @@ struct Lane {
     int32_t *dst_qtrim = nullptr; size_t n_qtrim = 0; bool qtrim_bounced = false;
 };
 
+// The rows of one kind for a slot's records (cg_fastq_request_rows): the request with its text, the device copy of the
+// text, the row sizes and offsets, and the rows (compressed into d_gz when asked), kept until the slot is submitted again
+#define CG_ROWS_KINDS 3
+struct FqRows {
+    bool requested = false;
+    bool gzip = false;
+    int32_t n_entries = 0;
+    std::vector<char> text;
+    std::vector<int32_t> text_off;
+    int64_t limit = -1;                         // cg_fastq_collect_info / _rows: the caller's row capacity, or -1
+    DevBuf<uint8_t> d_text, d_out, d_gz;
+    DevBuf<int32_t> d_textoff, d_row;
+    DevBuf<int64_t> d_rowoff;
+    int64_t bytes = 0, bytes_plain = 0;
+};
+
 // One FASTQ chunk in flight (cg_fastq_submit ... cg_fastq_collect)
 #define CG_FQ_SLOTS 4
 struct FastqSlot {
@@ -127,9 +143,9 @@ struct FastqSlot {
     DevBuf<uint32_t> d_tiles, d_nl;
     DevBuf<CgFastqRecord> d_rec;
     DevBuf<int32_t> d_len, d_interval, d_keep, d_outlen, d_qtrim, d_mask, d_adest, d_dmbytes, d_dest, d_pairkey, d_origin;
-    DevBuf<uint8_t> d_destkeep, d_names, d_infoout;
-    DevBuf<int32_t> d_nameoff, d_inforow;
-    DevBuf<int64_t> d_infooff;
+    DevBuf<uint8_t> d_destkeep;
+    FqRows rows[CG_ROWS_KINDS];                 // row requests and their rows
+    bool rows_ready = false;                    // the last collect of the slot succeeded: its rows can be read
     DevBuf<int64_t> d_dmbase;
     DevBuf<int64_t> d_offs, d_outoff;
     DevBuf<unsigned long long> d_scan;
@@ -1672,6 +1688,12 @@ static int fastq_format_error(const int err[2], int mate = 0)
 static int fastq_slot_init(cg_ctx *c, FastqSlot &f)
 {
     f.ilv = 0;
+    f.rows_ready = false;                       // a new chunk: the rows of the last one are gone, no requests yet
+    for (FqRows &q : f.rows) {
+        q.requested = false;
+        q.limit = -1;
+        q.bytes = q.bytes_plain = 0;
+    }
     if (!f.stream) CU(cudaStreamCreateWithFlags(&f.stream, cudaStreamNonBlocking));
     int rc;
     if ((rc = f.d_counters.ensure(1 + CG_FQ_COUNTERS)) != CG_OK || (rc = f.d_err.ensure(2)) != CG_OK) return rc;
@@ -2988,10 +3010,10 @@ static int fastq_copy_out(cg_ctx *c, FastqSlot &f, uint8_t *out, const uint8_t *
 
 // gzip outputs: the destinations of d_src at bounds[0 .. n_dest] (host), destination d compressed when gz[d], else copied.
 // Every destination is cut into pieces of GZ_MEMBER bytes from its start; gz_compress_kernel turns each gzip piece into a
-// member in its slot, the host places the pieces behind each other and gz_gather_kernel packs them into f.d_gzout.
-// bounds then hold where each destination lies there; *total is the packed size.
+// member in its slot, the host places the pieces behind each other and gz_gather_kernel packs them into `packed`
+// (f.d_gzout for the outputs).  bounds then hold where each destination lies there; *total is the packed size.
 static int fastq_gzip(cg_ctx *c, FastqSlot &f, const uint8_t *d_src, std::vector<int64_t> &bounds, const std::vector<char> &gz,
-                      long long *total, cudaStream_t st)
+                      DevBuf<uint8_t> &packed, long long *total, cudaStream_t st)
 {
     const size_t n_dest = gz.size();
     std::vector<CgGzPiece> pieces;
@@ -3019,9 +3041,9 @@ static int fastq_gzip(cg_ctx *c, FastqSlot &f, const uint8_t *d_src, std::vector
         for (int64_t i = 0; i < n_pieces; ++i, ++k) { off[k] = at; at += sizes[k]; }
     }
     bounds[n_dest] = at;
-    if ((rc = f.d_gzout.ensure((size_t)at + 64)) != CG_OK) return rc;
+    if ((rc = packed.ensure((size_t)at + 64)) != CG_OK) return rc;
     CU(cudaMemcpyAsync(f.d_gzoff.p, off.data(), np * sizeof(int64_t), cudaMemcpyHostToDevice, st));
-    CU(cg_launch_gzip_gather(f.d_gzslots.p, f.d_gzsizes.p, f.d_gzoff.p, (int)np, f.d_gzout.p, st));
+    CU(cg_launch_gzip_gather(f.d_gzslots.p, f.d_gzsizes.p, f.d_gzoff.p, (int)np, packed.p, st));
     c->launches += 2;
     *total = at;
     return CG_OK;
@@ -3068,7 +3090,7 @@ static int fastq_emit(cg_ctx *c, FastqSlot &f, std::vector<int64_t> &bounds, con
         if ((rc = f.d_out.ensure((size_t)bounds.back() + 64)) != CG_OK) return rc;
         if ((rc = write(f.d_out.p)) != CG_OK) return rc;
         long long packed = 0;
-        if ((rc = fastq_gzip(c, f, f.d_out.p, bounds, gz, &packed, st)) != CG_OK) return rc;
+        if ((rc = fastq_gzip(c, f, f.d_out.p, bounds, gz, f.d_gzout, &packed, st)) != CG_OK) return rc;
         for (int i = 0; i < n_out; ++i) m[i].res->out_bytes = bounds[(i + 1) * per] - bounds[i * per];
     }
     std::string need;
@@ -3171,52 +3193,129 @@ static int fastq_stage_output_interleaved(cg_ctx *c, const FqMate *m, const FqSp
                       });
 }
 
-// --info-file rows of a chunk, an extra output of a collect
-struct FqInfo {
-    const char *names = nullptr;          // host: adapter names back to back ...
-    const int32_t *name_off = nullptr;    // ... and n_adapters + 1 offsets
-    int n_adapters = 0;
-    uint8_t *out = nullptr;               // host
-    int64_t capacity = 0;
-    int64_t *bytes = nullptr;             // host out
-    int kind = 0;                         // 0 info rows, 1 rest rows, 2 wildcard rows (names = adapter sequences)
-};
+// ---- rows of a slot's records (cg_fastq_request_rows) ----
+static const char *const rows_kind_name[CG_ROWS_KINDS] = {"info", "rest", "wildcard"};
 
-static int fastq_stage_info(cg_ctx *c, FastqSlot &f, const FqStage &g, const cg_fastq_params *fp, const FqInfo &info,
-                            cudaStream_t st)
+// The requests of a slot against the collect's set: n_entries adapters (pairs with --pair-adapters, 0 without a set).
+// Checked before the collect does any work.
+static int fastq_rows_check(const FastqSlot &f, int n_entries, const char *who)
+{
+    for (int k = 0; k < CG_ROWS_KINDS; ++k) {
+        const FqRows &q = f.rows[k];
+        if (q.requested && q.n_entries != n_entries)
+            return fail(CG_EINVAL, std::string(who) + ": the " + rows_kind_name[k] + " rows were requested with " +
+                                       std::to_string(q.n_entries) + " entries of text, the collect's adapter set has " +
+                                       std::to_string(n_entries));
+    }
+    return CG_OK;
+}
+
+// Every requested kind of rows of a mate, after its matches are final and before the finish kernel:
+// fq_info_count_kernel -> scan -> fq_info_write_kernel into the kind's own buffer, then, for gzip rows, fastq_gzip
+// into the kind's own packed buffer (the output stage reuses the slot's d_out / d_gzout).  The walks cut the read as it
+// came: the record table keeps where the record lies in it (d_origin), also after the quality trimmers were folded in.
+static int fastq_stage_rows(cg_ctx *c, FastqSlot &f, const FqStage &g, const cg_fastq_params *fp, cudaStream_t st)
 {
     const long long n = g.n;
-    int rc;
-    const size_t name_bytes = (size_t)info.name_off[info.n_adapters];
-    if ((rc = f.d_names.ensure(name_bytes + 1)) != CG_OK) return rc;
-    if ((rc = f.d_nameoff.ensure((size_t)info.n_adapters + 1)) != CG_OK) return rc;
-    if ((rc = f.d_inforow.ensure((size_t)n)) != CG_OK) return rc;
-    if ((rc = f.d_infooff.ensure((size_t)n + 1)) != CG_OK) return rc;
-    if ((rc = f.d_scan.ensure((size_t)cg_scan_tiles(n) + 1)) != CG_OK) return rc;
-    if (name_bytes) CU(cudaMemcpyAsync(f.d_names.p, info.names, name_bytes, cudaMemcpyHostToDevice, st));
-    CU(cudaMemcpyAsync(f.d_nameoff.p, info.name_off, ((size_t)info.n_adapters + 1) * sizeof(int32_t), cudaMemcpyHostToDevice, st));
     const int upper = g.action == CG_FQ_ACTION_LOWERCASE;
-    CU(cg_launch_fastq_info(0, f.d_in.p, f.d_rec.p, f.d_origin.p, f.d_interval.p, f.d_mask.p, g.d_matches, g.times, g.slots,
-                            f.d_names.p, f.d_nameoff.p, fp->revcomp != 0, g.rc_suffix, upper, n, f.d_inforow.p, nullptr, nullptr,
-                            st, info.kind, g.d_qtrim, f.d_len.p, g.has_qual() ? 1 : 0));
-    CU(cg_launch_scan_i32(f.d_inforow.p, n, f.d_scan.p, f.d_infooff.p, st));
-    long long total = 0;
-    CU(cudaMemcpyAsync(&total, f.d_infooff.p + n, sizeof total, cudaMemcpyDeviceToHost, st));
-    CU(cudaStreamSynchronize(st));
-    c->launches += 4;
-    *info.bytes = total;
-    if (total > info.capacity)
-        return fail(CG_EINVAL, "cg_fastq_collect_info: info buffer too small (" + std::to_string(total) + " bytes needed)");
-    if (total == 0) return CG_OK;
-    if ((rc = f.d_infoout.ensure((size_t)total + 64)) != CG_OK) return rc;
-    CU(cg_launch_fastq_info(1, f.d_in.p, f.d_rec.p, f.d_origin.p, f.d_interval.p, f.d_mask.p, g.d_matches, g.times, g.slots,
-                            f.d_names.p, f.d_nameoff.p, fp->revcomp != 0, g.rc_suffix, upper, n, nullptr, f.d_infooff.p,
-                            f.d_infoout.p, st, info.kind, g.d_qtrim, f.d_len.p, g.has_qual() ? 1 : 0));
-    c->launches += 1;
-    CU(cudaMemcpyAsync(info.out, f.d_infoout.p, (size_t)total, cudaMemcpyDeviceToHost, st));
-    CU(cudaStreamSynchronize(st));
-    c->d2h_bytes += total;
+    int rc;
+    for (int k = 0; k < CG_ROWS_KINDS; ++k) {
+        FqRows &q = f.rows[k];
+        if (!q.requested) continue;
+        const size_t text_bytes = (size_t)q.text_off[(size_t)q.n_entries];
+        if ((rc = q.d_text.ensure(text_bytes + 1)) != CG_OK) return rc;
+        if ((rc = q.d_textoff.ensure((size_t)q.n_entries + 1)) != CG_OK) return rc;
+        if ((rc = q.d_row.ensure((size_t)n)) != CG_OK) return rc;
+        if ((rc = q.d_rowoff.ensure((size_t)n + 1)) != CG_OK) return rc;
+        if ((rc = f.d_scan.ensure((size_t)cg_scan_tiles(n) + 1)) != CG_OK) return rc;
+        if (text_bytes) CU(cudaMemcpyAsync(q.d_text.p, q.text.data(), text_bytes, cudaMemcpyHostToDevice, st));
+        CU(cudaMemcpyAsync(q.d_textoff.p, q.text_off.data(), ((size_t)q.n_entries + 1) * sizeof(int32_t),
+                           cudaMemcpyHostToDevice, st));
+        CU(cg_launch_fastq_info(0, f.d_in.p, f.d_rec.p, f.d_origin.p, f.d_interval.p, f.d_mask.p, g.d_matches, g.times,
+                                g.slots, q.d_text.p, q.d_textoff.p, fp->revcomp != 0, g.rc_suffix, upper, n, q.d_row.p,
+                                nullptr, nullptr, st, k, g.d_qtrim, f.d_len.p, g.has_qual() ? 1 : 0));
+        CU(cg_launch_scan_i32(q.d_row.p, n, f.d_scan.p, q.d_rowoff.p, st));
+        long long total = 0;
+        CU(cudaMemcpyAsync(&total, q.d_rowoff.p + n, sizeof total, cudaMemcpyDeviceToHost, st));
+        CU(cudaStreamSynchronize(st));
+        c->launches += 4;
+        q.bytes = q.bytes_plain = total;
+        if (q.limit >= 0 && total > q.limit)
+            return fail(CG_EINVAL, std::string(k == CG_ROWS_INFO ? "cg_fastq_collect_info: info" : "cg_fastq_collect_rows: rows") +
+                                       " buffer too small (" + std::to_string(total) + " bytes needed)");
+        if (total == 0) continue;
+        if ((rc = q.d_out.ensure((size_t)total + 64)) != CG_OK) return rc;
+        CU(cg_launch_fastq_info(1, f.d_in.p, f.d_rec.p, f.d_origin.p, f.d_interval.p, f.d_mask.p, g.d_matches, g.times,
+                                g.slots, q.d_text.p, q.d_textoff.p, fp->revcomp != 0, g.rc_suffix, upper, n, nullptr,
+                                q.d_rowoff.p, q.d_out.p, st, k, g.d_qtrim, f.d_len.p, g.has_qual() ? 1 : 0));
+        c->launches += 1;
+        if (q.gzip) {
+            std::vector<int64_t> bounds{0, (int64_t)total};
+            long long packed = 0;
+            if ((rc = fastq_gzip(c, f, q.d_out.p, bounds, std::vector<char>{1}, q.d_gz, &packed, st)) != CG_OK) return rc;
+            q.bytes = packed;
+        }
+    }
     return CG_OK;
+}
+
+// A collect that took slot f succeeded (rows_ready) or not: the rows can be read after the one only
+static int fastq_rows_done(FastqSlot &f, int rc)
+{
+    f.rows_ready = rc == CG_OK;
+    return rc;
+}
+
+extern "C" int cg_fastq_request_rows(cg_ctx *c, int32_t slot, int32_t kind, const char *adapter_text,
+                                     const int32_t *text_offsets, int32_t n_entries, int32_t gzip)
+{
+    if (!c || slot < 0 || slot >= CG_FQ_SLOTS || n_entries < 0 || !text_offsets)
+        return fail(CG_EINVAL, "cg_fastq_request_rows: bad argument");
+    if (kind < 0 || kind >= CG_ROWS_KINDS)
+        return fail(CG_EINVAL, "cg_fastq_request_rows: unknown kind " + std::to_string(kind) +
+                                   " (CG_ROWS_INFO, CG_ROWS_REST or CG_ROWS_WILDCARD)");
+    FastqSlot &f = c->fq[slot];
+    if (!f.busy) return fail(CG_EINVAL, "cg_fastq_request_rows: nothing was submitted to this slot");
+    FqRows &q = f.rows[kind];
+    if (q.requested)
+        return fail(CG_EINVAL, std::string("cg_fastq_request_rows: the ") + rows_kind_name[kind] +
+                                   " rows of this slot were requested already");
+    if (text_offsets[0] != 0) return fail(CG_EINVAL, "cg_fastq_request_rows: text_offsets must start at 0");
+    for (int a = 0; a < n_entries; ++a)
+        if (text_offsets[a + 1] < text_offsets[a])
+            return fail(CG_EINVAL, "cg_fastq_request_rows: text_offsets must not decrease");
+    if (text_offsets[n_entries] && !adapter_text) return fail(CG_EINVAL, "cg_fastq_request_rows: adapter_text is NULL");
+    q.text.assign(adapter_text, adapter_text + text_offsets[n_entries]);
+    q.text_off.assign(text_offsets, text_offsets + n_entries + 1);
+    q.n_entries = n_entries;
+    q.gzip = gzip != 0;
+    q.limit = -1;
+    q.bytes = q.bytes_plain = 0;
+    q.requested = true;
+    return CG_OK;
+}
+
+extern "C" int cg_fastq_read_rows(cg_ctx *c, int32_t slot, int32_t kind, uint8_t *dst, int64_t capacity, int64_t *n_bytes,
+                                  int64_t *n_bytes_plain)
+{
+    if (!c || slot < 0 || slot >= CG_FQ_SLOTS || capacity < 0) return fail(CG_EINVAL, "cg_fastq_read_rows: bad argument");
+    if (kind < 0 || kind >= CG_ROWS_KINDS)
+        return fail(CG_EINVAL, "cg_fastq_read_rows: unknown kind " + std::to_string(kind) +
+                                   " (CG_ROWS_INFO, CG_ROWS_REST or CG_ROWS_WILDCARD)");
+    FastqSlot &f = c->fq[slot];
+    const FqRows &q = f.rows[kind];
+    if (!q.requested)
+        return fail(CG_EINVAL, std::string("cg_fastq_read_rows: no ") + rows_kind_name[kind] +
+                                   " rows were requested for this slot");
+    if (f.busy || !f.rows_ready)
+        return fail(CG_EINVAL, "cg_fastq_read_rows: the slot's collect has not run or has failed; there are no rows");
+    if (n_bytes) *n_bytes = q.bytes;
+    if (n_bytes_plain) *n_bytes_plain = q.bytes_plain;
+    if (!dst) return CG_OK;
+    if (capacity < q.bytes)
+        return fail(CG_EINVAL, "cg_fastq_read_rows: buffer too small (" + std::to_string(q.bytes) + " bytes needed)");
+    CU(cudaSetDevice(c->device));
+    return fastq_copy_out(c, f, dst, q.gzip ? q.d_gz.p : q.d_out.p, q.bytes, f.stream);
 }
 
 // The part of a collect after the evaluation, for one mate (n_mates 1) or a pair, on stream st: the routes, the finish
@@ -3264,9 +3363,28 @@ static int fastq_collect_finish(cg_ctx *c, const FqMate *m, int n_mates, FqDemux
     return CG_OK;
 }
 
+static int fastq_collect_one(cg_ctx *c, FastqSlot &f, const cg_adapterset *s, const cg_fastq_params *fp, uint8_t *out,
+                             int64_t out_capacity, cg_fastq_result *res, FqDemux *dm, int64_t *segments, FqSplit *sp)
+{
+    memset(res, 0, sizeof *res);
+    int rc;
+    if (sp && (rc = split_check(*sp, fp, "cg_fastq_collect_split")) != CG_OK) return rc;
+    if ((rc = gzip_check(fp, "cg_fastq_collect")) != CG_OK) return rc;
+    if ((rc = fastq_rows_check(f, s ? s->host.n_adapters : 0, "cg_fastq_collect")) != CG_OK) return rc;
+    FqStage g;
+    rc = fqstats_lookup(c, fp->stats, s ? s->host.n_adapters : 0, &g.acc);
+    if (rc != CG_OK) return rc;
+    rc = fastq_stage_evaluate(c, f, s, fp, 1, f.stream, g);
+    if (rc != CG_OK || g.n == 0) return rc;
+    if ((rc = fastq_stage_rows(c, f, g, fp, f.stream)) != CG_OK) return rc;
+    FqMate m;
+    m.f = &f; m.g = &g; m.fp = fp; m.out = out; m.capacity = out_capacity; m.res = res; m.segments = segments;
+    return fastq_collect_finish(c, &m, 1, dm, sp, 0, 0, f.stream);
+}
+
 static int fastq_collect_impl(cg_ctx *c, int32_t slot, const cg_adapterset *s, const cg_fastq_params *fp,
                               uint8_t *out, int64_t out_capacity, cg_fastq_result *res, FqDemux *dm, int64_t *segments,
-                              const FqInfo *info = nullptr, FqSplit *sp = nullptr)
+                              FqSplit *sp = nullptr)
 {
     if (!c || !fp || !res || slot < 0 || slot >= CG_FQ_SLOTS) return fail(CG_EINVAL, "cg_fastq_collect: bad argument");
     if (s && s->ctx != c) return fail(CG_EINVAL, "adapter set belongs to another context");
@@ -3275,19 +3393,7 @@ static int fastq_collect_impl(cg_ctx *c, int32_t slot, const cg_adapterset *s, c
     if (f.ilv) return fail(CG_EINVAL, "cg_fastq_collect: the slot holds a mate of an interleaved chunk, collect it as a pair");
     CU(cudaSetDevice(c->device));
     f.busy = false;
-    memset(res, 0, sizeof *res);
-    int rc;
-    if (sp && (rc = split_check(*sp, fp, "cg_fastq_collect_split")) != CG_OK) return rc;
-    if ((rc = gzip_check(fp, "cg_fastq_collect")) != CG_OK) return rc;
-    FqStage g;
-    rc = fqstats_lookup(c, fp->stats, s ? s->host.n_adapters : 0, &g.acc);
-    if (rc != CG_OK) return rc;
-    rc = fastq_stage_evaluate(c, f, s, fp, 1, f.stream, g);
-    if (rc != CG_OK || g.n == 0) return rc;
-    if (info && (rc = fastq_stage_info(c, f, g, fp, *info, f.stream)) != CG_OK) return rc;
-    FqMate m;
-    m.f = &f; m.g = &g; m.fp = fp; m.out = out; m.capacity = out_capacity; m.res = res; m.segments = segments;
-    return fastq_collect_finish(c, &m, 1, dm, sp, 0, 0, f.stream);
+    return fastq_rows_done(f, fastq_collect_one(c, f, s, fp, out, out_capacity, res, dm, segments, sp));
 }
 
 extern "C" int cg_fastq_collect(cg_ctx *c, int32_t slot, const cg_adapterset *s, const cg_fastq_params *fp,
@@ -3311,7 +3417,31 @@ extern "C" int cg_fastq_collect_split(cg_ctx *c, int32_t slot, const cg_adapters
     FqSplit sp;
     sp.redirect = redirect;
     sp.fasta_dests = split_fasta_dests(fp, fasta_outputs);
-    return fastq_collect_impl(c, slot, s, fp, out, out_capacity, res, nullptr, segments, nullptr, &sp);
+    return fastq_collect_impl(c, slot, s, fp, out, out_capacity, res, nullptr, segments, &sp);
+}
+
+// cg_fastq_collect_info / _rows: a request of `kind` limited to the caller's buffer, the plain collect, the rows
+static int fastq_collect_rows_into(cg_ctx *c, int32_t slot, const cg_adapterset *s, const cg_fastq_params *fp, int32_t kind,
+                                   const char *text, const int32_t *text_offsets, uint8_t *out, int64_t out_capacity,
+                                   uint8_t *rows_out, int64_t rows_capacity, cg_fastq_result *res, int64_t *rows_bytes,
+                                   const char *who)
+{
+    if (!c || !s || !text || !text_offsets || !rows_bytes || rows_capacity < 0 || (rows_capacity && !rows_out) || slot < 0 ||
+        slot >= CG_FQ_SLOTS)
+        return fail(CG_EINVAL, std::string(who) + ": bad argument");
+    *rows_bytes = 0;
+    for (int a = 0; a < s->host.n_adapters; ++a)
+        if (text_offsets[a] < 0 || text_offsets[a + 1] < text_offsets[a])
+            return fail(CG_EINVAL, std::string(who) + (kind == CG_ROWS_INFO ? ": name_offsets" : ": text_offsets") +
+                                       " must not decrease");
+    int rc = cg_fastq_request_rows(c, slot, kind, text, text_offsets, s->host.n_adapters, 0);
+    if (rc != CG_OK) return rc;
+    FqRows &q = c->fq[slot].rows[kind];
+    q.limit = rows_capacity;
+    rc = fastq_collect_impl(c, slot, s, fp, out, out_capacity, res, nullptr, nullptr);
+    *rows_bytes = q.bytes_plain;
+    if (rc != CG_OK) return rc;
+    return cg_fastq_read_rows(c, slot, kind, rows_out, rows_capacity, nullptr, nullptr);
 }
 
 extern "C" int cg_fastq_collect_info(cg_ctx *c, int32_t slot, const cg_adapterset *s, const cg_fastq_params *fp,
@@ -3319,16 +3449,8 @@ extern "C" int cg_fastq_collect_info(cg_ctx *c, int32_t slot, const cg_adapterse
                                      int64_t out_capacity, uint8_t *info_out, int64_t info_capacity, cg_fastq_result *res,
                                      int64_t *info_bytes)
 {
-    if (!s || !adapter_names || !name_offsets || !info_bytes || info_capacity < 0 || (info_capacity && !info_out))
-        return fail(CG_EINVAL, "cg_fastq_collect_info: bad argument");
-    *info_bytes = 0;
-    FqInfo info;
-    info.names = adapter_names; info.name_off = name_offsets; info.n_adapters = s->host.n_adapters;
-    info.out = info_out; info.capacity = info_capacity; info.bytes = info_bytes;
-    for (int a = 0; a < info.n_adapters; ++a)
-        if (name_offsets[a] < 0 || name_offsets[a + 1] < name_offsets[a])
-            return fail(CG_EINVAL, "cg_fastq_collect_info: name_offsets must not decrease");
-    return fastq_collect_impl(c, slot, s, fp, out, out_capacity, res, nullptr, nullptr, &info);
+    return fastq_collect_rows_into(c, slot, s, fp, CG_ROWS_INFO, adapter_names, name_offsets, out, out_capacity, info_out,
+                                   info_capacity, res, info_bytes, "cg_fastq_collect_info");
 }
 
 extern "C" int cg_fastq_collect_rows(cg_ctx *c, int32_t slot, const cg_adapterset *s, const cg_fastq_params *fp,
@@ -3337,19 +3459,9 @@ extern "C" int cg_fastq_collect_rows(cg_ctx *c, int32_t slot, const cg_adapterse
                                      int64_t *rows_bytes)
 {
     if (kind < 0 || kind > 2) return fail(CG_EINVAL, "cg_fastq_collect_rows: kind must be 0 (info), 1 (rest) or 2 (wildcard)");
-    if (kind == 0)
-        return cg_fastq_collect_info(c, slot, s, fp, adapter_text, text_offsets, out, out_capacity, rows_out, rows_capacity,
-                                     res, rows_bytes);
-    if (!s || !adapter_text || !text_offsets || !rows_bytes || rows_capacity < 0 || (rows_capacity && !rows_out))
-        return fail(CG_EINVAL, "cg_fastq_collect_rows: bad argument");
-    *rows_bytes = 0;
-    FqInfo info;
-    info.names = adapter_text; info.name_off = text_offsets; info.n_adapters = s->host.n_adapters;
-    info.out = rows_out; info.capacity = rows_capacity; info.bytes = rows_bytes; info.kind = kind;
-    for (int a = 0; a < info.n_adapters; ++a)
-        if (text_offsets[a] < 0 || text_offsets[a + 1] < text_offsets[a])
-            return fail(CG_EINVAL, "cg_fastq_collect_rows: text_offsets must not decrease");
-    return fastq_collect_impl(c, slot, s, fp, out, out_capacity, res, nullptr, nullptr, &info);
+    return fastq_collect_rows_into(c, slot, s, fp, kind, adapter_text, text_offsets, out, out_capacity, rows_out,
+                                   rows_capacity, res, rows_bytes,
+                                   kind == CG_ROWS_INFO ? "cg_fastq_collect_info" : "cg_fastq_collect_rows");
 }
 
 static int demux_check(const cg_adapterset *s, const int32_t *adapter_dest, int32_t n_named, const char *who)
@@ -3437,12 +3549,12 @@ static int fastq_stage_pair_adapters(cg_ctx *c, FastqSlot &f1, FastqSlot &f2, co
     return fastq_stage_verdict(c, f2, fp2, 2, st, g2);
 }
 
-static int fastq_collect_paired_impl(cg_ctx *c, int32_t slot1, int32_t slot2, const cg_adapterset *s1,
-                                     const cg_adapterset *s2, const FqPairAdapters *pa, const cg_fastq_params *fp1,
-                                     const cg_fastq_params *fp2, int32_t pair_filter_mode, uint8_t *out1,
-                                     int64_t out_capacity1, uint8_t *out2, int64_t out_capacity2, cg_fastq_result *res1,
-                                     cg_fastq_result *res2, FqDemux *dm, int64_t *segments1, int64_t *segments2,
-                                     FqSplit *sp = nullptr)
+static int fastq_collect_paired_run(cg_ctx *c, int32_t slot1, int32_t slot2, const cg_adapterset *s1,
+                                    const cg_adapterset *s2, const FqPairAdapters *pa, const cg_fastq_params *fp1,
+                                    const cg_fastq_params *fp2, int32_t pair_filter_mode, uint8_t *out1,
+                                    int64_t out_capacity1, uint8_t *out2, int64_t out_capacity2, cg_fastq_result *res1,
+                                    cg_fastq_result *res2, FqDemux *dm, int64_t *segments1, int64_t *segments2,
+                                    FqSplit *sp)
 {
     if (!c || !fp1 || !fp2 || !res1 || !res2 || slot1 < 0 || slot1 >= CG_FQ_SLOTS || slot2 < 0 || slot2 >= CG_FQ_SLOTS ||
         slot1 == slot2 || pair_filter_mode < 0 || pair_filter_mode > 2)
@@ -3490,8 +3602,13 @@ static int fastq_collect_paired_impl(cg_ctx *c, int32_t slot1, int32_t slot2, co
             return fail(CG_EINVAL, "cg_fastq_collect_paired_interleaved: an interleaved output must have its gzip_outputs bit "
                                    "set alike in both mates' parameters");
     }
-    if ((rc = fqstats_lookup(c, fp1->stats, pa ? pa->n_pairs : (s1 ? s1->host.n_adapters : 0), &g1.acc)) != CG_OK ||
-        (rc = fqstats_lookup(c, fp2->stats, pa ? pa->n_pairs : (s2 ? s2->host.n_adapters : 0), &g2.acc)) != CG_OK)
+    const int n_entries1 = pa ? pa->n_pairs : (s1 ? s1->host.n_adapters : 0);
+    const int n_entries2 = pa ? pa->n_pairs : (s2 ? s2->host.n_adapters : 0);
+    if ((rc = fastq_rows_check(f1, n_entries1, "cg_fastq_collect_paired (mate 1)")) != CG_OK ||
+        (rc = fastq_rows_check(f2, n_entries2, "cg_fastq_collect_paired (mate 2)")) != CG_OK)
+        return rc;
+    if ((rc = fqstats_lookup(c, fp1->stats, n_entries1, &g1.acc)) != CG_OK ||
+        (rc = fqstats_lookup(c, fp2->stats, n_entries2, &g2.acc)) != CG_OK)
         return rc;
     if (pa) {
         if ((rc = fastq_stage_pair_adapters(c, f1, f2, *pa, fp1, fp2, st, g1, g2)) != CG_OK) return rc;
@@ -3503,6 +3620,8 @@ static int fastq_collect_paired_impl(cg_ctx *c, int32_t slot1, int32_t slot2, co
         return fail(CG_EINVAL, "paired FASTQ chunks differ in their number of records (" + std::to_string(g1.n) + " vs " +
                                    std::to_string(g2.n) + ")");
     if (g1.n == 0) return CG_OK;
+    if ((rc = fastq_stage_rows(c, f1, g1, fp1, st)) != CG_OK || (rc = fastq_stage_rows(c, f2, g2, fp2, st)) != CG_OK)
+        return rc;
     // --discard-untrimmed with adapters on one mate only tests "both" (cli.py:859-893)
     const int mode_untrimmed = (!pa && (!s1 || !s2)) ? 1 : pair_filter_mode;
     FqMate m[2];
@@ -3511,6 +3630,22 @@ static int fastq_collect_paired_impl(cg_ctx *c, int32_t slot1, int32_t slot2, co
     m[1].f = &f2; m[1].g = &g2; m[1].fp = fp2; m[1].out = out2; m[1].capacity = out_capacity2; m[1].res = res2;
     m[1].segments = segments2;
     return fastq_collect_finish(c, m, 2, dm, sp, pair_filter_mode, mode_untrimmed, st);
+}
+
+static int fastq_collect_paired_impl(cg_ctx *c, int32_t slot1, int32_t slot2, const cg_adapterset *s1,
+                                     const cg_adapterset *s2, const FqPairAdapters *pa, const cg_fastq_params *fp1,
+                                     const cg_fastq_params *fp2, int32_t pair_filter_mode, uint8_t *out1,
+                                     int64_t out_capacity1, uint8_t *out2, int64_t out_capacity2, cg_fastq_result *res1,
+                                     cg_fastq_result *res2, FqDemux *dm, int64_t *segments1, int64_t *segments2,
+                                     FqSplit *sp = nullptr)
+{
+    const int rc = fastq_collect_paired_run(c, slot1, slot2, s1, s2, pa, fp1, fp2, pair_filter_mode, out1, out_capacity1,
+                                            out2, out_capacity2, res1, res2, dm, segments1, segments2, sp);
+    if (c && slot1 >= 0 && slot1 < CG_FQ_SLOTS && slot2 >= 0 && slot2 < CG_FQ_SLOTS && slot1 != slot2) {
+        fastq_rows_done(c->fq[slot1], rc);
+        fastq_rows_done(c->fq[slot2], rc);
+    }
+    return rc;
 }
 
 extern "C" int cg_fastq_collect_paired(cg_ctx *c, int32_t slot1, int32_t slot2, const cg_adapterset *s1,

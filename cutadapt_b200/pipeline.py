@@ -1079,6 +1079,75 @@ def _demux_names(adapters):
     return outputs, np.array([number[n] for n in names], dtype=np.int32)
 
 
+# the per-read text outputs (cg_fastq_request_rows): --info-file, --rest-file, --wildcard-file
+ROW_KINDS = ("info", "rest", "wildcard")
+
+
+def _row_kinds(rows, gzip_rows, what: str = "rows") -> Tuple[tuple, tuple]:
+    """(kinds, compressed kinds) from names out of ROW_KINDS; a compressed kind must be requested."""
+    rows = tuple(dict.fromkeys(rows or ()))
+    gzip_rows = tuple(dict.fromkeys(gzip_rows or ()))
+    for name in rows + gzip_rows:
+        if name not in ROW_KINDS:
+            raise ValueError(f"unknown row output {name!r} (one of {', '.join(ROW_KINDS)})")
+    for name in gzip_rows:
+        if name not in rows:
+            raise ValueError(f"the {name} rows are to be compressed but are not in {what}")
+    return rows, gzip_rows
+
+
+def _text_blob(texts) -> Tuple[bytes, np.ndarray]:
+    blobs = [t.encode("latin-1") for t in texts]
+    offsets = np.zeros(len(blobs) + 1, dtype=np.int32)
+    offsets[1:] = np.cumsum([len(b) for b in blobs])
+    return b"".join(blobs), offsets
+
+
+def _row_text(adapters, kind: str, pair_list: bool = False) -> Tuple[bytes, np.ndarray]:
+    """(text, offsets) a kind of rows needs for the adapters of a mate: names as the info file shows them (the parts
+    of a linked adapter are "name;1" / "name;2", LinkedMatch.get_info_records, adapters.py:1157-1171), nothing for
+    rest rows, the sequences for wildcard rows.  pair_list: the -a or -A list of --pair-adapters, whose matches name
+    the pair; no adapters: no entries."""
+    if adapters is None:
+        return b"", np.zeros(1, dtype=np.int32)
+    if pair_list:
+        singles = list(adapters)
+        names = [a.name for a in singles]
+    else:
+        singles, groups, owners = adapters._flatten()
+        names = [s.name for s in singles]
+        for (typ, a0, a1, _, _), owner in zip(groups, owners):
+            if typ == _lib.CG_GROUP_LINKED:
+                base = "none" if owner.name is None else owner.name
+                names[a0], names[a1] = base + ";1", base + ";2"
+    if kind == "info":
+        return _text_blob(names)
+    if kind == "rest":
+        return _text_blob([""] * len(singles))
+    return _text_blob([s.sequence for s in singles])
+
+
+def _request_rows(ctx, slot: int, kinds, texts: dict, gzip_rows) -> None:
+    for kind in kinds:
+        blob, offsets = texts[kind]
+        _lib.check(_lib.lib().cg_fastq_request_rows(ctx.handle, slot, ROW_KINDS.index(kind), blob, offsets.ctypes.data,
+                                                    offsets.size - 1, int(kind in gzip_rows)))
+
+
+def _read_rows(ctx, slot: int, kinds) -> dict:
+    """{kind: bytes} of the collect that took ``slot`` (cg_fastq_read_rows)."""
+    rows = {}
+    for kind in kinds:
+        k, n, plain = ROW_KINDS.index(kind), C.c_int64(0), C.c_int64(0)
+        _lib.check(_lib.lib().cg_fastq_read_rows(ctx.handle, slot, k, None, 0, C.byref(n), C.byref(plain)))
+        buf = np.empty(n.value, dtype=np.uint8)
+        if n.value:
+            _lib.check(_lib.lib().cg_fastq_read_rows(ctx.handle, slot, k, buf.ctypes.data, buf.size, C.byref(n),
+                                                     C.byref(plain)))
+        rows[kind] = buf.tobytes()
+    return rows
+
+
 class FastqTrimmer:
     """
     FASTQ chunks in, trimmed FASTQ chunks out -- the per-chunk worker of the reference
@@ -1115,6 +1184,12 @@ class FastqTrimmer:
                         method then returns gzip members (65 280 plain bytes each, see cg_fastq_params.gzip_outputs;
                         "output" covers every demultiplexed output), which concatenate into one gzip file, and
                         ``statistics`` gains ``out_bytes_plain``, the uncompressed size
+    rows                names out of ROW_KINDS ("info", "rest", "wildcard") -- --info-file / --rest-file /
+                        --wildcard-file: every chunk method also formats these rows of the chunk's reads on the device
+                        (every read, filtered or not, in input order; cg_fastq_request_rows) and leaves them in
+                        ``last_rows`` = {kind: bytes} for the chunk it just returned or yielded
+    gzip_rows           names out of ``rows`` whose rows are compressed on the device (gzip members as for
+                        gzip_outputs)
 
     ``process_chunk(bytes) -> bytes``; ``process_chunks(iterable)`` keeps one chunk in flight so that the
     upload of chunk i+1 overlaps the download of chunk i.  With ``redirect``: ``process_chunk_split(bytes) ->
@@ -1133,7 +1208,8 @@ class FastqTrimmer:
                  input_format: str = "fastq", output_format: Optional[str] = None,
                  ctx: Optional[_lib.Context] = None, collect_statistics: bool = False,
                  redirect: Sequence[str] = (), redirect_formats: Optional[dict] = None,
-                 gzip_outputs: Sequence[str] = ()):
+                 gzip_outputs: Sequence[str] = (), rows: Sequence[str] = (), gzip_rows: Sequence[str] = ()):
+        self.rows, self.gzip_rows = _row_kinds(rows, gzip_rows)
         self.params = _fastq_params(times, quality_cutoff, quality_base, nextseq_cutoff, minimum_length, maximum_length,
                                     max_n, max_expected_errors, discard_trimmed, discard_untrimmed, cut, poly_a, length,
                                     trim_n, discard_casava, action, revcomp, rc_suffix, input_format, output_format)
@@ -1150,10 +1226,30 @@ class FastqTrimmer:
             self.params.stats = self._stats.handle
         self.statistics = {}
         self._out_bufs, self._out_keep = {}, {}
+        self._row_texts = {}
+        self._slot_rows = {}          # slot -> the kinds requested for the chunk in it
+        self._rows_taken = {}
+        self.last_rows = {}
 
-    def _submit(self, chunk) -> Tuple[int, int, object]:
+    def _texts(self, kinds) -> dict:
+        for kind in kinds:
+            if kind not in self._row_texts:
+                self._row_texts[kind] = _row_text(self.adapters, kind)
+        return self._row_texts
+
+    def _submit(self, chunk, rows: Optional[tuple] = None) -> Tuple[int, int, object]:
+        """Upload a chunk and request its rows (``rows``: kinds, default the trimmer's)."""
         slot, buf = _submit_chunk(self.ctx, chunk)
+        kinds = self.rows if rows is None else rows
+        _request_rows(self.ctx, slot, kinds, self._texts(kinds), self.gzip_rows)
+        self._slot_rows[slot] = kinds
         return slot, buf.size, buf
+
+    def _take_rows(self, slot: int) -> None:
+        """The rows of the collect that just took ``slot``: every kind requested for it, and the trimmer's kinds in
+        last_rows."""
+        self._rows_taken = _read_rows(self.ctx, slot, self._slot_rows.pop(slot, ()))
+        self.last_rows = {kind: self._rows_taken[kind] for kind in self.rows}
 
     def _capacity(self, n_bytes: int, n_dest: int = 4, chunk=None) -> int:
         # a device chunk cannot be submitted again, so FASTA output with " rc" suffixes gets room for all of them
@@ -1190,12 +1286,13 @@ class FastqTrimmer:
             # FASTA output: " rc" suffixes can exceed the bound; the call says how much it needs, run the chunk again
             if (rc != 0 and self.params.format != _lib.CG_FORMAT_FASTQ and res.out_bytes > out.size
                     and not isinstance(chunk, DeviceChunk)):
-                slot, _, chunk = self._submit(chunk)
+                slot, _, chunk = self._submit(chunk, self._slot_rows.pop(slot, None))
                 out = self._out_buffer(slot, res.out_bytes)
                 continue
             _lib.check(rc)
             break
         self._account(res)
+        self._take_rows(slot)
         return out[: res.out_bytes].tobytes() if copy else out[: res.out_bytes]
 
     def _no_redirect(self, what: str):
@@ -1218,12 +1315,13 @@ class FastqTrimmer:
                 self._redirect, self._fasta_outputs, out.ctypes.data, out.size, C.byref(res), segments.ctypes.data)
             # " rc" suffixes can exceed the bound; the call says how much it needs, run the chunk again
             if rc != 0 and res.out_bytes > out.size and not isinstance(chunk, DeviceChunk):
-                slot, _, chunk = self._submit(chunk)
+                slot, _, chunk = self._submit(chunk, self._slot_rows.pop(slot, None))
                 out = self._out_buffer(slot, res.out_bytes)
                 continue
             _lib.check(rc)
             break
         self._account(res)
+        self._take_rows(slot)
         names = ("output",) + REDIRECT_OUTPUTS
         part = (lambda a, b: out[a:b].tobytes()) if copy else (lambda a, b: out[a:b])
         return {name: part(segments[d], segments[d + 1]) for d, name in enumerate(names)
@@ -1254,74 +1352,36 @@ class FastqTrimmer:
             self.ctx.handle, slot, self._set.handle, C.byref(self.params), dest.ctypes.data, len(outputs),
             out.ctypes.data, out.size, C.byref(res), segments.ctypes.data))
         self._account(res)
+        self._take_rows(slot)
         return {name: out[segments[i]:segments[i + 1]].tobytes() for i, name in enumerate(outputs + [unknown])}
 
     def _info_names(self):
         """Adapter names as the info file shows them: the parts of a linked adapter are "name;1" / "name;2"
         (LinkedMatch.get_info_records, adapters.py:1157-1171)."""
-        singles, groups, owners = self.adapters._flatten()
-        names = [s.name for s in singles]
-        for (typ, a0, a1, _, _), owner in zip(groups, owners):
-            if typ == _lib.CG_GROUP_LINKED:
-                base = "none" if owner.name is None else owner.name
-                names[a0], names[a1] = base + ";1", base + ";2"
-        blobs = [n.encode("latin-1") for n in names]
-        offsets = np.zeros(len(blobs) + 1, dtype=np.int32)
-        offsets[1:] = np.cumsum([len(b) for b in blobs])
-        return b"".join(blobs), offsets
+        return _row_text(self.adapters, "info")
 
-    def _process_chunk_rows(self, chunk, kind: int, blob: bytes, offsets: np.ndarray) -> Tuple[bytes, bytes]:
-        self._no_redirect(("info", "rest", "wildcard")[kind] + " file rows")
+    def _process_chunk_rows(self, chunk, kind: str) -> Tuple[bytes, bytes]:
+        """(trimmed output, the rows of one kind) of a chunk: that kind is requested next to the trimmer's rows."""
+        self._no_redirect(kind + " file rows")
         if self.adapters is None:
             raise ValueError("these outputs need adapters")
-        per_read = max(1, self.params.trim.times) * 2
-        n_bytes = len(chunk)
-        capacity = per_read * 2 * n_bytes + (1 << 20)
-        if isinstance(chunk, DeviceChunk):
-            # a chunk inflated on the device can only be collected once: its plain bytes are kept on the host, so
-            # that a second try with a larger row buffer submits them as an ordinary chunk
-            plain, got = np.empty(n_bytes, dtype=np.uint8), C.c_int64(0)
-            _lib.check(_lib.lib().cg_fastq_slot_read(self.ctx.handle, chunk.slot, plain.ctypes.data, plain.size,
-                                                     C.byref(got)))
-            first, chunk = chunk, plain[: got.value]
-        else:
-            first = chunk
-        while True:
-            slot, _, _ = self._submit(first)
-            first = chunk
-            out = self._out_buffer(slot, self._capacity(n_bytes))
-            rows = np.empty(capacity, dtype=np.uint8)
-            res = _lib.cg_fastq_result()
-            n_rows = C.c_int64(0)
-            rc = _lib.lib().cg_fastq_collect_rows(
-                self.ctx.handle, slot, self._set.handle, C.byref(self.params), kind, blob, offsets.ctypes.data,
-                out.ctypes.data, out.size, rows.ctypes.data, rows.size, C.byref(res), C.byref(n_rows))
-            if rc != 0 and n_rows.value > capacity:      # many short reads: rows larger than estimated
-                capacity = n_rows.value
-                continue
-            _lib.check(rc)
-            break
-        self._account(res)
-        return out[: res.out_bytes].tobytes(), rows[: n_rows.value].tobytes()
+        out = self._collect(self._submit(chunk, tuple(dict.fromkeys(self.rows + (kind,)))))
+        return out, self._rows_taken[kind]
 
     def process_chunk_info(self, chunk) -> Tuple[bytes, bytes]:
         """(trimmed FASTQ, the rows ``--info-file`` gets for the chunk), both formatted on the device
-        (``cg_fastq_collect_rows`` kind 0; InfoFileWriter, steps.py:222-253)."""
+        (``cg_fastq_request_rows`` CG_ROWS_INFO; InfoFileWriter, steps.py:222-253)."""
         if self.adapters is None:
             raise ValueError("the info file needs adapters")
-        blob, offsets = self._info_names()
-        return self._process_chunk_rows(chunk, 0, blob, offsets)
+        return self._process_chunk_rows(chunk, "info")
 
     def process_chunk_rest(self, chunk) -> Tuple[bytes, bytes]:
         """(trimmed FASTQ, the rows of ``--rest-file``): RestFileWriter, steps.py:193-206."""
-        return self._process_chunk_rows(chunk, 1, b"", np.zeros(len(self.adapters._flatten()[0]) + 1, dtype=np.int32))
+        return self._process_chunk_rows(chunk, "rest")
 
     def process_chunk_wildcards(self, chunk) -> Tuple[bytes, bytes]:
         """(trimmed FASTQ, the rows of ``--wildcard-file``): WildcardFileWriter, steps.py:209-220."""
-        blobs = [s.sequence.encode("latin-1") for s in self.adapters._flatten()[0]]
-        offsets = np.zeros(len(blobs) + 1, dtype=np.int32)
-        offsets[1:] = np.cumsum([len(b) for b in blobs])
-        return self._process_chunk_rows(chunk, 2, b"".join(blobs), offsets)
+        return self._process_chunk_rows(chunk, "wildcard")
 
     @property
     def collect_statistics(self) -> bool:
@@ -1390,6 +1450,12 @@ class PairedFastqTrimmer:
     ``(bytes, b"")`` (the reference interleaves an output whose paired path is missing).  Not with ``pair_adapters``
     or demultiplexing.  ``gzip_outputs`` / ``gzip_outputs2``: as FastqTrimmer's ``gzip_outputs``, for R1's files and for
     R2's (default: the same names); an interleaved output must be named in both.
+
+    ``rows`` / ``rows2``: FastqTrimmer's ``rows`` for R1's reads and for R2's (--info-file, --rest-file and
+    --wildcard-file write R1's rows, PairedSingleEndStep, cli.py:675-696; --info-file-paired adds R2's info rows,
+    PairedInfoFileWriter, steps.py:256-269); ``gzip_rows`` / ``gzip_rows2`` the kinds compressed (default for R2: those
+    of ``gzip_rows`` it has).  Every chunk method leaves ``last_rows`` = {kind: (bytes of R1, bytes of R2)}, b"" for a
+    mate without that kind.  With ``pair_adapters`` the info rows name adapter i of each mate's own list.
     """
 
     MODES = {"any": 0, "both": 1, "first": 2}
@@ -1400,9 +1466,15 @@ class PairedFastqTrimmer:
                  ctx: Optional[_lib.Context] = None, collect_statistics: bool = False,
                  redirect: Sequence[str] = (), redirect_formats: Optional[dict] = None,
                  interleaved_outputs: Sequence[str] = (), gzip_outputs: Sequence[str] = (),
-                 gzip_outputs2: Optional[Sequence[str]] = None):
+                 gzip_outputs2: Optional[Sequence[str]] = None, rows: Sequence[str] = (),
+                 rows2: Sequence[str] = (), gzip_rows: Sequence[str] = (), gzip_rows2: Optional[Sequence[str]] = None):
         if pair_filter not in self.MODES:
             raise ValueError("pair_filter must be 'any', 'both' or 'first'")
+        self.rows, self.gzip_rows = _row_kinds(rows, gzip_rows)
+        if gzip_rows2 is None:
+            gzip_rows2 = [k for k in self.gzip_rows if k in (rows2 or ())]
+        self.rows2, self.gzip_rows2 = _row_kinds(rows2, gzip_rows2, "rows2")
+        self.last_rows = {}
         formats = dict(input_format=input_format, output_format=output_format)
         self.params1 = _fastq_params(**{**(options1 or {}), **formats})
         self.params2 = _fastq_params(**{**(options2 or {}), **formats})
@@ -1453,6 +1525,9 @@ class PairedFastqTrimmer:
                 counts = tuple(len(a._flatten()[0]) if a is not None else 0 for a in (self.adapters1, self.adapters2))
             self._stats = tuple(_lib.FastqStatistics(self.ctx, n) for n in counts)
             self.params1.stats, self.params2.stats = self._stats[0].handle, self._stats[1].handle
+        pair_list = self._pairs is not None
+        self._row_texts = ({k: _row_text(self.adapters1, k, pair_list) for k in self.rows},
+                           {k: _row_text(self.adapters2, k, pair_list) for k in self.rows2})
 
     @property
     def collect_statistics(self) -> bool:
@@ -1490,7 +1565,15 @@ class PairedFastqTrimmer:
         return tuple(written_lengths(v, max_len) for v, max_len, _ in self.statistics_vector())
 
     def _submit_pair(self, chunk1, chunk2):
-        """((slot1, chunk), (slot2, chunk)): two chunks, or one interleaved chunk (chunk2 None) split on the device."""
+        """((slot1, chunk), (slot2, chunk)): two chunks, or one interleaved chunk (chunk2 None) split on the device;
+        the rows of each mate are requested."""
+        tickets = self._upload_pair(chunk1, chunk2)
+        for (slot, _), kinds, texts, gz in zip(tickets, (self.rows, self.rows2), self._row_texts,
+                                                (self.gzip_rows, self.gzip_rows2)):
+            _request_rows(self.ctx, slot, kinds, texts, gz)
+        return tickets
+
+    def _upload_pair(self, chunk1, chunk2):
         if chunk2 is not None:
             return _submit_chunk(self.ctx, chunk1), _submit_chunk(self.ctx, chunk2)
         if isinstance(chunk1, DeviceChunk):            # interleaved, already split into two slots
@@ -1500,6 +1583,12 @@ class PairedFastqTrimmer:
         _lib.check(_lib.lib().cg_fastq_submit_interleaved(self.ctx.handle, buf.ctypes.data if buf.size else None,
                                                           buf.size, self.params1.format, C.byref(s1), C.byref(s2)))
         return (s1.value, buf), (s2.value, buf)
+
+    def _take_rows(self, tickets) -> None:
+        """last_rows of the pair of slots just collected: {kind: (R1's rows, R2's rows)}."""
+        (s1, _), (s2, _) = tickets
+        r1, r2 = _read_rows(self.ctx, s1, self.rows), _read_rows(self.ctx, s2, self.rows2)
+        self.last_rows = {k: (r1.get(k, b""), r2.get(k, b"")) for k in ROW_KINDS if k in r1 or k in r2}
 
     def _out_buffers(self, tickets, n_dest: int = 4):
         """Output buffers of a pair: out1 also holds R2 of the interleaved outputs."""
@@ -1540,6 +1629,7 @@ class PairedFastqTrimmer:
                 self._redirect, self._fasta_outputs, out1.ctypes.data, out1.size, out2.ctypes.data, out2.size,
                 C.byref(r1), C.byref(r2), seg1.ctypes.data, seg2.ctypes.data))
         self._account(r1, r2)
+        self._take_rows(tickets)
         names = ("output",) + REDIRECT_OUTPUTS
         return {name: (out1[seg1[d]:seg1[d + 1]].tobytes(), out2[seg2[d]:seg2[d + 1]].tobytes())
                 for d, name in enumerate(names) if d == 0 or name in self.redirect}
@@ -1578,6 +1668,7 @@ class PairedFastqTrimmer:
                 self._set2.handle if self._set2 is not None else None, C.byref(self.params1), C.byref(self.params2),
                 self.mode, out1.ctypes.data, out1.size, out2.ctypes.data, out2.size, C.byref(r1), C.byref(r2)))
         self._account(r1, r2)
+        self._take_rows(tickets)
         return out1[: r1.out_bytes].tobytes(), out2[: r2.out_bytes].tobytes()
 
     def process_chunk_demux(self, chunk1, chunk2=None, combinatorial: bool = False, discard_untrimmed: bool = False,
@@ -1618,6 +1709,7 @@ class PairedFastqTrimmer:
             dest2.ctypes.data if dest2 is not None else None, n2, keep.ctypes.data, out1.ctypes.data, out1.size,
             out2.ctypes.data, out2.size, C.byref(r1), C.byref(r2), seg1.ctypes.data, seg2.ctypes.data))
         self._account(r1, r2)
+        self._take_rows(tickets)
         return {key: (out1[seg1[i]:seg1[i + 1]].tobytes(), out2[seg2[i]:seg2[i + 1]].tobytes())
                 for i, key in enumerate(keys) if keep[i]}
 

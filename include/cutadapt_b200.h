@@ -464,7 +464,9 @@ int cg_fastq_collect_paired(cg_ctx *ctx, int32_t slot1, int32_t slot2, const cg_
  * --revcomp is on), coordinates applied to the read as it came; reads without a match: name, -1, the read as written.
  * Rows of ALL records, filtered or not (the writer sits in front of the filters).  adapter_names: the names of the
  * set's adapters back to back (the parts of a linked adapter as "name;1" / "name;2"), name_offsets: n_adapters + 1
- * offsets into it.  *info_bytes: size of the rows; CG_EINVAL if info_capacity is too small. */
+ * offsets into it.  *info_bytes: size of the rows; CG_EINVAL if info_capacity is too small (nothing is then added
+ * to the statistics accumulator).  The same as cg_fastq_request_rows(CG_ROWS_INFO) + cg_fastq_collect +
+ * cg_fastq_read_rows. */
 int cg_fastq_collect_info(cg_ctx *ctx, int32_t slot, const cg_adapterset *set, const cg_fastq_params *params,
                           const char *adapter_names, const int32_t *name_offsets, uint8_t *out, int64_t out_capacity,
                           uint8_t *info_out, int64_t info_capacity, cg_fastq_result *res, int64_t *info_bytes);
@@ -478,6 +480,37 @@ int cg_fastq_collect_info(cg_ctx *ctx, int32_t slot, const cg_adapterset *set, c
 int cg_fastq_collect_rows(cg_ctx *ctx, int32_t slot, const cg_adapterset *set, const cg_fastq_params *params, int32_t kind,
                           const char *adapter_text, const int32_t *text_offsets, uint8_t *out, int64_t out_capacity,
                           uint8_t *rows_out, int64_t rows_capacity, cg_fastq_result *res, int64_t *rows_bytes);
+
+/* Rows from any collect.  A row request belongs to a submitted slot (from any cg_fastq_submit*, a mate of an
+ * interleaved chunk included) and is honoured by whatever collect takes that slot, next to its usual outputs: the
+ * plain, split, demultiplexing and paired collects all format the rows of each of their slots that has requests, after
+ * the adapters were matched and before the filters, so the rows cover every record of the slot, filtered or not, in
+ * input order -- the row writers sit in front of the filters in the reference (steps.py:193-269).  On pairs this is
+ * PairedSingleEndStep (cli.py:675-696: --info-file, --rest-file and --wildcard-file write R1's rows) and
+ * PairedInfoFileWriter (steps.py:256-269: --info-file-paired adds R2's info rows): request the kinds on each mate's
+ * slot.  The rows and their format are those of cg_fastq_collect_info / cg_fastq_collect_rows; the coordinates of info
+ * rows apply to the read as it came (before -u and the quality trimmers) on every path.  With --pair-adapters,
+ * `adapter` of a match is the number of the pair, so the text of each mate is that mate's list (R1: the -a adapters, R2:
+ * the -A adapters; PairedAdapterCutter, modifiers.py:476-477).
+ *
+ * cg_fastq_request_rows: ask the next collect that takes `slot` for the rows of `kind` as well.  adapter_text /
+ * text_offsets as for cg_fastq_collect_rows (names for CG_ROWS_INFO, anything for CG_ROWS_REST, sequences for
+ * CG_ROWS_WILDCARD), n_entries + 1 offsets; both are copied before the call returns.  gzip != 0: the rows are
+ * compressed on the device in the member format of cg_fastq_params.gzip_outputs (members of at most 65 280 plain
+ * bytes).  At most one request per kind and slot; a request applies to one collect.  The collect fails with CG_EINVAL
+ * when n_entries is not the number of adapters of its set for that slot (the number of pairs with --pair-adapters, 0
+ * without a set).  A collect without requests does what it did without this call. */
+#define CG_ROWS_INFO 0          /* --info-file      (InfoFileWriter)     */
+#define CG_ROWS_REST 1          /* --rest-file      (RestFileWriter)     */
+#define CG_ROWS_WILDCARD 2      /* --wildcard-file  (WildcardFileWriter) */
+int cg_fastq_request_rows(cg_ctx *ctx, int32_t slot, int32_t kind, const char *adapter_text, const int32_t *text_offsets,
+                          int32_t n_entries, int32_t gzip);
+/* After the collect that took `slot` returned CG_OK: the rows of `kind` into dst (dst == NULL: the sizes only).  They
+ * stay on the device until the slot is submitted again.  *n_bytes: the bytes delivered (compressed if requested),
+ * *n_bytes_plain: the size of the text; CG_EINVAL if capacity < *n_bytes, if that kind was not requested, or before
+ * the collect or after a failed one. */
+int cg_fastq_read_rows(cg_ctx *ctx, int32_t slot, int32_t kind, uint8_t *dst, int64_t capacity, int64_t *n_bytes,
+                       int64_t *n_bytes_plain);
 
 /* --pair-adapters (PairedAdapterCutter, modifiers.py:412-503): adapter i of the -a list is removed from R1 only
  * together with adapter i of the -A list from R2.  sets1[i] / sets2[i] hold adapter i alone (one group each); every

@@ -38,6 +38,12 @@ tool's rule (prefixes of the reads compressed as one member of about 4 to 64 MiB
 three rounds alternating) and the smallest size from which the device wins at every larger size.  Last lines: the
 inflate kernels' device time per MiB of plain output from torch.profiler, in runs of their own, on the multi-member
 input and on the split stream.  The card's name and power limit are read in the run.
+--rows [n_reads] [chunk_megabytes] [--baseline-tree DIR]: the "paired" variant with the info rows of both mates
+(--info-file and --info-file-paired), four arms alternating over three rounds in one process: no rows, plain rows, rows
+compressed on the device (gzip_rows), and plain rows compressed by host zlib level 1 (one stream per mate, one thread).
+Per arm: host-to-host reads/s and the row bytes downloaded.  With --baseline-tree (a built checkout of another commit):
+its "paired" run and this tree's, both without rows, in alternating processes, three each.  The card's name and power
+limit are read in the run.
 """
 import json
 import subprocess
@@ -335,7 +341,77 @@ def measure_gzip_input(n, submit_mb):
                           "ms_per_MiB_plain_total": sum(ms.values()) / mib, "launches": launches}))
 
 
+def measure_rows(n, chunk_mb, baseline_tree=None):
+    """--rows: the "paired" variant with info rows on both mates (--info-file + --info-file-paired), four arms
+    alternating over three rounds in one process; then, with a baseline tree, its "paired" run without rows against
+    this tree's, alternating processes."""
+    n -= n % 2
+    data, rec_len = build_fastq(n, pair_names=True)
+    per_chunk = max(2, max(1, (chunk_mb << 20) // rec_len) // 2 * 2)
+    mates = [np.ascontiguousarray(data.reshape(n // 2, 2, rec_len)[:, k]).reshape(-1) for k in (0, 1)]
+    mates = [torch.from_numpy(m).pin_memory().numpy() for m in mates]
+    half = per_chunk // 2
+    chunks = [tuple(m[i * rec_len:min(n // 2, i + half) * rec_len] for m in mates) for i in range(0, n // 2, half)]
+    adapters = [PA.BackAdapter("AGATCGGAAGAGC", max_errors=0.1, name="adapter")]
+    opts = dict(quality_cutoff=(0, 20), minimum_length=20)
+    info = dict(rows=("info",), rows2=("info",))
+    arms = {"no_rows": PairedFastqTrimmer(adapters, adapters, opts, opts),
+            "plain_rows": PairedFastqTrimmer(adapters, adapters, opts, opts, **info),
+            "device_gzip_rows": PairedFastqTrimmer(adapters, adapters, opts, opts, **info, gzip_rows=("info",)),
+            "host_zlib1_rows": PairedFastqTrimmer(adapters, adapters, opts, opts, **info)}
+
+    def run(name, cs):
+        t = arms[name]
+        z = [zlib.compressobj(1, zlib.DEFLATED, 31) for _ in (0, 1)] if name == "host_zlib1_rows" else None
+        downloaded = written = 0
+        for parts in t.process_chunks_split(cs):
+            for k, r in enumerate(t.last_rows.get("info", ())):
+                downloaded += len(r)
+                written += len(z[k].compress(r)) if z else len(r)
+        if z:
+            written += sum(len(x.flush()) for x in z)
+        return downloaded, written
+
+    for name in arms:
+        run(name, chunks[:3])                     # warm-up: buffers, module load
+    res = {name: {"wall_s": 0.0} for name in arms}
+    for _ in range(3):
+        for name in arms:
+            t0 = time.perf_counter()
+            downloaded, written = run(name, chunks)
+            res[name]["wall_s"] += time.perf_counter() - t0
+            res[name]["row_bytes_downloaded"], res[name]["row_bytes_written"] = downloaded, written
+    for r in res.values():
+        r["reads_per_s"] = 3 * n / r["wall_s"]
+    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader",
+                           "-i", str(torch.cuda.current_device())], capture_output=True, text=True).stdout.strip()
+    print(json.dumps({"what": "paired FASTQ (-a/-A AGATCGGAAGAGC -q 20 -m 20), host to host, info rows of both mates: "
+                              "none, plain, device gzip, plain + host zlib level 1 (one thread per mate's stream)",
+                      "reads": n, "chunk_mb": chunk_mb, "chunks": len(chunks), "gpu": torch.cuda.get_device_name(),
+                      "card_and_power_limit": card, "arms": res}))
+    if baseline_tree is None:
+        return
+    # a collect without requests: this tree against the baseline tree (library and Python), alternating processes
+    runs = {"baseline": [], "this": []}
+    for _ in range(3):
+        for name, tree in (("baseline", baseline_tree), ("this", __file__.rsplit("/", 2)[0])):
+            out = subprocess.run([sys.executable, f"{tree}/tools/measure_fastq.py", str(n), str(chunk_mb), "paired"],
+                                 capture_output=True, text=True, check=True).stdout
+            runs[name].append(json.loads(out.strip().split("\n")[-1])["reads_per_s"])
+    print(json.dumps({"what": "paired variant without rows, this tree against the baseline tree, alternating processes",
+                      "card_and_power_limit": card, "reads_per_s": runs,
+                      "median": {k: sorted(v)[len(v) // 2] for k, v in runs.items()}}))
+
+
 def main():
+    if "--rows" in sys.argv:
+        argv = [a for a in sys.argv if a != "--rows"]
+        base = None
+        if "--baseline-tree" in argv:
+            i = argv.index("--baseline-tree")
+            base = argv[i + 1]
+            del argv[i:i + 2]
+        return measure_rows(int(argv[1]) if len(argv) > 1 else 4_000_000, int(argv[2]) if len(argv) > 2 else 64, base)
     if "--gzip-input" in sys.argv:
         argv = [a for a in sys.argv if a != "--gzip-input"]
         return measure_gzip_input(int(argv[1]) if len(argv) > 1 else 4_000_000, int(argv[2]) if len(argv) > 2 else 64)

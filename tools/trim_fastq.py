@@ -12,6 +12,8 @@ command line (no reports): it shows the per-chunk worker of INTEGRATION.md secti
       -o out.fastq in.fastq                                                            (filter outputs)
   python tools/trim_fastq.py --interleaved -a ADAPT1 -A ADAPT2 -m 20:25 -o out.fastq in.interleaved.fastq
   python tools/trim_fastq.py -a AGATCGGAAGAGC -o out.fastq.gz in.fastq.gz                   (gzip)
+  python tools/trim_fastq.py -a ADAPT1 -A ADAPT2 --info-file info1.txt.gz --info-file-paired info2.txt.gz \
+      -o out.1.fastq -p out.2.fastq in.1.fastq in.2.fastq                               (per-read row files)
 
 The input format comes from the first byte of the (first) input, as cutadapt's files.detect_file_format does: '>' or
 '#' is FASTA, anything else (an empty file included) FASTQ.  The output is FASTA when the input is, when -o ends in
@@ -37,6 +39,12 @@ input of at least 16 MiB (DEVICE_GZIP_SPLIT_MIN; the single member that gzip and
 block-parallel (split_members=True).  Smaller ones are decompressed on the host with Python's gzip module.  The outputs are the same either way; the stderr line's "in_bytes_gzip" (the
 compressed bytes consumed) appears only when the device inflated the input.  The format is detected from the first
 decompressed byte.
+
+Row files: --info-file, -r/--rest-file and --wildcard-file get the rows of every read, filtered or not, formatted on the
+device next to every kind of output above.  On pairs they get R1's rows, as in the reference (PairedSingleEndStep,
+cli.py:675-696); --info-file-paired adds R2's info rows, and only together with --info-file; it also makes the run
+paired (cli.py:537), so one input then needs --interleaved.  A row file whose name ends in .gz is compressed on the
+device like the other outputs.  Row files cannot go to standard output.
 """
 import argparse
 import gzip
@@ -256,8 +264,21 @@ def main():
                         help=f"write the reads the {name} filter removes to FILE instead of dropping them")
         ap.add_argument(f"--{name}-paired-output", dest=dest + "_paired_output", metavar="FILE",
                         help=f"the second mates of the pairs --{name}-output gets")
+    ap.add_argument("--info-file", metavar="FILE", help="write one row per adapter match (or per read without one)")
+    ap.add_argument("--info-file-paired", dest="info_file2", metavar="FILE",
+                    help="the info rows of the second mates (with --info-file)")
+    ap.add_argument("-r", "--rest-file", metavar="FILE", help="write what follows (3') / precedes (5') the last match")
+    ap.add_argument("--wildcard-file", metavar="FILE", help="write the read characters under the adapters' N positions")
     ap.add_argument("inputs", nargs="+")
     args = ap.parse_args()
+    if args.info_file2 and len(args.inputs) == 1 and not args.interleaved:
+        # --info-file-paired enables paired-end mode (cli.py:525-538, 560-566)
+        ap.error("You used an option that enables paired-end mode (such as -p, -A, -G, -B, -U), but only provided one "
+                 "input file. Please either provide two input files or use use --interleaved as appropriate.")
+    for path in (args.info_file, args.info_file2, args.rest_file, args.wildcard_file):
+        if path == "-":
+            ap.error("row files (--info-file, --info-file-paired, --rest-file, --wildcard-file) cannot be written to "
+                     "standard output")
     if args.interleaved and len(args.inputs) == 2 and args.paired_output:
         ap.error("--interleaved was given with two input files and two output files (-o and -p): use it for interleaved "
                  "input (one input file) or interleaved output (no -p)")
@@ -315,6 +336,20 @@ def main():
     ads2 = (make_adapters(args.back2, "back", args.error_rate, args.overlap)
             + make_adapters(args.front2, "front", args.error_rate, args.overlap)
             + make_adapters(args.anywhere2, "anywhere", args.error_rate, args.overlap))
+    # row files: R1's (of the single reads), and R2's info rows with --info-file-paired (PairedInfoFileWriter)
+    row_paths1 = {k: p for k, p in (("info", args.info_file), ("rest", args.rest_file), ("wildcard", args.wildcard_file))
+                  if p}
+    row_paths2 = {"info": args.info_file2} if paired and args.info_file and args.info_file2 else {}
+    row_files = ({k: OutputFile(p) for k, p in row_paths1.items()}, {k: OutputFile(p) for k, p in row_paths2.items()})
+    rows = dict(rows=tuple(row_paths1), gzip_rows=[k for k, p in row_paths1.items() if p.endswith(".gz")])
+
+    def write_rows(t):
+        """The rows of the chunk t returned last into the row files."""
+        for kind, data in t.last_rows.items():
+            r1, r2 = data if paired else (data, b"")
+            row_files[0][kind].write(r1)
+            if kind in row_files[1]:
+                row_files[1][kind].write(r2)
 
     if paired:
         if not args.paired_output and not args.interleaved:
@@ -326,7 +361,9 @@ def main():
         interleaved = [d for d in ["output"] + redirect
                        if not (args.paired_output if d == "output" else getattr(args, d + "_paired_output"))]
         t = PairedFastqTrimmer(ads1, ads2, common, options2, args.pair_filter, **formats, **split,
-                               interleaved_outputs=interleaved, gzip_outputs=gzip1, gzip_outputs2=gzip2)
+                               interleaved_outputs=interleaved, gzip_outputs=gzip1, gzip_outputs2=gzip2, **rows,
+                               rows2=tuple(row_paths2),
+                               gzip_rows2=[k for k, p in row_paths2.items() if p.endswith(".gz")])
         routes = [gzip_route(p) for p in args.inputs]
         if len(args.inputs) == 2 and all(routes):
             f1, f2 = open(args.inputs[0], "rb"), open(args.inputs[1], "rb")
@@ -349,6 +386,7 @@ def main():
                 files[name][0].write(r1)
                 if files[name][1] is not None:
                     files[name][1].write(r2)
+            write_rows(t)
         for fhs in files.values():
             for fh in fhs:
                 if fh is not None:
@@ -360,7 +398,7 @@ def main():
         # every demultiplexed output, "unknown" included, is compressed alike
         if args.untrimmed_output and args.untrimmed_output.endswith(".gz") != args.output.endswith(".gz"):
             ap.error("with demultiplexing, --untrimmed-output must be compressed (.gz) exactly when the -o template is")
-        t = FastqTrimmer(ads1, **common, **formats, gzip_outputs=gzip1)
+        t = FastqTrimmer(ads1, **common, **formats, gzip_outputs=gzip1, **rows)
         files = {}
         f, chunks = single_input(t)
         with f:
@@ -374,11 +412,12 @@ def main():
                             args.output.replace("{name}", name)
                         files[name] = OutputFile(path)
                     files[name].write(data)
+                write_rows(t)
         for fh in files.values():
             fh.close()
         stats = t.statistics
     elif redirect:
-        t = FastqTrimmer(ads1, **common, **formats, **split, gzip_outputs=gzip1)
+        t = FastqTrimmer(ads1, **common, **formats, **split, gzip_outputs=gzip1, **rows)
         f, chunks = single_input(t)
         with f:
             files = {d: OutputFile(getattr(args, d + "_output")) for d in redirect}
@@ -386,18 +425,22 @@ def main():
             for parts in t.process_chunks_split(chunks, copy=False):
                 for name, data in parts.items():
                     files[name].write(data)
+                write_rows(t)
             for fh in files.values():
                 fh.close()
         stats = t.statistics
     else:
-        t = FastqTrimmer(ads1, **common, **formats, gzip_outputs=gzip1)
+        t = FastqTrimmer(ads1, **common, **formats, gzip_outputs=gzip1, **rows)
         o = OutputFile(args.output)
         f, chunks = single_input(t)
         with f:
             for out in t.process_chunks(chunks, copy=False):
                 o.write(out.tobytes() if hasattr(out, "tobytes") else out)
+                write_rows(t)
         o.close()
         stats = t.statistics
+    for fh in list(row_files[0].values()) + list(row_files[1].values()):
+        fh.close()
     print(json.dumps(stats), file=sys.stderr)
     if args.json is not None:
         if paired:
