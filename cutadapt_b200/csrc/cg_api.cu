@@ -222,9 +222,6 @@ struct cg_ctx {
     DevBuf<uint32_t> scratch_p;
     DevBuf<int> scratch_w;
     DevBuf<unsigned long long> d_stats;  // cg_process_batch_stats: the statistics vector of the batch in flight
-    // statistics wanted together with the next trimming pass (launch_trim_with_stats): the split pipeline counts the
-    // reads its first stage settles while it has them in shared memory, the plan and run kernels list the others
-    struct { unsigned long long *d_stats = nullptr; int max_len = 0, kmax = 0; bool armed = false, done = false; } fuse;
     DevBuf<uint4> tasks;                 // split pipeline: 2 x uint4 per read of a sub-batch
     DevBuf<uint4> tasks2, tasks3;        // run-record lists (ping-pong): 4 x uint4 per read of a sub-batch
     DevBuf<uint2> stat_ents;             // fused statistics: one entry per read the plan and run kernels finish
@@ -545,94 +542,115 @@ extern "C" int cg_adapterset_effective_length(const cg_adapterset *s, int32_t ad
 // ------------------------------------------------------------------------------------------
 // Launch of the trimming pass on device-resident data
 // ------------------------------------------------------------------------------------------
-static int launch_trim_single(cg_ctx *c, const cg_adapterset *s, const uint8_t *d_seq, const uint8_t *d_qual,
-                              const int64_t *d_offsets, int64_t n_reads, int max_read_len, const cg_params *p,
-                              cg_match_rec *d_out, int32_t *d_qtrim, const int32_t *d_view, cudaStream_t st,
-                              bool timed)
+// The environment switches of the trimming pass (kernel choices of the parity tests, measured experiments), read when
+// a TrimSwitches is made: once per launch_trim call, not per context, since tests change them between calls.
+struct TrimSwitches {
+    static bool is(const char *name, const char *value) { const char *e = getenv(name); return e && strcmp(e, value) == 0; }
+    static long long at_least_1024(const char *e) { const long long v = e ? atoll(e) : 0; return v >= 1024 ? v : 0; }
+    bool force_general = is("CUTADAPT_B200_KERNEL", "general");
+    bool force_block = is("CUTADAPT_B200_KERNEL", "block");
+    bool force_warp = is("CUTADAPT_B200_KERNEL", "warp");
+    bool shiftand = is("CUTADAPT_B200_SCAN", "shiftand");
+    bool no_band = getenv("CUTADAPT_B200_NO_BAND") != nullptr;
+    bool no_light = getenv("CUTADAPT_B200_NO_LIGHT") != nullptr;
+    bool no_index_kernel = getenv("CUTADAPT_B200_NO_INDEX_KERNEL") != nullptr;
+    bool two_lists = getenv("CUTADAPT_B200_TWO_LISTS") != nullptr;
+    bool task_bytes = getenv("CUTADAPT_B200_TASK_BYTES") != nullptr;
+    bool no_band_lists = getenv("CUTADAPT_B200_NO_BAND_LISTS") != nullptr;
+    bool stage_times = getenv("CUTADAPT_B200_STAGE_TIMES") != nullptr;
+    bool jit_never = is("CUTADAPT_B200_JIT", "0"), jit_always = is("CUTADAPT_B200_JIT", "1");
+    long long sub_reads = at_least_1024(getenv("CUTADAPT_B200_SUB_READS"));   // 0: the schedule's default
+};
+
+// Statistics wanted together with a trimming pass (cg_stats_*), added to d_stats.
+struct StatsRequest { unsigned long long *d_stats; int max_len, kmax; };
+
+enum class TrimKind { Index, Light, Split, Warp, Fast, Generic, MultiPass };
+
+// What choose_schedule decided for one call, and what the launcher of that schedule needs.
+struct TrimSchedule {
+    TrimKind kind = TrimKind::Generic;
+    int tile_cap = 0, mini_cap = 0, carry_slot = 0;   // CgKernelArgs geometry
+    size_t smem = 0;                // the first kernel (fast, warp, or the split pipeline's first stage)
+    int occ = 0;                    // and its CTAs per SM
+    bool simple = false;            // fast: the SIMPLE variant
+    size_t list_smem = 0;           // split: the plan and run kernels
+    int plan_occ = 0, run_occ = 0;
+    int plane_w = 0, plane_rec = 0; // split: plane words of the first stage (0: shift-and scan), uint4 words per task
+    long long sub = 0;              // reads per sub-batch (index, split, multi-pass)
+    CgJitKernel *jit = nullptr;     // split: the specialised first stage, or null
+    int jit_occ = 0;
+    bool fuse_stats = false;        // split: the pass counts the statistics of its reads
+};
+
+// Decides how one call trims.  has_view: the call is a pass of the multi-pass schedule.  Besides deciding, it counts
+// the reads of the set's plane stage and builds the specialised first stage once.
+static int choose_schedule(cg_ctx *c, const cg_adapterset *s, int64_t n_reads, int max_read_len, const cg_params *p,
+                           bool has_view, const StatsRequest *stats, const TrimSwitches &sw, TrimSchedule &d)
 {
-    if (n_reads <= 0) return CG_OK;
+    const CgBuiltSet &h = s->host;
     const int times = p->times < 1 ? 1 : p->times;
     const bool want_q = p->quality_trim != 0 || p->nextseq_trim != 0;
-    if (want_q && !d_qual) return fail(CG_ENOQUAL, "Cannot do quality trimming when no qualities are available");
-    CgKernelArgs a;
-    memset(&a, 0, sizeof a);
-    a.blob = s->d_blob; a.blob_bytes = (uint32_t)s->host.blob.size();
-    a.masks64 = s->d_masks; a.enc = c->d_enc; a.index = s->d_index;
-    a.seq = d_seq; a.qual = want_q ? d_qual : nullptr; a.offsets = d_offsets; a.n_reads = n_reads;
-    // flags and packed base/cutoff as pre_trim_core expects them
-    a.quality_trim = (p->quality_trim ? 1 : 0) | (p->nextseq_trim ? 2 : 0);
-    a.cutoff_front = p->cutoff_front; a.cutoff_back = p->cutoff_back;
-    a.qbase = (p->quality_base & 255) | (int)((unsigned)p->nextseq_cutoff << 8); a.times = times; a.slots = s->host.slots;
-    a.out = d_out; a.qtrim = d_qtrim; a.view = d_view; a.err_flag = c->d_err;
-    a.col_rows = s->host.max_m + 1;
-    a.no_band = getenv("CUTADAPT_B200_NO_BAND") != nullptr;
-
-    const long long tile_cap_ll = ((long long)CG_NT * max_read_len + 32 + 15) / 16 * 16;
-    bool fast = !s->host.any_wide && max_read_len <= CG_PACKED_MAX_N && tile_cap_ll < (1 << 24);
-    size_t smem = 0;
-    int occ = 0;
+    // several groups, one round: per-adapter passes + selection (CUTADAPT_B200_KERNEL=general: the one-phase kernel)
+    if (!s->passes.empty() && times == 1 && !sw.force_general) {
+        d.kind = TrimKind::MultiPass;
+        d.sub = sw.sub_reads ? sw.sub_reads : 32LL << 20;
+        return CG_OK;
+    }
+    // sets of index lookups only (demultiplexing), no quality trimming: the light kernel -- nothing to stage; for one
+    // round without views the lookups alone (cg_index_kernel), in sub-batches so that 32-bit read numbers and one list
+    // suffice
+    if (h.all_indexed && !want_q && !h.any_wide && h.max_m + 1 <= CG_LIGHT_ROWS && !sw.force_general && !sw.no_light) {
+        d.kind = times == 1 && !has_view && h.slots == 1 && !sw.no_index_kernel ? TrimKind::Index : TrimKind::Light;
+        d.sub = 64LL << 20;
+        return CG_OK;
+    }
+    const uint32_t blob_bytes = (uint32_t)h.blob.size();
+    const long long tile_cap = ((long long)CG_NT * max_read_len + 32 + 15) / 16 * 16;
+    bool fast = !h.any_wide && max_read_len <= CG_PACKED_MAX_N && tile_cap < (1 << 24);
     if (fast) {
-        a.tile_cap = (int)tile_cap_ll;
-        smem = cg_fast_smem_bytes(a.blob_bytes, a.tile_cap, a.col_rows, want_q);
-        if (smem > c->smem_optin) fast = false;
+        d.tile_cap = (int)tile_cap;
+        d.smem = cg_fast_smem_bytes(blob_bytes, d.tile_cap, h.max_m + 1, want_q);
+        fast = d.smem <= c->smem_optin;
     }
     // two-phase schedule when the set is one aligner adapter and a single round is asked for;
     // CUTADAPT_B200_KERNEL=general forces the one-phase kernel (used by the parity tests)
-    const char *kernel_env = getenv("CUTADAPT_B200_KERNEL");
-    const bool force_general = kernel_env && strcmp(kernel_env, "general") == 0;
-    const bool simple = fast && s->host.simple_ok && times == 1 && !force_general;
+    d.simple = fast && h.simple_ok && times == 1 && !sw.force_general;
     if (fast) {
-        CU(cg_fast_occupancy(want_q, simple, smem, &occ));
-        if (occ < 1) fast = false;
+        CU(cg_fast_occupancy(want_q, d.simple, d.smem, &d.occ));
+        fast = d.occ >= 1;
+    }
+    d.kind = fast ? TrimKind::Fast : TrimKind::Generic;
+    const long long mini = ((long long)32 * max_read_len + 32 + 15) / 16 * 16;
+    // warp-autonomous fused kernel (kept selectable: CUTADAPT_B200_KERNEL=warp)
+    if (d.simple && h.max_m <= 32 && sw.force_warp && mini < (1 << 20)) {
+        d.mini_cap = (int)mini;
+        d.carry_slot = (int)(((long long)max_read_len + 4 + 15) / 16 * 16 + 16);   // + 4: word-granular reads past the last group
+        const size_t wsmem = cg_warp_smem_bytes(blob_bytes, d.mini_cap, d.carry_slot, want_q);
+        int wocc = 0;
+        if (wsmem <= c->smem_optin) CU(cg_warp_occupancy(want_q, wsmem, &wocc));
+        if (wocc >= 1) { d.kind = TrimKind::Warp; d.smem = wsmem; d.occ = wocc; }
+        return CG_OK;
     }
     // split pipeline (default for one aligner adapter with m <= 64): scan kernel -> task list -> DP kernel
-    const bool force_block = kernel_env && strcmp(kernel_env, "block") == 0;
-    const bool force_warp = kernel_env && strcmp(kernel_env, "warp") == 0;
-    bool split = false;
-    int plane_w = 0;
-    size_t scan_smem = 0, list_smem = 0;
-    int scan_occ = 0, plan_occ = 0, run_occ = 0;
-    if (simple && s->host.max_m <= 64 && !force_block && !force_warp) {
-        const long long mini = ((long long)32 * max_read_len + 32 + 15) / 16 * 16;
-        const long long cslot = ((long long)max_read_len + 4 + 15) / 16 * 16 + 32;   // + 4: word-granular reads past the last group
-        // bit-plane first stage (plane_scan_core) when the adapter has a plane program and the reads fit 8 plane
-        // words; CUTADAPT_B200_SCAN=shiftand keeps the shift-and scan kernel (parity tests run both)
-        const CgSetHeader *hdr = (const CgSetHeader *)s->host.blob.data();
-        const char *scan_env = getenv("CUTADAPT_B200_SCAN");
-        if (hdr->plane_count > 0 && max_read_len <= 256 && !(scan_env && strcmp(scan_env, "shiftand") == 0))
-            plane_w = max_read_len <= 160 ? 5 : 8;
-        long long cslot_need = cslot;
-        if (plane_w) cslot_need = std::max<long long>(cslot, 16LL * (2 * plane_w + 1) + 16);   // the window bytes a plane task carries
-        if (mini < (1 << 20)) {
-            a.mini_cap = (int)mini; a.carry_slot = (int)cslot_need;
-            scan_smem = plane_w ? cg_pscan_smem_bytes(a.blob_bytes, a.mini_cap, want_q)
-                                : cg_scan_smem_bytes(a.blob_bytes, a.mini_cap, want_q);
-            list_smem = cg_dp_smem_bytes(a.blob_bytes, a.carry_slot);
-            if (scan_smem <= c->smem_optin && list_smem <= c->smem_optin) {
-                if (plane_w) CU(cg_pscan_occupancy(want_q, plane_w, false, scan_smem, &scan_occ));
-                else CU(cg_scan_occupancy(want_q, scan_smem, &scan_occ));
-                CU(cg_list_occupancy(true, s->host.max_m, false, list_smem, &plan_occ));
-                CU(cg_list_occupancy(false, s->host.max_m, false, list_smem, &run_occ));
-                split = scan_occ >= 1 && plan_occ >= 1 && run_occ >= 1;
-            }
-        }
-    }
-    // warp-autonomous fused kernel (kept selectable: CUTADAPT_B200_KERNEL=warp)
-    bool warpk = false;
-    size_t wsmem = 0;
-    int wocc = 0;
-    if (simple && s->host.max_m <= 32 && force_warp) {
-        const long long mini = ((long long)32 * max_read_len + 32 + 15) / 16 * 16;
-        const long long cslot = ((long long)max_read_len + 4 + 15) / 16 * 16 + 16;   // + 4: word-granular reads past the last group
-        if (mini < (1 << 20)) {
-            a.mini_cap = (int)mini; a.carry_slot = (int)cslot;
-            wsmem = cg_warp_smem_bytes(a.blob_bytes, a.mini_cap, a.carry_slot, want_q);
-            if (wsmem <= c->smem_optin) {
-                CU(cg_warp_occupancy(want_q, wsmem, &wocc));
-                warpk = wocc >= 1;
-            }
-        }
-    }
+    if (!d.simple || h.max_m > 64 || sw.force_block || sw.force_warp || mini >= (1 << 20)) return CG_OK;
+    // bit-plane first stage (plane_scan_core) when the adapter has a plane program and the reads fit 8 plane
+    // words; CUTADAPT_B200_SCAN=shiftand keeps the shift-and scan kernel (parity tests run both)
+    const CgSetHeader *hdr = (const CgSetHeader *)h.blob.data();
+    if (hdr->plane_count > 0 && max_read_len <= 256 && !sw.shiftand) d.plane_w = max_read_len <= 160 ? 5 : 8;
+    const long long cslot = ((long long)max_read_len + 4 + 15) / 16 * 16 + 32;   // + 4: word-granular reads past the last group
+    d.mini_cap = (int)mini;
+    d.carry_slot = (int)(d.plane_w ? std::max<long long>(cslot, 16LL * (2 * d.plane_w + 1) + 16) : cslot);   // the window bytes a plane task carries
+    size_t scan_smem = d.plane_w ? cg_pscan_smem_bytes(blob_bytes, d.mini_cap, want_q)
+                                 : cg_scan_smem_bytes(blob_bytes, d.mini_cap, want_q);
+    d.list_smem = cg_dp_smem_bytes(blob_bytes, d.carry_slot);
+    if (scan_smem > c->smem_optin || d.list_smem > c->smem_optin) return CG_OK;
+    int scan_occ = 0;
+    if (d.plane_w) CU(cg_pscan_occupancy(want_q, d.plane_w, false, scan_smem, &scan_occ));
+    else CU(cg_scan_occupancy(want_q, scan_smem, &scan_occ));
+    CU(cg_list_occupancy(true, h.max_m, false, d.list_smem, &d.plan_occ));
+    CU(cg_list_occupancy(false, h.max_m, false, d.list_smem, &d.run_occ));
+    if (scan_occ < 1 || d.plan_occ < 1 || d.run_occ < 1) return CG_OK;
     // statistics counted inside the pass: one plain adapter, one round, the whole set in this call (not a pass of the
     // multi-pass schedule), no quality trimming, and the first stage keeps its CTAs per SM with the histogram in shared
     // memory.  The first stage counts the reads it settles (88 % on the benchmark's reads) while they are in shared
@@ -641,248 +659,200 @@ static int launch_trim_single(cg_ctx *c, const cg_adapterset *s, const uint8_t *
     // Otherwise launch_trim_with_stats runs cg_stats_kernel over all records after the pass.
     // Measured on an H100 (DESIGN.md section 4.1): with quality trimming (config 4) the first stage grew by more than
     // the statistics kernel costs, so quality-trimmed passes keep the kernel.
-    bool fuse_stats = split && plane_w && c->fuse.armed && !d_view && s->host.n_adapters == 1 && times == 1 &&
-                      s->host.slots == 1 && !want_q && !getenv("CUTADAPT_B200_TWO_LISTS") && c->fuse.max_len <= 4096 &&
-                      cg_stats_entries_smem_bytes(c->fuse.max_len, c->fuse.kmax) <= 48 * 1024;
-    if (fuse_stats) {
-        const size_t fsmem = cg_pscan_smem_bytes(a.blob_bytes, a.mini_cap, want_q, c->fuse.max_len);
+    if (d.plane_w && stats && !has_view && h.n_adapters == 1 && times == 1 && h.slots == 1 && !want_q && !sw.two_lists &&
+        stats->max_len <= 4096 && cg_stats_entries_smem_bytes(stats->max_len, stats->kmax) <= 48 * 1024) {
+        const size_t fsmem = cg_pscan_smem_bytes(blob_bytes, d.mini_cap, want_q, stats->max_len);
         int focc = 0;
-        if (fsmem <= c->smem_optin) CU(cg_pscan_occupancy(want_q, plane_w, true, fsmem, &focc));
+        if (fsmem <= c->smem_optin) CU(cg_pscan_occupancy(want_q, d.plane_w, true, fsmem, &focc));
         // (the listing variants of the plan and run kernels: same shared memory, the attribute set for them too)
         int pocc = 0, rocc = 0;
-        CU(cg_list_occupancy(true, s->host.max_m, true, list_smem, &pocc));
-        CU(cg_list_occupancy(false, s->host.max_m, true, list_smem, &rocc));
-        fuse_stats = focc >= 1 && focc >= scan_occ && pocc >= plan_occ && rocc >= run_occ;
-        if (fuse_stats) {
-            a.stats = c->fuse.d_stats; a.stats_max_len = c->fuse.max_len; a.stats_kmax = c->fuse.kmax;
-            scan_smem = fsmem; scan_occ = focc;
-        }
+        CU(cg_list_occupancy(true, h.max_m, true, d.list_smem, &pocc));
+        CU(cg_list_occupancy(false, h.max_m, true, d.list_smem, &rocc));
+        d.fuse_stats = focc >= 1 && focc >= scan_occ && pocc >= d.plan_occ && rocc >= d.run_occ;
+        if (d.fuse_stats) { scan_smem = fsmem; scan_occ = focc; }
     }
     // Run-time specialisation of the first stage for this adapter set (cg_jit.h): compiled once the set has seen
     // enough reads to pay for the ~1 s of NVRTC (CUTADAPT_B200_JIT=1: at once, =0: never), one kernel per variant
     // (with or without the statistics); any failure keeps the precompiled interpreter kernel.
-    CgJitKernel *jit_kernel = nullptr;
-    int jit_occ = 0;
-    if (split && plane_w) {
-        const int wi = plane_w <= 5 ? 0 : 1, qi = want_q ? 1 : 0, vi = fuse_stats ? 1 : 0;
+    if (d.plane_w) {
+        const int wi = d.plane_w <= 5 ? 0 : 1, qi = want_q ? 1 : 0, vi = d.fuse_stats ? 1 : 0;
         s->plane_reads += n_reads;
-        const char *je = getenv("CUTADAPT_B200_JIT");
-        const bool never = je && strcmp(je, "0") == 0, always = je && strcmp(je, "1") == 0;
-        if (!never && s->jit_state[wi][qi][vi] == 0 && (always || s->plane_reads >= (4LL << 20))) {
+        if (!sw.jit_never && s->jit_state[wi][qi][vi] == 0 && (sw.jit_always || s->plane_reads >= (4LL << 20))) {
             std::string err;
-            s->jit[wi][qi][vi] = cg_jit_build_pscan(s->host, plane_w, want_q, fuse_stats, err);
+            s->jit[wi][qi][vi] = cg_jit_build_pscan(h, d.plane_w, want_q, d.fuse_stats, err);
             s->jit_state[wi][qi][vi] = s->jit[wi][qi][vi] ? 1 : -1;
             if (!s->jit[wi][qi][vi]) s->jit_error = err;
         }
-        if (!never && s->jit_state[wi][qi][vi] == 1) {
-            jit_occ = cg_jit_occupancy(s->jit[wi][qi][vi], CG_NT, scan_smem);
-            if (jit_occ >= 1) jit_kernel = s->jit[wi][qi][vi];
+        if (!sw.jit_never && s->jit_state[wi][qi][vi] == 1) {
+            d.jit_occ = cg_jit_occupancy(s->jit[wi][qi][vi], CG_NT, scan_smem);
+            if (d.jit_occ >= 1) d.jit = s->jit[wi][qi][vi];
         }
     }
-    const bool stage_times = getenv("CUTADAPT_B200_STAGE_TIMES") != nullptr;
-    cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-    if (timed && c->timing.size() < 8192) {
-        for (cudaEvent_t *ev : {&ev0, &ev1}) {
-            if (!c->event_pool.empty()) { *ev = c->event_pool.back(); c->event_pool.pop_back(); }
-            else CU(cudaEventCreate(ev));
-        }
-        CU(cudaEventRecord(ev0, st));
-    }
-    // sets of index lookups only (demultiplexing), no quality trimming: the light kernel -- nothing to stage
-    const bool light = s->host.all_indexed && !want_q && !s->host.any_wide && s->host.max_m + 1 <= CG_LIGHT_ROWS &&
-                       !(kernel_env && strcmp(kernel_env, "general") == 0) && !getenv("CUTADAPT_B200_NO_LIGHT");
-    if (light && times == 1 && !d_view && a.slots == 1 && !getenv("CUTADAPT_B200_NO_INDEX_KERNEL")) {
-        // the lookups alone (cg_index_kernel), in sub-batches so that 32-bit read numbers and one list suffice
-        const long long SUBI = 64LL << 20;
-        int rc = c->tasks.ensure((size_t)((std::min<long long>(n_reads, SUBI) + 3) / 4));
-        if (rc != CG_OK) return rc;
-        for (long long r0 = 0; r0 < n_reads; r0 += SUBI) {
-            const long long n_sub = std::min<long long>(SUBI, n_reads - r0);
-            CgKernelArgs b = a;
-            b.offsets = a.offsets + r0; b.n_reads = n_sub; b.out = a.out + (size_t)r0 * a.slots;
-            b.tasks = c->tasks.p; b.task_count = c->d_task_count;
-            CU(cudaMemsetAsync(c->d_task_count, 0, sizeof(unsigned long long), st));
-            const long long need = (n_sub + CG_NT - 1) / CG_NT;
-            const int grid = (int)std::max<long long>(1, std::min<long long>((long long)c->sm_count * 16, need));
-            CU(cg_launch_index(b, grid, st));
-            c->launches += 1;
-        }
-    } else if (light) {
-        const long long need = (n_reads + CG_NT - 1) / CG_NT;
-        const int grid = (int)std::max<long long>(1, std::min<long long>((long long)c->sm_count * 16, need));
-        CU(cg_launch_light(a, grid, st));
-    } else if (split) {
-        // scan -> plan -> up to four DP rounds (one run of every unfinished read per round)
-        // reads per sub-batch: bounds the lists to 1 + 2 x 2 GiB at the default 32 Mi (measured: fewer,
-        // larger sub-batches amortise the kernel tails and the small late DP rounds; 32 Mi vs 4 Mi = +15 % on the 100 M-read bench).
-        // CUTADAPT_B200_SUB_READS overrides it for experiments.
-        long long SUB = (plane_w && getenv("CUTADAPT_B200_TASK_BYTES")) ? (16LL << 20) : (32LL << 20);   // (tasks with bytes: 240 B each)
-        if (const char *e = getenv("CUTADAPT_B200_SUB_READS")) { const long long v = atoll(e); if (v >= 1024) SUB = v; }
-        SUB = std::min<long long>(SUB, 1LL << 31);     // tasks name their read with 32 bits
-        const long long cap = std::min<long long>(n_reads, SUB);
-        // header (4 words) and, with CUTADAPT_B200_TASK_BYTES=1, the window bytes (cg_pscan.cuh).  Carrying the bytes
-        // turns the plan stage's gather into a stream but was measured neutral (plan 2.55 -> 2.65 ms, first stage
-        // 4.44 -> 4.64 ms per 100 M reads): the plan stage is bound by its dependent shared-memory chains, not by HBM.
-        const bool task_bytes = plane_w && getenv("CUTADAPT_B200_TASK_BYTES") != nullptr;
-        const int plane_rec = plane_w ? (task_bytes ? 4 + 2 * plane_w + 1 : 4) : 2;
-        int rc = c->tasks.ensure((size_t)cap * plane_rec);
-        if (rc == CG_OK) rc = c->tasks2.ensure((size_t)cap * 4);
-        if (rc == CG_OK) rc = c->tasks3.ensure((size_t)cap * 4);
-        if (rc == CG_OK && fuse_stats) rc = c->stat_ents.ensure((size_t)cap);
-        if (rc != CG_OK) return rc;
-        unsigned long long *cnt = c->d_task_count;
-        for (long long r0 = 0; r0 < n_reads; r0 += SUB) {
-            const long long n_sub = std::min<long long>(SUB, n_reads - r0);
-            CgKernelArgs b = a;
-            b.offsets = a.offsets + r0;
-            b.n_reads = n_sub;
-            b.out = a.out + (size_t)r0 * a.times * a.slots;
-            b.qtrim = a.qtrim ? a.qtrim + 2 * r0 : nullptr;
-            b.view = a.view ? a.view + 2 * r0 : nullptr;
-            b.task_cap = n_sub;
-            CU(cudaMemsetAsync(cnt, 0, 8 * sizeof(unsigned long long), st));
-            const long long n_mt = (n_sub + 31) / 32;
-            const long long need = (n_mt + 3) / 4;
-            auto grid_for = [&](int occ) { return (int)std::max<long long>(1, std::min<long long>((long long)occ * c->sm_count, need)); };
-            std::array<cudaEvent_t, 4> sev = {nullptr, nullptr, nullptr, nullptr};
-            if (stage_times && c->stage_events.size() < 4096) {
-                for (auto &e : sev) CU(cudaEventCreate(&e));
-                CU(cudaEventRecord(sev[0], st));
-            }
-            b.tasks = c->tasks.p; b.task_count = cnt;
-            b.task_rec = plane_rec;
-            // (two input lists for the plan stage -- reads with / without locator hits -- were measured: the first
-            //  stage got 2.3x slower and the plan stage no faster, it is bound by its memory traffic; kept as an
-            //  experiment: CUTADAPT_B200_TWO_LISTS=1)
-            b.task_count_b = (plane_w && getenv("CUTADAPT_B200_TWO_LISTS")) ? cnt + 4 : nullptr;
-            if (plane_w && jit_kernel) {
-                const int rcj = cg_jit_launch(jit_kernel, grid_for(jit_occ), CG_NT, scan_smem, (void *)st, &b);
-                if (rcj != 0) return fail(CG_ECUDA, "launch of the specialised first stage failed (CUresult " + std::to_string(rcj) + ")");
-            }
-            else if (plane_w) CU(cg_launch_pscan(b, want_q, plane_w, grid_for(scan_occ), scan_smem, st));
-            else CU(cg_launch_scan(b, want_q, grid_for(scan_occ), scan_smem, st));
-            if (sev[0]) CU(cudaEventRecord(sev[1], st));
-            b.stat_ents = c->stat_ents.p; b.stat_count = cnt + 6;
-            b.tasks2 = c->tasks2.p; b.task2_count = cnt + 1;
-            b.tasks3 = c->tasks3.p; b.task3_count = cnt + 2;
-            // run records of the plane path go to two lists (banded first runs / the others): cnt[5] counts the second
-            // (only with the band compiled in, CG_RUN_BAND)
-            b.task2_count_b = (CG_RUN_BAND && plane_w && !getenv("CUTADAPT_B200_NO_BAND_LISTS")) ? cnt + 5 : nullptr;
-            CU(cg_launch_list(b, true, s->host.max_m, grid_for(plan_occ), list_smem, st));
-            c->launches += 2;
-            if (plane_w) {
-                // second plan launch: the reads the first one set aside (windows with other letters than A/C/G/T),
-                // scanned exactly on dense warps; its run records continue the same list
-                CgKernelArgs b2 = b;
-                b2.tasks = c->tasks3.p; b2.task_count = cnt + 2; b2.task_rec = 2;
-                b2.tasks3 = nullptr; b2.task3_count = cnt + 3; b2.task_count_b = nullptr;
-                CU(cg_launch_list(b2, true, s->host.max_m, grid_for(plan_occ), list_smem, st));
-                CU(cudaMemsetAsync(cnt + 2, 0, sizeof(unsigned long long), st));
-                c->launches += 1;
-            }
-            if (sev[0]) CU(cudaEventRecord(sev[2], st));
-            uint4 *lists[2] = {c->tasks2.p, c->tasks3.p};
-            for (int round = 0; round < 4; ++round) {
-                const int in = round & 1, outl = in ^ 1;
-                if (round > 0) CU(cudaMemsetAsync(cnt + 1 + outl, 0, sizeof(unsigned long long), st));
-                b.tasks = lists[in]; b.task_count = cnt + 1 + in;
-                b.task_count_b = round == 0 ? b.task2_count_b : nullptr;     // the plan stage's second list
-                b.tasks2 = lists[outl]; b.task2_count = cnt + 1 + outl;
-                if (round == 0) b.task2_count_b = nullptr;                   // later rounds: one list
-                else b.task_count_b = nullptr;
-                CU(cg_launch_list(b, false, s->host.max_m, grid_for(run_occ), list_smem, st));
-                c->launches += 1;
-            }
-            if (sev[0]) { CU(cudaEventRecord(sev[3], st)); c->stage_events.push_back(sev); }
-            if (fuse_stats) {
-                // the reads the first stage handed on, as the plan and run kernels listed them (the event pair of the
-                // call brackets these launches too)
-                CU(cg_launch_stats_entries(c->stat_ents.p, cnt + 6, n_sub, a.stats_max_len, a.stats_kmax, a.stats, st));
-                c->launches += 1;
-            }
-        }
-        if (fuse_stats) c->fuse.done = true;
-        c->launches -= 1;    // the common tail below adds one
-    } else if (warpk) {
-        const long long n_mt = (n_reads + 31) / 32;
-        long long grid = (long long)wocc * c->sm_count;
-        const long long need = (n_mt + 3) / 4;
-        if (grid > need) grid = need;
-        if (grid < 1) grid = 1;
-        CU(cg_launch_warp(a, want_q, (int)grid, wsmem, st));
-    } else if (fast) {
-        const long long n_tiles = (n_reads + CG_NT - 1) / CG_NT;
-        long long grid = (long long)occ * c->sm_count;
-        if (grid > n_tiles) grid = n_tiles;
-        CU(cg_launch_fast(a, want_q, simple, (int)grid, smem, st));
-    } else {
-        // generic path: thread per read, columns in HBM scratch (16 bytes per cell)
-        const int block = 128;
-        long long threads = (long long)c->sm_count * 8 * block;
-        const long long per_thread = (long long)a.col_rows * 16;
-        while (threads > 32 * block && threads * per_thread > (1LL << 30)) threads /= 2;
-        if (threads > ((n_reads + block - 1) / block) * block) threads = ((n_reads + block - 1) / block) * block;
-        int rc = c->scratch_p.ensure((size_t)threads * a.col_rows);
-        if (rc != CG_OK) return rc;
-        rc = c->scratch_w.ensure((size_t)threads * a.col_rows * 3);
-        if (rc != CG_OK) return rc;
-        a.scratch_p = c->scratch_p.p; a.scratch_w = c->scratch_w.p; a.scratch_stride = threads;
-        CU(cg_launch_generic(a, (int)(threads / block), block, st));
-    }
-    c->launches += 1;
-    if (ev0) {
-        CU(cudaEventRecord(ev1, st));
-        c->timing.emplace_back(ev0, ev1);
+    d.kind = TrimKind::Split;
+    d.smem = scan_smem; d.occ = scan_occ;
+    // reads per sub-batch: bounds the lists to 1 + 2 x 2 GiB at the default 32 Mi (measured: fewer,
+    // larger sub-batches amortise the kernel tails and the small late DP rounds; 32 Mi vs 4 Mi = +15 % on the 100 M-read bench).
+    // CUTADAPT_B200_SUB_READS overrides it for experiments.
+    d.sub = sw.sub_reads ? sw.sub_reads : (d.plane_w && sw.task_bytes) ? (16LL << 20) : (32LL << 20);   // (tasks with bytes: 240 B each)
+    d.sub = std::min<long long>(d.sub, 1LL << 31);     // tasks name their read with 32 bits
+    // header (4 words) and, with CUTADAPT_B200_TASK_BYTES=1, the window bytes (cg_pscan.cuh).  Carrying the bytes
+    // turns the plan stage's gather into a stream but was measured neutral (plan 2.55 -> 2.65 ms, first stage
+    // 4.44 -> 4.64 ms per 100 M reads): the plan stage is bound by its dependent shared-memory chains, not by HBM.
+    d.plane_rec = d.plane_w ? (sw.task_bytes ? 4 + 2 * d.plane_w + 1 : 4) : 2;
+    return CG_OK;
+}
+
+// CTAs of a launch: `need`, at most blocks_per_sm per SM, at least one
+static int trim_grid(const cg_ctx *c, int blocks_per_sm, long long need)
+{
+    return (int)std::max<long long>(1, std::min<long long>((long long)blocks_per_sm * c->sm_count, need));
+}
+
+static int launch_index(cg_ctx *c, const CgKernelArgs &a, const TrimSchedule &d, cudaStream_t st)
+{
+    int rc = c->tasks.ensure((size_t)((std::min<long long>(a.n_reads, d.sub) + 3) / 4));
+    if (rc != CG_OK) return rc;
+    for (long long r0 = 0; r0 < a.n_reads; r0 += d.sub) {
+        const long long n_sub = std::min<long long>(d.sub, a.n_reads - r0);
+        CgKernelArgs b = a;
+        b.offsets = a.offsets + r0; b.n_reads = n_sub; b.out = a.out + (size_t)r0 * a.slots;
+        b.tasks = c->tasks.p; b.task_count = c->d_task_count;
+        CU(cudaMemsetAsync(c->d_task_count, 0, sizeof(unsigned long long), st));
+        CU(cg_launch_index(b, trim_grid(c, 16, (n_sub + CG_NT - 1) / CG_NT), st));
+        c->launches += 2;     // cg_index_kernel and cg_trim_listed_kernel
     }
     return CG_OK;
 }
 
-// Several groups, one round: per-adapter passes + selection (see plan_passes_for).
-static int launch_trim_inner(cg_ctx *c, const cg_adapterset *s, const uint8_t *d_seq, const uint8_t *d_qual,
-                             const int64_t *d_offsets, int64_t n_reads, int max_read_len, const cg_params *p,
-                             cg_match_rec *d_out, int32_t *d_qtrim, cudaStream_t st, bool timed)
+// scan -> plan -> up to four DP rounds (one run of every unfinished read per round), per sub-batch
+static int launch_split(cg_ctx *c, const cg_adapterset *s, const CgKernelArgs &a, const TrimSchedule &d,
+                        const TrimSwitches &sw, cudaStream_t st)
 {
-    if (n_reads <= 0) return CG_OK;
-    const int times = p->times < 1 ? 1 : p->times;
-    const char *kernel_env = getenv("CUTADAPT_B200_KERNEL");
-    const bool force_general = kernel_env && strcmp(kernel_env, "general") == 0;
-    if (s->passes.empty() || times != 1 || force_general)
-        return launch_trim_single(c, s, d_seq, d_qual, d_offsets, n_reads, max_read_len, p, d_out, d_qtrim, nullptr,
-                                  st, timed);
-    const bool want_q = p->quality_trim != 0 || p->nextseq_trim != 0;
-    if (want_q && !d_qual) return fail(CG_ENOQUAL, "Cannot do quality trimming when no qualities are available");
-    // the passes below see single-adapter sub-sets: their statistics are not the set's (no fusing; the caller runs the
-    // statistics kernel on the selected records)
-    struct Disarm { cg_ctx *c; bool was; ~Disarm() { c->fuse.armed = was; } } disarm{c, c->fuse.armed};
-    c->fuse.armed = false;
+    const long long cap = std::min<long long>(a.n_reads, d.sub);
+    int rc = c->tasks.ensure((size_t)cap * d.plane_rec);
+    if (rc == CG_OK) rc = c->tasks2.ensure((size_t)cap * 4);
+    if (rc == CG_OK) rc = c->tasks3.ensure((size_t)cap * 4);
+    if (rc == CG_OK && d.fuse_stats) rc = c->stat_ents.ensure((size_t)cap);
+    if (rc != CG_OK) return rc;
+    unsigned long long *cnt = c->d_task_count;
+    for (long long r0 = 0; r0 < a.n_reads; r0 += d.sub) {
+        const long long n_sub = std::min<long long>(d.sub, a.n_reads - r0);
+        CgKernelArgs b = a;
+        b.offsets = a.offsets + r0;
+        b.n_reads = n_sub;
+        b.out = a.out + (size_t)r0 * a.times * a.slots;
+        b.qtrim = a.qtrim ? a.qtrim + 2 * r0 : nullptr;
+        b.view = a.view ? a.view + 2 * r0 : nullptr;
+        b.task_cap = n_sub;
+        CU(cudaMemsetAsync(cnt, 0, 8 * sizeof(unsigned long long), st));
+        const long long need = ((n_sub + 31) / 32 + 3) / 4;
+        std::array<cudaEvent_t, 4> sev = {nullptr, nullptr, nullptr, nullptr};
+        if (sw.stage_times && c->stage_events.size() < 4096) {
+            for (auto &e : sev) CU(cudaEventCreate(&e));
+            CU(cudaEventRecord(sev[0], st));
+        }
+        b.tasks = c->tasks.p; b.task_count = cnt;
+        b.task_rec = d.plane_rec;
+        // (two input lists for the plan stage -- reads with / without locator hits -- were measured: the first
+        //  stage got 2.3x slower and the plan stage no faster, it is bound by its memory traffic; kept as an
+        //  experiment: CUTADAPT_B200_TWO_LISTS=1)
+        b.task_count_b = (d.plane_w && sw.two_lists) ? cnt + 4 : nullptr;
+        if (d.plane_w && d.jit) {
+            const int rcj = cg_jit_launch(d.jit, trim_grid(c, d.jit_occ, need), CG_NT, d.smem, (void *)st, &b);
+            if (rcj != 0) return fail(CG_ECUDA, "launch of the specialised first stage failed (CUresult " + std::to_string(rcj) + ")");
+        }
+        else if (d.plane_w) CU(cg_launch_pscan(b, a.quality_trim != 0, d.plane_w, trim_grid(c, d.occ, need), d.smem, st));
+        else CU(cg_launch_scan(b, a.quality_trim != 0, trim_grid(c, d.occ, need), d.smem, st));
+        if (sev[0]) CU(cudaEventRecord(sev[1], st));
+        b.stat_ents = c->stat_ents.p; b.stat_count = cnt + 6;
+        b.tasks2 = c->tasks2.p; b.task2_count = cnt + 1;
+        b.tasks3 = c->tasks3.p; b.task3_count = cnt + 2;
+        // run records of the plane path go to two lists (banded first runs / the others): cnt[5] counts the second
+        // (only with the band compiled in, CG_RUN_BAND)
+        b.task2_count_b = (CG_RUN_BAND && d.plane_w && !sw.no_band_lists) ? cnt + 5 : nullptr;
+        CU(cg_launch_list(b, true, s->host.max_m, trim_grid(c, d.plan_occ, need), d.list_smem, st));
+        c->launches += 2;
+        if (d.plane_w) {
+            // second plan launch: the reads the first one set aside (windows with other letters than A/C/G/T),
+            // scanned exactly on dense warps; its run records continue the same list
+            CgKernelArgs b2 = b;
+            b2.tasks = c->tasks3.p; b2.task_count = cnt + 2; b2.task_rec = 2;
+            b2.tasks3 = nullptr; b2.task3_count = cnt + 3; b2.task_count_b = nullptr;
+            CU(cg_launch_list(b2, true, s->host.max_m, trim_grid(c, d.plan_occ, need), d.list_smem, st));
+            CU(cudaMemsetAsync(cnt + 2, 0, sizeof(unsigned long long), st));
+            c->launches += 1;
+        }
+        if (sev[0]) CU(cudaEventRecord(sev[2], st));
+        uint4 *lists[2] = {c->tasks2.p, c->tasks3.p};
+        for (int round = 0; round < 4; ++round) {
+            const int in = round & 1, outl = in ^ 1;
+            if (round > 0) CU(cudaMemsetAsync(cnt + 1 + outl, 0, sizeof(unsigned long long), st));
+            b.tasks = lists[in]; b.task_count = cnt + 1 + in;
+            b.task_count_b = round == 0 ? b.task2_count_b : nullptr;     // the plan stage's second list
+            b.tasks2 = lists[outl]; b.task2_count = cnt + 1 + outl;
+            if (round == 0) b.task2_count_b = nullptr;                   // later rounds: one list
+            else b.task_count_b = nullptr;
+            CU(cg_launch_list(b, false, s->host.max_m, trim_grid(c, d.run_occ, need), d.list_smem, st));
+            c->launches += 1;
+        }
+        if (sev[0]) { CU(cudaEventRecord(sev[3], st)); c->stage_events.push_back(sev); }
+        if (d.fuse_stats) {
+            // the reads the first stage handed on, as the plan and run kernels listed them (the event pair of the
+            // call brackets these launches too)
+            CU(cg_launch_stats_entries(c->stat_ents.p, cnt + 6, n_sub, a.stats_max_len, a.stats_kmax, a.stats, st));
+            c->launches += 1;
+        }
+    }
+    return CG_OK;
+}
+
+// generic path: thread per read, columns in HBM scratch (16 bytes per cell)
+static int launch_generic(cg_ctx *c, CgKernelArgs a, cudaStream_t st)
+{
+    const int block = 128;
+    long long threads = (long long)c->sm_count * 8 * block;
+    const long long per_thread = (long long)a.col_rows * 16;
+    while (threads > 32 * block && threads * per_thread > (1LL << 30)) threads /= 2;
+    if (threads > ((a.n_reads + block - 1) / block) * block) threads = ((a.n_reads + block - 1) / block) * block;
+    int rc = c->scratch_p.ensure((size_t)threads * a.col_rows);
+    if (rc != CG_OK) return rc;
+    rc = c->scratch_w.ensure((size_t)threads * a.col_rows * 3);
+    if (rc != CG_OK) return rc;
+    a.scratch_p = c->scratch_p.p; a.scratch_w = c->scratch_w.p; a.scratch_stride = threads;
+    CU(cg_launch_generic(a, (int)(threads / block), block, st));
+    c->launches += 1;
+    return CG_OK;
+}
+
+static int trim_pass(cg_ctx *c, const cg_adapterset *s, const uint8_t *d_seq, const uint8_t *d_qual,
+                     const int64_t *d_offsets, int64_t n_reads, int max_read_len, const cg_params *p,
+                     cg_match_rec *d_out, int32_t *d_qtrim, const int32_t *d_view, cudaStream_t st, bool timed,
+                     const StatsRequest *stats, const TrimSwitches &sw, bool *stats_counted);
+
+// Several groups, one round: per-adapter passes + selection (see plan_passes_for).  The passes see single-adapter
+// sub-sets whose statistics are not the set's, so they count none (the caller counts them on the selected records).
+static int launch_multi_pass(cg_ctx *c, const cg_adapterset *s, const CgKernelArgs &a, int max_read_len,
+                             const cg_params *p, const TrimSchedule &d, const TrimSwitches &sw, cudaStream_t st)
+{
+    const bool want_q = a.quality_trim != 0;
     const int np = (int)s->passes.size();
-    long long SUB = 32LL << 20;
-    if (const char *e = getenv("CUTADAPT_B200_SUB_READS")) { const long long v = atoll(e); if (v >= 1024) SUB = v; }
-    const long long cap = std::min<long long>(n_reads, SUB);
+    const long long cap = std::min<long long>(a.n_reads, d.sub);
     int rc = c->pass_tmp.ensure((size_t)cap * np);
     if (rc != CG_OK) return rc;
     bool any_linked = false;
     for (auto &P : s->passes) any_linked = any_linked || P.role == 1;
     if (any_linked) { rc = c->view_back.ensure((size_t)cap * 2); if (rc != CG_OK) return rc; }
-    if (want_q && !d_qtrim) { rc = c->view_base.ensure((size_t)cap * 2); if (rc != CG_OK) return rc; }
+    if (want_q && !a.qtrim) { rc = c->view_base.ensure((size_t)cap * 2); if (rc != CG_OK) return rc; }
 
     CgSelectArgs sel;
     memset(&sel, 0, sizeof sel);
     sel.tmp = c->pass_tmp.p; sel.stride = cap; sel.pass_map = s->d_pass_map;
     sel.t = s->select_tables;
 
-    cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-    if (timed && c->timing.size() < 8192) {
-        for (cudaEvent_t *ev : {&ev0, &ev1}) {
-            if (!c->event_pool.empty()) { *ev = c->event_pool.back(); c->event_pool.pop_back(); }
-            else CU(cudaEventCreate(ev));
-        }
-        CU(cudaEventRecord(ev0, st));
-    }
-    for (long long r0 = 0; r0 < n_reads; r0 += SUB) {
-        const long long n_sub = std::min<long long>(SUB, n_reads - r0);
-        const int64_t *offs = d_offsets + r0;
-        int32_t *qt = want_q ? (d_qtrim ? d_qtrim + 2 * r0 : c->view_base.p) : nullptr;
+    for (long long r0 = 0; r0 < a.n_reads; r0 += d.sub) {
+        const long long n_sub = std::min<long long>(d.sub, a.n_reads - r0);
+        const int64_t *offs = a.offsets + r0;
+        int32_t *qt = want_q ? (a.qtrim ? a.qtrim + 2 * r0 : c->view_base.p) : nullptr;
         const int32_t *base_view = nullptr;
         for (int pi = 0; pi < np; ++pi) {
             const auto &P = s->passes[pi];
@@ -896,24 +866,80 @@ static int launch_trim_inner(cg_ctx *c, const cg_adapterset *s, const uint8_t *d
                 c->launches += 1;
                 view = c->view_back.p;
             }
-            if (want_q && pi == 0) {        // the first pass does the quality trimming (fused) for all
-                rc = launch_trim_single(c, P.sub, d_seq, d_qual, offs, n_sub, max_read_len, &pp, tmp, qt, nullptr, st, false);
-                base_view = qt;
-            } else {
-                pp.quality_trim = 0; pp.nextseq_trim = 0;
-                rc = launch_trim_single(c, P.sub, d_seq, nullptr, offs, n_sub, max_read_len, &pp, tmp, nullptr, view, st, false);
-            }
+            const bool trims = want_q && pi == 0;    // the first pass does the quality trimming (fused) for all
+            if (!trims) { pp.quality_trim = 0; pp.nextseq_trim = 0; }
+            rc = trim_pass(c, P.sub, a.seq, trims ? a.qual : nullptr, offs, n_sub, max_read_len, &pp, tmp,
+                           trims ? qt : nullptr, trims ? nullptr : view, st, false, nullptr, sw, nullptr);
             if (rc != CG_OK) return rc;
+            if (trims) base_view = qt;
         }
         sel.n_reads = n_sub;
-        sel.out = d_out + (size_t)r0 * s->host.slots;
+        sel.out = a.out + (size_t)r0 * s->host.slots;
         CU(cg_launch_select(sel, st));
         c->launches += 1;
     }
-    if (ev0) {
-        CU(cudaEventRecord(ev1, st));
-        c->timing.emplace_back(ev0, ev1);
+    return CG_OK;
+}
+
+// One trimming pass as choose_schedule decides it.  *stats_counted (when not null): whether the pass added the
+// statistics of its reads to stats->d_stats.
+static int trim_pass(cg_ctx *c, const cg_adapterset *s, const uint8_t *d_seq, const uint8_t *d_qual,
+                     const int64_t *d_offsets, int64_t n_reads, int max_read_len, const cg_params *p,
+                     cg_match_rec *d_out, int32_t *d_qtrim, const int32_t *d_view, cudaStream_t st, bool timed,
+                     const StatsRequest *stats, const TrimSwitches &sw, bool *stats_counted)
+{
+    const bool want_q = p->quality_trim != 0 || p->nextseq_trim != 0;
+    if (want_q && !d_qual) return fail(CG_ENOQUAL, "Cannot do quality trimming when no qualities are available");
+    TrimSchedule d;
+    int rc = choose_schedule(c, s, n_reads, max_read_len, p, d_view != nullptr, stats, sw, d);
+    if (rc != CG_OK) return rc;
+    CgKernelArgs a;
+    memset(&a, 0, sizeof a);
+    a.blob = s->d_blob; a.blob_bytes = (uint32_t)s->host.blob.size();
+    a.masks64 = s->d_masks; a.enc = c->d_enc; a.index = s->d_index;
+    a.seq = d_seq; a.qual = want_q ? d_qual : nullptr; a.offsets = d_offsets; a.n_reads = n_reads;
+    // flags and packed base/cutoff as pre_trim_core expects them
+    a.quality_trim = (p->quality_trim ? 1 : 0) | (p->nextseq_trim ? 2 : 0);
+    a.cutoff_front = p->cutoff_front; a.cutoff_back = p->cutoff_back;
+    a.qbase = (p->quality_base & 255) | (int)((unsigned)p->nextseq_cutoff << 8);
+    a.times = p->times < 1 ? 1 : p->times; a.slots = s->host.slots;
+    a.out = d_out; a.qtrim = d_qtrim; a.view = d_view; a.err_flag = c->d_err;
+    a.col_rows = s->host.max_m + 1; a.no_band = sw.no_band;
+    a.tile_cap = d.tile_cap; a.mini_cap = d.mini_cap; a.carry_slot = d.carry_slot;
+    if (d.fuse_stats) { a.stats = stats->d_stats; a.stats_max_len = stats->max_len; a.stats_kmax = stats->kmax; }
+    // the event pair of a timed call (cg_ctx_kernel_time) brackets everything the call launches
+    cudaEvent_t ev[2] = {nullptr, nullptr};
+    if (timed && c->timing.size() < 8192) {
+        for (cudaEvent_t &e : ev) {
+            if (!c->event_pool.empty()) { e = c->event_pool.back(); c->event_pool.pop_back(); }
+            else CU(cudaEventCreate(&e));
+        }
+        CU(cudaEventRecord(ev[0], st));
     }
+    switch (d.kind) {
+    case TrimKind::Index: rc = launch_index(c, a, d, st); break;
+    case TrimKind::Light:
+        CU(cg_launch_light(a, trim_grid(c, 16, (n_reads + CG_NT - 1) / CG_NT), st));
+        c->launches += 1;
+        break;
+    case TrimKind::Split: rc = launch_split(c, s, a, d, sw, st); break;
+    case TrimKind::Warp:
+        CU(cg_launch_warp(a, want_q, trim_grid(c, d.occ, ((n_reads + 31) / 32 + 3) / 4), d.smem, st));
+        c->launches += 1;
+        break;
+    case TrimKind::Fast:
+        CU(cg_launch_fast(a, want_q, d.simple, trim_grid(c, d.occ, (n_reads + CG_NT - 1) / CG_NT), d.smem, st));
+        c->launches += 1;
+        break;
+    case TrimKind::Generic: rc = launch_generic(c, a, st); break;
+    case TrimKind::MultiPass: rc = launch_multi_pass(c, s, a, max_read_len, p, d, sw, st); break;
+    }
+    if (rc != CG_OK) return rc;
+    if (ev[0]) {
+        CU(cudaEventRecord(ev[1], st));
+        c->timing.emplace_back(ev[0], ev[1]);
+    }
+    if (stats_counted) *stats_counted = d.fuse_stats;
     return CG_OK;
 }
 
@@ -963,38 +989,39 @@ extern "C" int cg_locate_debug(cg_ctx *c, const cg_adapter_desc *adapter, const 
 // The work lists, counters and per-pass scratch of a context are shared by all of its streams: the
 // kernels of one trimming pass are ordered after those of the previous pass, whichever lane issued it.
 // (They fill the GPU on their own; what overlaps across lanes are the copies.)
+// stats: statistics wanted with the pass, or null; *stats_counted (when not null): whether the pass counted them.
 static int launch_trim(cg_ctx *c, const cg_adapterset *s, const uint8_t *d_seq, const uint8_t *d_qual,
                        const int64_t *d_offsets, int64_t n_reads, int max_read_len, const cg_params *p,
-                       cg_match_rec *d_out, int32_t *d_qtrim, cudaStream_t st, bool timed)
+                       cg_match_rec *d_out, int32_t *d_qtrim, cudaStream_t st, bool timed,
+                       const StatsRequest *stats = nullptr, bool *stats_counted = nullptr)
 {
     if (n_reads <= 0) return CG_OK;
     if (c->scratch_busy && c->scratch_stream != st) CU(cudaStreamWaitEvent(st, c->scratch_ev, 0));
-    const int rc = launch_trim_inner(c, s, d_seq, d_qual, d_offsets, n_reads, max_read_len, p, d_out, d_qtrim, st, timed);
+    const int rc = trim_pass(c, s, d_seq, d_qual, d_offsets, n_reads, max_read_len, p, d_out, d_qtrim, nullptr, st, timed,
+                             stats, TrimSwitches(), stats_counted);
     CU(cudaEventRecord(c->scratch_ev, st));
     c->scratch_busy = true;
     c->scratch_stream = st;
     return rc;
 }
 
-// A trimming pass plus the statistics of its reads (cg_stats_*) added to d_stats: fused into the split pipeline where
-// that is possible, otherwise cg_stats_kernel over the records afterwards.
+// A trimming pass plus the statistics of its reads (cg_stats_*) added to d_stats: counted inside the split pipeline
+// where choose_schedule fuses them, otherwise by cg_stats_kernel over the records afterwards.
 static int launch_trim_with_stats(cg_ctx *c, const cg_adapterset *s, const uint8_t *d_seq, const uint8_t *d_qual,
                                   const int64_t *d_offsets, int64_t n_reads, int max_read_len, const cg_params *p,
                                   cg_match_rec *d_out, int32_t *d_qtrim, cudaStream_t st, bool timed,
                                   unsigned long long *d_stats, int stats_max_len, int stats_kmax)
 {
     if (n_reads <= 0) return CG_OK;
-    c->fuse.d_stats = d_stats; c->fuse.max_len = stats_max_len; c->fuse.kmax = stats_kmax;
-    c->fuse.armed = true; c->fuse.done = false;
-    const int rc = launch_trim(c, s, d_seq, d_qual, d_offsets, n_reads, max_read_len, p, d_out, d_qtrim, st, timed);
-    c->fuse.armed = false;
-    if (rc != CG_OK) return rc;
-    if (!c->fuse.done) {
-        const int times = p->times < 1 ? 1 : p->times;
-        CU(cg_launch_stats(d_seq, d_offsets, n_reads, (p->quality_trim || p->nextseq_trim) && d_qtrim, times, s->host.slots,
-                           d_out, d_qtrim, s->host.n_adapters, stats_max_len, stats_kmax, d_stats, st));
-        c->launches += 1;
-    }
+    const StatsRequest req = {d_stats, stats_max_len, stats_kmax};
+    bool counted = false;
+    const int rc = launch_trim(c, s, d_seq, d_qual, d_offsets, n_reads, max_read_len, p, d_out, d_qtrim, st, timed, &req,
+                               &counted);
+    if (rc != CG_OK || counted) return rc;
+    const int times = p->times < 1 ? 1 : p->times;
+    CU(cg_launch_stats(d_seq, d_offsets, n_reads, (p->quality_trim || p->nextseq_trim) && d_qtrim, times, s->host.slots,
+                       d_out, d_qtrim, s->host.n_adapters, stats_max_len, stats_kmax, d_stats, st));
+    c->launches += 1;
     return CG_OK;
 }
 

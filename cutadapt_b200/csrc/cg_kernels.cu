@@ -723,7 +723,7 @@ __global__ void __launch_bounds__(CG_NT, W <= 5 ? CG_PSCAN_BLOCKS : 5) cg_pscan_
 typedef void (*pscan_kernel_t)(const CgKernelArgs);
 static pscan_kernel_t pick_pscan(bool has_qual, int w, bool stats)
 {
-    // (the statistics are counted in this stage only for passes without quality trimming: launch_trim_single)
+    // (the statistics are counted in this stage only for passes without quality trimming: choose_schedule)
     if (stats) return w <= 5 ? cg_pscan_kernel<false, 5, true> : cg_pscan_kernel<false, 8, true>;
     if (w <= 5) return has_qual ? cg_pscan_kernel<true, 5, false> : cg_pscan_kernel<false, 5, false>;
     return has_qual ? cg_pscan_kernel<true, 8, false> : cg_pscan_kernel<false, 8, false>;
@@ -766,7 +766,7 @@ __host__ __device__ inline DpSmem dp_smem_layout(uint32_t blob_bytes, int slot_b
 size_t cg_dp_smem_bytes(uint32_t blob_bytes, int slot_bytes) { return dp_smem_layout(blob_bytes, slot_bytes).total; }
 
 // Fused statistics of the reads the list kernels finish (one round, one slot, no quality trimming: the only passes
-// that fuse the statistics, launch_trim_single): every lane that writes a final record now (fin; the window is the
+// that fuse the statistics, choose_schedule): every lane that writes a final record now (fin; the window is the
 // whole read) appends what stats_read_core needs of it as one 8-byte entry to a.stat_ents, which
 // cg_stats_entries_kernel counts after the DP rounds -- a stream instead of the gather of every record and of the
 // base in front of its match.  Entry: x = read length | final length << 16, y = match | 3' side << 1 | adjacent-base

@@ -33,7 +33,7 @@ struct ScanSmem { size_t blob_off, enc_off, stats_off, warp_off, warp_stride, ba
                                   // {M0, flags, M1, M2}, {M3 .. M6}, {M7, window offset, 0, 0} with M = PlaneOut::M (+ CG_TASK_BYTES);
                                   // flags bits 12-15: plane words W, bit 20: PlaneOut::end_hit, bit 21: PlaneOut::no_end
 // ------------------------------------------------------------------------------------------
-// Fused statistics (one plain adapter, one round, one slot: the passes launch_trim_single fuses them into): per-CTA
+// Fused statistics (one plain adapter, one round, one slot: the passes choose_schedule fuses them into): per-CTA
 // histograms in shared memory, flushed once at the end of the CTA.  Layout: read lengths (max_len + 1), removed
 // lengths for 5' then for 3' matches ((max_len + 1) x cols each: cols = 1 keeps 0 errors only, kmax + 1 every error
 // count), adjacent bases (8), then 8 64-bit scalars (reads, matches, bases, quality-trimmed, adapter bases).
