@@ -141,6 +141,9 @@ class cg_fastq_params(C.Structure):
         ("format", C.c_int32),
         ("stats", C.c_int32),
         ("gzip_outputs", C.c_int32),
+        ("max_average_error_rate", C.c_double),
+        ("zero_cap", C.c_int32),
+        ("reserved_pad", C.c_int32),
     ]
 
 
@@ -148,12 +151,12 @@ class cg_fastq_result(C.Structure):
     _fields_ = [(name, C.c_int64) for name in (
         "n_records", "n_written", "bp_in", "bp_out", "out_bytes", "with_adapters", "quality_trimmed_bp",
         "too_short", "too_long", "too_many_n", "too_many_expected_errors", "discarded", "casava_filtered",
-        "reverse_complemented", "out_bytes_plain")] + [("reserved", C.c_int64 * 1)]
+        "reverse_complemented", "out_bytes_plain", "too_high_average_error_rate")]
 
     def as_dict(self, plain_bytes: bool = False) -> dict:
         """The counters; out_bytes_plain (the uncompressed size of gzip outputs) only with plain_bytes."""
         return {name: int(getattr(self, name)) for name, _ in self._fields_
-                if name != "reserved" and (plain_bytes or name != "out_bytes_plain")}
+                if plain_bytes or name != "out_bytes_plain"}
 
 
 class cg_gzin_result(C.Structure):

@@ -2431,6 +2431,7 @@ struct FqStage {
     FqStatsAcc *acc = nullptr;           // statistics on: the accumulator of this mate ...
     int st_len = 0, st_kmax = 0;         // ... and the layout of the chunk's vector in d_fqstats
     bool st_poly_a = false;              // d_polya was filled
+    int zero_cap = 0;                    // ZeroCapper: the quality base the written qualities are capped at, 0 = off
     bool has_qual() const { return format != CG_FORMAT_FASTA; }
     bool fasta_out() const { return format != CG_FORMAT_FASTQ; }
 };
@@ -2439,7 +2440,7 @@ static int fastq_enabled_filters(const cg_fastq_params *fp)
 {
     return (fp->minimum_length > 0 ? 1 : 0) | (fp->maximum_length >= 0 ? 2 : 0) | (fp->max_n >= 0.0 ? 4 : 0) |
            (fp->max_expected_errors >= 0.0 ? 8 : 0) | (fp->discard_casava ? 16 : 0) | (fp->discard_trimmed ? 32 : 0) |
-           (fp->discard_untrimmed ? 64 : 0);
+           (fp->discard_untrimmed ? 64 : 0) | (fp->max_average_error_rate > 0.0 ? 128 : 0);
 }
 
 // FASTA chunk (format 1) -> normalised chunk in f.d_in + record table: line classes, two scans, scatter, records.
@@ -2618,10 +2619,16 @@ static int fastq_stage_records(cg_ctx *c, FastqSlot &f, const cg_fastq_params *f
 {
     if (fp->format < CG_FORMAT_FASTQ || fp->format > CG_FORMAT_FASTQ_TO_FASTA)
         return fail(CG_EINVAL, "cg_fastq: format must be 0 (FASTQ), 1 (FASTA) or 2 (FASTQ in, FASTA out)");
-    if (fp->format == CG_FORMAT_FASTA &&
-        (fp->trim.quality_trim || fp->trim.nextseq_trim || fp->max_expected_errors >= 0.0))
-        return fail(CG_EINVAL, "FASTA input has no qualities: quality trimming, --nextseq-trim and --max-ee need FASTQ");
+    if (fp->format == CG_FORMAT_FASTA && (fp->trim.quality_trim || fp->trim.nextseq_trim || fp->max_expected_errors >= 0.0 ||
+                                          fp->max_average_error_rate != 0.0 || fp->zero_cap))
+        return fail(CG_EINVAL, "FASTA input has no qualities: quality trimming, --nextseq-trim, --max-ee, --max-aer and "
+                               "--zero-cap need FASTQ");
+    // TooHighAverageErrorRate rejects a rate outside (0, 1) (predicates.py:81-85); 0 here means off
+    if (!(fp->max_average_error_rate >= 0.0 && fp->max_average_error_rate < 1.0))
+        return fail(CG_EINVAL, "cg_fastq: max_average_error_rate must be between 0.0 and 1.0 (0 = off)");
+    if (fp->zero_cap != 0 && fp->zero_cap != 1) return fail(CG_EINVAL, "cg_fastq: zero_cap must be 0 or 1");
     g.format = fp->format;
+    g.zero_cap = fp->zero_cap ? (fp->trim.quality_base & 255) : 0;
     CU(cudaStreamSynchronize(f.stream));        // upload + newline count of this slot
     const int64_t n_bytes = f.n_bytes;
     g.n_nl = (long long)f.h_counters.p[0];
@@ -2748,6 +2755,8 @@ static int fastq_stage_verdict(cg_ctx *c, FastqSlot &f, const cg_fastq_params *f
     flt.trim_n = fp->trim_n;
     flt.discard_casava = fp->discard_casava;
     flt.action = g.action;
+    flt.max_aer = fp->max_average_error_rate;
+    flt.zero_cap = g.zero_cap;
     CU(cg_launch_fastq_evaluate(f.d_in.p, f.d_rec.p, f.d_len.p, g.n, g.d_matches, g.times, g.slots, g.d_qtrim, flt,
                                 c->d_phred, g.d_is_rc, f.d_interval.p, f.d_keep.p, f.d_mask.p, f.d_counters.p + 1, f.d_err.p,
                                 st, d_poly_a));
@@ -2861,7 +2870,7 @@ static void fastq_stats_commit(const FastqSlot &f, const FqStage &g, const cg_fa
     v[0] += res.n_records; v[1] += res.bp_in; v[2] += res.with_adapters; v[3] += res.quality_trimmed_bp;
     v[4] += (int64_t)h[4]; v[5] += res.reverse_complemented; v[6] += res.n_written; v[7] += res.bp_out;
     v[8] += res.too_short; v[9] += res.too_long; v[10] += res.too_many_n; v[11] += res.too_many_expected_errors;
-    v[12] += res.casava_filtered;
+    v[12] += res.casava_filtered; v[15] += res.too_high_average_error_rate;
     // --discard-trimmed and --discard-untrimmed exclude each other (cli.py:798-808)
     v[fp->discard_trimmed ? 13 : 14] += res.discarded;
 }
@@ -2991,6 +3000,7 @@ static int fastq_stage_result(FastqSlot &f, const FqStage &g, cudaStream_t st, c
     res->too_many_expected_errors = (int64_t)k[9];
     res->casava_filtered = (int64_t)k[10];
     res->reverse_complemented = (int64_t)k[11];
+    res->too_high_average_error_rate = (int64_t)k[12];
     return CG_OK;
 }
 
@@ -3001,7 +3011,7 @@ static int fastq_write_records(cg_ctx *c, FastqSlot &f, const FqStage &g, uint8_
 {
     if (!sp) {
         CU(cg_launch_fastq_write(f.d_in.p, f.d_rec.p, f.d_interval.p, f.d_outoff.p, f.d_outlen.p, g.n, d_out, g.action,
-                                 f.d_keep.p, f.d_mask.p, g.rc_suffix, st, g.fasta_out() ? 1 : 0));
+                                 f.d_keep.p, f.d_mask.p, g.rc_suffix, st, g.fasta_out() ? 1 : 0, nullptr, 0, g.zero_cap));
         c->launches += 1;
         return CG_OK;
     }
@@ -3011,7 +3021,7 @@ static int fastq_write_records(cg_ctx *c, FastqSlot &f, const FqStage &g, uint8_
             present |= ((sp->fasta_dests >> d) & 1) == fa && segments[d + 1] > segments[d];
         if (!present) continue;
         CU(cg_launch_fastq_write(f.d_in.p, f.d_rec.p, f.d_interval.p, f.d_outoff.p, f.d_outlen.p, g.n, d_out, g.action,
-                                 f.d_keep.p, f.d_mask.p, g.rc_suffix, st, fa, sp->d_route, sp->fasta_dests));
+                                 f.d_keep.p, f.d_mask.p, g.rc_suffix, st, fa, sp->d_route, sp->fasta_dests, g.zero_cap));
         c->launches += 1;
     }
     return CG_OK;
@@ -3260,7 +3270,7 @@ static int fastq_stage_rows(cg_ctx *c, FastqSlot &f, const FqStage &g, const cg_
                            cudaMemcpyHostToDevice, st));
         CU(cg_launch_fastq_info(0, f.d_in.p, f.d_rec.p, f.d_origin.p, f.d_interval.p, f.d_mask.p, g.d_matches, g.times,
                                 g.slots, q.d_text.p, q.d_textoff.p, fp->revcomp != 0, g.rc_suffix, upper, n, q.d_row.p,
-                                nullptr, nullptr, st, k, g.d_qtrim, f.d_len.p, g.has_qual() ? 1 : 0));
+                                nullptr, nullptr, st, k, g.d_qtrim, f.d_len.p, g.has_qual() ? 1 : 0, g.zero_cap));
         CU(cg_launch_scan_i32(q.d_row.p, n, f.d_scan.p, q.d_rowoff.p, st));
         long long total = 0;
         CU(cudaMemcpyAsync(&total, q.d_rowoff.p + n, sizeof total, cudaMemcpyDeviceToHost, st));
@@ -3274,7 +3284,7 @@ static int fastq_stage_rows(cg_ctx *c, FastqSlot &f, const FqStage &g, const cg_
         if ((rc = q.d_out.ensure((size_t)total + 64)) != CG_OK) return rc;
         CU(cg_launch_fastq_info(1, f.d_in.p, f.d_rec.p, f.d_origin.p, f.d_interval.p, f.d_mask.p, g.d_matches, g.times,
                                 g.slots, q.d_text.p, q.d_textoff.p, fp->revcomp != 0, g.rc_suffix, upper, n, nullptr,
-                                q.d_rowoff.p, q.d_out.p, st, k, g.d_qtrim, f.d_len.p, g.has_qual() ? 1 : 0));
+                                q.d_rowoff.p, q.d_out.p, st, k, g.d_qtrim, f.d_len.p, g.has_qual() ? 1 : 0, g.zero_cap));
         c->launches += 1;
         if (q.gzip) {
             std::vector<int64_t> bounds{0, (int64_t)total};

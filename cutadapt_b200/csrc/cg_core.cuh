@@ -463,19 +463,21 @@ CG_HD int poly_a_trim_core(const uint8_t *seq, int n, int revcomp)
 // reference's order -- four accumulators over groups of four, the tail into the first, then
 // ((e0 + e1) + e2) + e3 -- so the double is bit-identical.  -1.0 = a character outside [base, 126].
 // `table` = 256 doubles, table[q] = 10^(-q/10) (cg_build_phred_table).
-CG_HD double expected_errors_core(const uint8_t *q, int n, int base, const double *table)
+// cap (ZeroCapper, modifiers.py:806-822): every character below it counts as the cap itself; 0 = as they are.
+CG_HD double expected_errors_core(const uint8_t *q, int n, int base, const double *table, int cap = 0)
 {
     double e0 = 0.0, e1 = 0.0, e2 = 0.0, e3 = 0.0;
-    const uint8_t b = (uint8_t)base, max_phred = (uint8_t)(126 - base);
+    const uint8_t b = (uint8_t)base, max_phred = (uint8_t)(126 - base), c = (uint8_t)cap;
+    auto at = [&](int i) -> uint8_t { return q[i] < c ? c : q[i]; };
     int i = 0;
     for (; i + 3 < n; i += 4) {
-        const uint8_t p0 = (uint8_t)(q[i] - b), p1 = (uint8_t)(q[i + 1] - b);
-        const uint8_t p2 = (uint8_t)(q[i + 2] - b), p3 = (uint8_t)(q[i + 3] - b);
+        const uint8_t p0 = (uint8_t)(at(i) - b), p1 = (uint8_t)(at(i + 1) - b);
+        const uint8_t p2 = (uint8_t)(at(i + 2) - b), p3 = (uint8_t)(at(i + 3) - b);
         if (p0 > max_phred || p1 > max_phred || p2 > max_phred || p3 > max_phred) return -1.0;
         e0 += table[p0]; e1 += table[p1]; e2 += table[p2]; e3 += table[p3];
     }
     for (; i < n; ++i) {
-        const uint8_t ph = (uint8_t)(q[i] - b);
+        const uint8_t ph = (uint8_t)(at(i) - b);
         if (ph > max_phred) return -1.0;
         e0 += table[ph];
     }

@@ -457,8 +457,9 @@ __global__ void fq_evaluate_kernel(const uint8_t *buf, const CgFastqRecord *rec,
 }
 
 // counter slot of filter bit k (the layout of cg_fastq_result): 4 too_short, 5 too_long, 8 too_many_n,
-// 9 too_many_expected_errors, 10 casava_filtered, 7 discarded (trimmed / untrimmed)
-__device__ __constant__ int kFilterCounter[7] = {4, 5, 8, 9, 10, 7, 7};
+// 9 too_many_expected_errors, 10 casava_filtered, 7 discarded (trimmed / untrimmed), 12 too_high_average_error_rate
+__device__ __constant__ int kFilterCounter[8] = {4, 5, 8, 9, 10, 7, 7, 12};
+#define FQ_FIRED_NO_WRITER 8     // a demultiplexed pair without a writer: dropped, counted by no filter
 
 // The verdict on a read (mask2 == nullptr) or a pair.  For every enabled filter, in chain order, the pair is
 // filtered according to PairedEndFilter (steps.py:105-180): a filter given for one mate only tests that mate;
@@ -483,7 +484,7 @@ __global__ void fq_finish_kernel(long long n_records, const CgFastqRecord *rec1,
     if (r < n_records) {
         fired = fq_finish_core(mask1[r], mask2 ? mask2[r] : 0, mask2 != nullptr, enabled1, enabled2, mode, mode_untrimmed);
         // a demultiplexer without a writer for this destination drops the pair without counting it (steps.py:574-577)
-        if (fired < 0 && dest_keep && !dest_keep[dest[r]]) fired = 7;
+        if (fired < 0 && dest_keep && !dest_keep[dest[r]]) fired = FQ_FIRED_NO_WRITER;
         int to = fired < 0 ? 0 : -1;
         bool fa = fasta_out != 0;
         if (route) {
@@ -511,7 +512,7 @@ __global__ void fq_finish_kernel(long long n_records, const CgFastqRecord *rec1,
         bp2 += __shfl_down_sync(0xFFFFFFFFu, bp2, d);
     }
     // filter counters: one atomic per warp and filter that fired
-    for (int k = 0; k < 7; ++k) {
+    for (int k = 0; k < 8; ++k) {
         const unsigned cnt = __popc(__ballot_sync(0xFFFFFFFFu, fired == k));
         if (cnt && (threadIdx.x & 31) == 0) {
             atomicAdd(&counters1[kFilterCounter[k]], (unsigned long long)cnt);
@@ -576,14 +577,16 @@ __global__ void fq_stats_tail_kernel(long long n_records, const int32_t *interva
 
 // the trimmed records, one warp per record; FASTA_OUT: ">name\nsequence\n", the sequence on one line.
 // route != nullptr (filter outputs): only the records whose destination d has bit d of fasta_dests == FASTA_OUT (the
-// other format's records are left to the other instantiation)
+// other format's records are left to the other instantiation).  zero_cap (ZeroCapper, modifiers.py:806-822): quality
+// characters below it are written as it; 0 = as they are.
 template <bool FASTA_OUT>
 __global__ void __launch_bounds__(256) fq_write_kernel(const uint8_t *buf, const CgFastqRecord *rec, const int32_t *interval,
                                                         const int64_t *out_off, const int32_t *out_len,
                                                         long long n_records, uint8_t *out, int action,
                                                         const int32_t *keep_interval, const int32_t *mask, int rc_suffix,
-                                                        const int32_t *route, int fasta_dests)
+                                                        const int32_t *route, int fasta_dests, int zero_cap)
 {
+    const uint8_t cap = (uint8_t)zero_cap;
     const int lane = threadIdx.x & 31;
     const long long warps = ((long long)gridDim.x * blockDim.x) >> 5;
     for (long long r = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5; r < n_records; r += warps) {
@@ -620,7 +623,10 @@ __global__ void __launch_bounds__(256) fq_write_kernel(const uint8_t *buf, const
             continue;
         }
         if (lane < 3) p[lane] = lane == 1 ? '+' : '\n';
-        for (int j = lane; j < left; j += 32) p[3 + j] = buf[m.qual_start + start + j];
+        for (int j = lane; j < left; j += 32) {
+            const uint8_t q = buf[m.qual_start + start + j];
+            p[3 + j] = q < cap ? cap : q;
+        }
         if (lane == 0) p[3 + left] = '\n';
     }
 }
@@ -630,11 +636,12 @@ __global__ void __launch_bounds__(256) fq_write_kernel(const uint8_t *buf, const
 // Per match: name, errors, rstart, rstop, before, match, after, adapter name, three quality parts, rc flag; the
 // coordinates of every round are applied to info.original_read -- the read AS IT CAME (before -u and the quality
 // trimmers; reverse-complemented if the reverse complement was chosen) -- from its first base, and the read is then
-// cut the way the match cuts it.  Reads without a match: name, -1, sequence and qualities of the read as written.
+// cut the way the match cuts it.  Reads without a match: name, -1, sequence and qualities of the read as written
+// (ZeroCapper included; the rows of a match show the original qualities).
 // The same walk runs twice: with a counting sink (row bytes per record) and, after a scan, with a writing sink.
 struct InfoCountSink {
     long long n = 0;
-    __device__ void bytes(const uint8_t *, int len, bool = false) { n += len; }
+    __device__ void bytes(const uint8_t *, int len, bool = false, uint8_t = 0) { n += len; }
     __device__ void ch(uint8_t) { n += 1; }
     __device__ void number(int v)
     {
@@ -647,11 +654,12 @@ struct InfoCountSink {
 struct InfoWriteSink {                  // all 32 lanes of a warp walk together
     uint8_t *p;
     int lane;
-    __device__ void bytes(const uint8_t *src, int len, bool upper = false)
+    __device__ void bytes(const uint8_t *src, int len, bool upper = false, uint8_t cap = 0)
     {
         for (int j = lane; j < len; j += 32) {
             uint8_t c = src[j];
             if (upper && (uint8_t)(c - 'a') < 26) c = (uint8_t)(c & ~0x20);
+            if (c < cap) c = cap;
             p[j] = c;
         }
         p += len;
@@ -697,6 +705,7 @@ struct InfoArgs {
     const int32_t *qtrim;        // quality-trimmed interval of the record (the read the cutter saw), or null
     const int32_t *seq_len;
     int has_qual;                // 0: FASTA input, the quality columns are empty (adapters.py:408-415, steps.py:250)
+    int zero_cap;                // ZeroCapper's cap of the qualities of reads without a match (as written); 0 = off
 };
 
 template <class Sink>
@@ -752,7 +761,7 @@ __device__ void info_rows(const InfoArgs &a, long long r, Sink &out)
         name();
         out.ch('\t'); out.ch('-'); out.ch('1');
         out.ch('\t'); out.bytes(a.buf + m.seq_start + start, left, a.upper_unmatched != 0);
-        out.ch('\t'); out.bytes(a.buf + m.qual_start + start, a.has_qual ? left : 0);
+        out.ch('\t'); out.bytes(a.buf + m.qual_start + start, a.has_qual ? left : 0, false, (uint8_t)a.zero_cap);
         out.ch('\n');
     }
 }
@@ -1178,18 +1187,20 @@ cudaError_t cg_launch_fastq_finish(long long n_records, const CgFastqRecord *d_r
 cudaError_t cg_launch_fastq_write(const uint8_t *d_buf, const CgFastqRecord *d_rec, const int32_t *d_interval,
                                   const int64_t *d_out_off, const int32_t *d_out_len, long long n_records,
                                   uint8_t *d_out, int action, const int32_t *d_keep_interval, const int32_t *d_mask,
-                                  int rc_suffix, cudaStream_t st, int fasta_out, const int32_t *d_route, int fasta_dests)
+                                  int rc_suffix, cudaStream_t st, int fasta_out, const int32_t *d_route, int fasta_dests,
+                                  int zero_cap)
 {
     if (n_records <= 0) return cudaSuccess;
     long long grid = (n_records + 7) / 8;
     grid = cg_grid_cap(grid, 16);
     if (fasta_out)
         fq_write_kernel<true><<<(unsigned)grid, 256, 0, st>>>(d_buf, d_rec, d_interval, d_out_off, d_out_len, n_records, d_out,
-                                                              action, d_keep_interval, d_mask, rc_suffix, d_route, fasta_dests);
+                                                              action, d_keep_interval, d_mask, rc_suffix, d_route, fasta_dests,
+                                                              zero_cap);
     else
         fq_write_kernel<false><<<(unsigned)grid, 256, 0, st>>>(d_buf, d_rec, d_interval, d_out_off, d_out_len, n_records, d_out,
                                                                action, d_keep_interval, d_mask, rc_suffix, d_route,
-                                                               fasta_dests);
+                                                               fasta_dests, zero_cap);
     return cudaGetLastError();
 }
 
@@ -1267,11 +1278,11 @@ cudaError_t cg_launch_fastq_info(int phase, const uint8_t *d_buf, const CgFastqR
                                  int slots, const uint8_t *d_names, const int32_t *d_name_off, int revcomp, int rc_suffix,
                                  int upper_unmatched, long long n_records, int32_t *d_row_bytes, const int64_t *d_row_off,
                                  uint8_t *d_out, cudaStream_t st, int kind, const int32_t *d_qtrim, const int32_t *d_seq_len,
-                                 int has_qual)
+                                 int has_qual, int zero_cap)
 {
     if (n_records <= 0) return cudaSuccess;
     InfoArgs a;
-    a.kind = kind; a.qtrim = d_qtrim; a.seq_len = d_seq_len; a.has_qual = has_qual;
+    a.kind = kind; a.qtrim = d_qtrim; a.seq_len = d_seq_len; a.has_qual = has_qual; a.zero_cap = zero_cap;
     a.buf = d_buf; a.rec = d_rec; a.origin = d_origin; a.interval = d_interval; a.mask = d_mask; a.matches = d_matches;
     a.times = times; a.slots = slots; a.names = d_names; a.name_off = d_name_off; a.revcomp = revcomp;
     a.rc_suffix = rc_suffix; a.upper_unmatched = upper_unmatched;

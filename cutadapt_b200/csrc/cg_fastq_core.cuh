@@ -23,6 +23,8 @@ struct CgFastqFilter {
     int trim_n;              // NEndTrimmer
     int discard_casava;      // CasavaFiltered
     int action;              // CG_FQ_ACTION_*: AdapterCutter's action
+    double max_aer = 0.0;    // TooHighAverageErrorRate: expected errors per base above this fail; 0 = off
+    int zero_cap = 0;        // ZeroCapper: quality characters below this one (the quality base) become it; 0 = off
 };
 #define CG_FQ_ACTION_TRIM 0
 #define CG_FQ_ACTION_NONE 1
@@ -30,7 +32,7 @@ struct CgFastqFilter {
 #define CG_FQ_ACTION_LOWERCASE 3
 #define CG_FQ_ACTION_RETAIN 4
 #define CG_FQ_ACTION_CROP 5
-// fail_mask word of a record: bits 0-6 failed filters, bits 8-29 adapter of the most recent match + 1,
+// fail_mask word of a record: bits 0-7 failed filters, bits 8-29 adapter of the most recent match + 1,
 // bit 30: the record was replaced by its reverse complement (--revcomp)
 #define CG_FQ_MASK_RC (1 << 30)
 #define CG_FQ_MASK_ADAPTER(mask) ((((mask) >> 8) & 0x3FFFFF) - 1)
@@ -167,7 +169,9 @@ struct FqVerdict {
 // PolyATrimmer, Shortener, NEndTrimmer after the adapters) and which filters it fails, one bit per filter in the
 // order cli.py:700-830 + 870-910 appends them:
 //   bit 0 TooShort, 1 TooLong (predicates.py:29-53), 2 TooManyN (96-122), 3 TooManyExpectedErrors (56-71),
-//   4 CasavaFiltered (125-139), 5 IsTrimmed (--discard-trimmed), 6 IsUntrimmed (--discard-untrimmed).
+//   4 CasavaFiltered (125-139), 5 IsTrimmed (--discard-trimmed), 6 IsUntrimmed (--discard-untrimmed),
+//   7 TooHighAverageErrorRate (74-95; it comes after bit 3 in the chain, see fq_finish_core).
+// ZeroCapper (modifiers.py:806-822) runs last, after NEndTrimmer: the quality filters see the capped characters.
 // Every predicate is evaluated (a pair filter may need the verdict of a filter that the mate passes).
 // `matches`: the times * slots records of THIS read (or nullptr); (qs, qe): its quality-trimmed interval.
 CG_HD FqVerdict fq_evaluate_core(const uint8_t *buf, const CgFastqRecord &rec, int n, const cg_match_rec *matches,
@@ -288,11 +292,14 @@ CG_HD FqVerdict fq_evaluate_core(const uint8_t *buf, const CgFastqRecord &rec, i
                                             : (double)n_count > f.max_n;
         if (too_many) mask |= 4;
     }
-    if (f.max_ee >= 0.0) {
-        // expected_errors(qualities) with its default base 33
-        const double ee = expected_errors_core(buf + rec.qual_start + start, left, 33, phred);
+    if (f.max_ee >= 0.0 || f.max_aer > 0.0) {
+        // expected_errors(qualities) with its default base 33, once for both filters
+        const double ee = expected_errors_core(buf + rec.qual_start + start, left, 33, phred, f.zero_cap);
         if (ee < 0.0) v.bad_quality = true;
-        else if (ee > f.max_ee) mask |= 8;
+        else {
+            if (f.max_ee >= 0.0 && ee > f.max_ee) mask |= 8;
+            if (f.max_aer > 0.0 && left > 0 && ee / (double)left > f.max_aer) mask |= 128;
+        }
     }
     if (f.discard_casava) {
         // name.partition(" ")[2][1:4] == ":Y:"
@@ -308,13 +315,15 @@ CG_HD FqVerdict fq_evaluate_core(const uint8_t *buf, const CgFastqRecord &rec, i
     return v;
 }
 
-// The verdict on a read (pair == false) or a pair: the first enabled filter, in chain order, that fires, or -1.
+// The verdict on a read (pair == false) or a pair: the first enabled filter, in chain order, that fires (its bit
+// number), or -1.  Chain order (cli.py:700-830): bits 0, 1, 2, 3, 7, 4, 5, 6.
 // PairedEndFilter (steps.py:105-180): a filter given for one mate only tests that mate; otherwise mode 0 "any",
 // 1 "both", 2 "first" (mode_untrimmed: cli.py:859-893 overrides the mode of --discard-untrimmed to "both" when only one
 // mate has adapters).
 CG_HD int fq_finish_core(int m1, int m2, bool pair, int enabled1, int enabled2, int mode, int mode_untrimmed)
 {
-    for (int k = 0; k < 7; ++k) {
+    for (int i = 0; i < 8; ++i) {
+        const int k = i < 4 ? i : (i == 4 ? 7 : i - 1);
         const int bit = 1 << k;
         const bool e1 = (enabled1 & bit) != 0, e2 = pair && (enabled2 & bit) != 0;
         if (!e1 && !e2) continue;

@@ -92,7 +92,8 @@ cudaError_t cg_launch_unpack3(const uint8_t *d_packed, long long packed_bytes, u
 // ---- FASTQ chunk parse / trimmed-record formatting (cg_fastq.cu) ---------------------------------------
 #include "cg_fastq_core.cuh"   // CgFastqRecord, CgFastqFilter, CG_FQ_ACTION_*, the per-record logic
 #define CG_FQ_COUNTERS 16    // written, bp_in, bp_out, with_adapters, too_short, too_long, quality_trimmed_bp,
-                             // discarded (trimmed/untrimmed), too_many_n, too_many_expected_errors, casava_filtered
+                             // discarded (trimmed/untrimmed), too_many_n, too_many_expected_errors, casava_filtered,
+                             // reverse_complemented, too_high_average_error_rate
 long long cg_fastq_tiles(long long n_bytes);
 long long cg_scan_tiles(long long n);
 // phase 0: newline count per tile + exclusive scan (total -> *d_total); phase 1: positions of the newlines
@@ -131,7 +132,7 @@ cudaError_t cg_launch_fastq_pretrim(const uint8_t *d_buf, const CgFastqRecord *d
                                     long long n_records, int flags, int cutoff_front, int cutoff_back, int qbase,
                                     int32_t *d_qtrim, cudaStream_t st);
 // kept interval + one bit per filter the read fails (bit order: too short, too long, too many N, too many expected
-// errors, casava, trimmed, untrimmed; CG_FQ_MASK_RC from d_is_rc); per-read counters (with_adapters, quality_trimmed_bp)
+// errors, casava, trimmed, untrimmed, too high average error rate; CG_FQ_MASK_RC from d_is_rc); per-read counters (with_adapters, quality_trimmed_bp)
 cudaError_t cg_launch_fastq_evaluate(const uint8_t *d_buf, const CgFastqRecord *d_rec, const int32_t *d_seq_len,
                                      long long n_records, const cg_match_rec *d_matches, int times, int slots,
                                      const int32_t *d_qtrim, CgFastqFilter f, const double *d_phred, const uint8_t *d_is_rc,
@@ -157,12 +158,13 @@ cudaError_t cg_launch_fastq_finish(long long n_records, const CgFastqRecord *d_r
                                    unsigned long long *d_counters2, int mode, int mode_untrimmed, int rc_suffix,
                                    const int32_t *d_dest, const uint8_t *d_dest_keep, cudaStream_t st, int fasta_out = 0,
                                    int redirect = 0, int fasta_dests = 0, int32_t *d_route = nullptr);
-// d_route (may be null): write only the records whose destination's bit in fasta_dests equals fasta_out
+// d_route (may be null): write only the records whose destination's bit in fasta_dests equals fasta_out; zero_cap:
+// quality characters below it are written as it (ZeroCapper), 0 = off
 cudaError_t cg_launch_fastq_write(const uint8_t *d_buf, const CgFastqRecord *d_rec, const int32_t *d_interval,
                                   const int64_t *d_out_off, const int32_t *d_out_len, long long n_records,
                                   uint8_t *d_out, int action, const int32_t *d_keep_interval, const int32_t *d_mask,
                                   int rc_suffix, cudaStream_t st, int fasta_out = 0, const int32_t *d_route = nullptr,
-                                  int fasta_dests = 0);
+                                  int fasta_dests = 0, int zero_cap = 0);
 // demultiplexing: cg_launch_fastq_dest gives every record its destination (adapter of the most recent match of R1, or
 // of both mates: d1 * (n_named2 + 1) + d2; reads without a match: the last value of the dimension); phase 0 fills
 // d_bytes[n_dest][tiles] (output bytes per destination and tile of 256 records); after an exclusive scan of that
@@ -180,7 +182,8 @@ cudaError_t cg_launch_fastq_info(int phase, const uint8_t *d_buf, const CgFastqR
                                  int upper_unmatched, long long n_records, int32_t *d_row_bytes, const int64_t *d_row_off,
                                  uint8_t *d_out, cudaStream_t st, int kind = 0, const int32_t *d_qtrim = nullptr,
                                  const int32_t *d_seq_len = nullptr,    // kind 1 / 2: --rest-file / --wildcard-file rows
-                                 int has_qual = 1);                     // 0: FASTA input, empty quality columns
+                                 int has_qual = 1,                      // 0: FASTA input, empty quality columns
+                                 int zero_cap = 0);                     // ZeroCapper on the rows of unmatched reads
 // interleaved input: phase 0 = per record of the chunk its span (d_start, d_size), mate (d_dest = r & 1) and name
 // (d_rec; FASTQ: from the line index d_nl_pos, format checked; FASTA, d_nl_pos == nullptr: d_rec is the normalised
 // chunk's record table), then the mate-name check per pair; d_err: first problem, record << 32 | code.  After the

@@ -167,8 +167,9 @@ struct CgSelectTables {
 // Trim statistics vector (cg_stats_accumulate_device; the payload of the end-of-run all-reduce):
 //   [0] n_reads  [1] total_bp  [2] reads_with_adapters  [3] quality_trimmed_bp  [4] bp_removed_by_adapters
 //   [5] reverse_complemented  [6] n_written  [7] bp_written  [8..14] filtered[7]: too_short, too_long,
-//   too_many_n, too_many_expected_errors, casava_filtered, discard_trimmed, discard_untrimmed  [15] reserved
-//       ([5..14] belong to steps outside the match records -- ReverseComplementer, the filters, the writer -- and are
+//   too_many_n, too_many_expected_errors, casava_filtered, discard_trimmed, discard_untrimmed
+//   [15] too_high_average_error_rate (filtered, but not in filtered[7]: the reference's report does not list it)
+//       ([5..15] belong to steps outside the match records -- ReverseComplementer, the filters, the writer -- and are
 //        filled by whoever runs those steps; they are part of the vector so that ONE all-reduce carries everything
 //        Statistics.__iadd__ adds up, report.py:81-126)
 //   [16 .. 16 + max_len]   read-length histogram: final length of every read after all trimming

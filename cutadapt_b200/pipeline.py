@@ -33,7 +33,7 @@ from .adapters import Matchable, MultipleAdapters
 STAT_N_READS, STAT_TOTAL_BP, STAT_WITH_ADAPTERS, STAT_QUALITY_TRIMMED_BP, STAT_ADAPTER_BP = 0, 1, 2, 3, 4
 STAT_REVERSE_COMPLEMENTED, STAT_N_WRITTEN, STAT_BP_WRITTEN, STAT_FILTERED = 5, 6, 7, 8
 FILTER_NAMES = ("too_short", "too_long", "too_many_n", "too_many_expected_errors", "casava_filtered", "discard_trimmed",
-                "discard_untrimmed")
+                "discard_untrimmed", "too_high_average_error_rate")     # slots STAT_FILTERED .. STAT_FILTERED + 7
 _SCALARS, _ADJ = 16, 8
 
 
@@ -215,7 +215,7 @@ def allreduce_statistics(stats, group=None):
 
 FASTQ_COUNTERS = ("n_records", "n_written", "bp_in", "bp_out", "out_bytes", "with_adapters", "quality_trimmed_bp",
                   "too_short", "too_long", "too_many_n", "too_many_expected_errors", "discarded", "casava_filtered",
-                  "reverse_complemented")
+                  "reverse_complemented", "too_high_average_error_rate")
 
 
 def allreduce_fastq_statistics(statistics: dict, group=None, device=None) -> dict:
@@ -979,7 +979,7 @@ def _fastq_params(times=1, quality_cutoff=None, quality_base=33, nextseq_cutoff=
                   maximum_length=None, max_n=None, max_expected_errors=None, discard_trimmed=False,
                   discard_untrimmed=False, cut=(), poly_a=False, length=None, trim_n=False,
                   discard_casava=False, action="trim", revcomp=False, rc_suffix=True, input_format="fastq",
-                  output_format=None) -> "_lib.cg_fastq_params":
+                  output_format=None, max_average_error_rate=None, zero_cap=False) -> "_lib.cg_fastq_params":
     fp = _lib.cg_fastq_params()
     fp.format = _format_code(input_format, output_format)
     fp.trim = _lib.make_params(
@@ -1008,6 +1008,12 @@ def _fastq_params(times=1, quality_cutoff=None, quality_base=33, nextseq_cutoff=
         raise ValueError("'retain' and 'crop' cannot be combined with times > 1")     # modifiers.py:117-118
     fp.action = actions[action]
     fp.revcomp = 0 if not revcomp else (1 if rc_suffix else 2)
+    if max_average_error_rate is not None:
+        rate = float(max_average_error_rate)
+        if not 0.0 < rate < 1.0:                                                         # predicates.py:81-85
+            raise ValueError(f"max_error_rate must be between 0.0 and 1.0, got {rate}.")
+        fp.max_average_error_rate = rate
+    fp.zero_cap = int(bool(zero_cap))
     return fp
 
 
@@ -1161,6 +1167,10 @@ class FastqTrimmer:
     times               -n                                                   (modifiers.py:225-231)
     minimum_length, maximum_length   -m / -M                                 (predicates.py:29-53)
     max_n, max_expected_errors       --max-n / --max-ee                      (predicates.py:56-122)
+    max_average_error_rate           --max-aer: expected errors per base     (predicates.py:74-95), counted in
+                                     ``too_high_average_error_rate``
+    zero_cap            -z: quality characters below quality_base are written as quality_base, last in the modifier
+                        chain, so the quality filters see them capped (ZeroCapper, modifiers.py:806-822)
     discard_trimmed, discard_untrimmed                                       (predicates.py:127-160)
     cut                 -u values (UnconditionalCutter, modifiers.py:66-95), applied first
     poly_a, length, trim_n           --poly-a / --length / --trim-n, after the adapters (modifiers.py:861-918)
@@ -1208,11 +1218,13 @@ class FastqTrimmer:
                  input_format: str = "fastq", output_format: Optional[str] = None,
                  ctx: Optional[_lib.Context] = None, collect_statistics: bool = False,
                  redirect: Sequence[str] = (), redirect_formats: Optional[dict] = None,
-                 gzip_outputs: Sequence[str] = (), rows: Sequence[str] = (), gzip_rows: Sequence[str] = ()):
+                 gzip_outputs: Sequence[str] = (), rows: Sequence[str] = (), gzip_rows: Sequence[str] = (),
+                 max_average_error_rate: Optional[float] = None, zero_cap: bool = False):
         self.rows, self.gzip_rows = _row_kinds(rows, gzip_rows)
         self.params = _fastq_params(times, quality_cutoff, quality_base, nextseq_cutoff, minimum_length, maximum_length,
                                     max_n, max_expected_errors, discard_trimmed, discard_untrimmed, cut, poly_a, length,
-                                    trim_n, discard_casava, action, revcomp, rc_suffix, input_format, output_format)
+                                    trim_n, discard_casava, action, revcomp, rc_suffix, input_format, output_format,
+                                    max_average_error_rate, zero_cap)
         self.gzip_outputs = tuple(dict.fromkeys(gzip_outputs or ()))
         self.params.gzip_outputs = _gzip_bits(self.gzip_outputs)
         self.redirect = tuple(dict.fromkeys(redirect or ()))
@@ -1431,10 +1443,10 @@ class PairedFastqTrimmer:
     Paired-end FASTQ chunks (``PairedEndPipeline.process_reads``, pipeline.py:125-153): record i of the two
     chunks is one pair.  ``adapters1`` / ``adapters2`` are the -a / -A adapters (None or [] for none),
     ``options1`` / ``options2`` dicts with FastqTrimmer's keyword arguments for each mate (-q / -Q, -u / -U,
-    -l / -L ...; filters such as ``minimum_length`` or ``discard_trimmed`` go into both unless the command
-    line gives them for one mate only).  ``pair_filter`` is "any" (default), "both" or "first"
-    (PairedEndFilter, steps.py:105-180).  ``input_format`` / ``output_format`` as for FastqTrimmer, for both
-    mates (read_paired_fasta_chunks).  ``process_chunk(chunk1, chunk2) -> (bytes, bytes)``;
+    -l / -L ...; ``max_average_error_rate`` and ``zero_cap`` go into both, as on the command line; filters such as
+    ``minimum_length`` or ``discard_trimmed`` go into both unless the command line gives them for one mate only).
+    ``pair_filter`` is "any" (default), "both" or "first" (PairedEndFilter, steps.py:105-180).  ``input_format`` /
+    ``output_format`` as for FastqTrimmer, for both mates (read_paired_fasta_chunks).  ``process_chunk(chunk1, chunk2) -> (bytes, bytes)``;
     ``statistics`` = (dict for R1, dict for R2).  ``collect_statistics``: as for FastqTrimmer, one accumulator per
     mate; ``statistics_vector()``, ``adapter_statistics()``, ``poly_a_trimmed_lengths`` and ``written_lengths`` give
     one value per mate.  ``redirect`` / ``redirect_formats``: as for FastqTrimmer, both mates of a removed pair go to

@@ -300,8 +300,8 @@ int cg_poly_a_trim_batch(cg_ctx *ctx, const uint8_t *seq, const int64_t *offsets
  * The per-chunk worker of the reference as one call: WorkerProcess.run (runners.py:174-214) parses a chunk of
  * complete 4-line records (dnaio.read_chunks, runners.py:116-126), runs the modifiers per read
  * (pipeline.py:47-73, in the order cli.py:937-975 builds them: UnconditionalCutter, NextseqQualityTrimmer,
- * QualityTrimmer, AdapterCutter with its action, PolyATrimmer, Shortener, NEndTrimmer), the filters
- * (TooShort, TooLong, TooManyN, TooManyExpectedErrors, CasavaFiltered, then DiscardTrimmed /
+ * QualityTrimmer, AdapterCutter with its action, PolyATrimmer, Shortener, NEndTrimmer, ZeroCapper), the filters
+ * (TooShort, TooLong, TooManyN, TooManyExpectedErrors, TooHighAverageErrorRate, CasavaFiltered, then DiscardTrimmed /
  * DiscardUntrimmed: predicates.py:29-160 in the order of cli.py:700-830) and formats the surviving records
  * ("@name\nsequence\n+\nqualities\n", SingleEndSink steps.py:299-319).  Here the chunk is indexed, packed,
  * trimmed, filtered and formatted on the device; it crosses PCIe once in each direction.
@@ -337,6 +337,13 @@ typedef struct cg_fastq_params {
     int32_t stats;               /* 0 = off, else a handle of cg_fastq_stats_create: the call ADDS this mate's
                                     statistics to that accumulator if it succeeds (cg_fastq_stats_read, below) */
     int32_t gzip_outputs;        /* CG_GZIP_MAIN / CG_REDIRECT_* bits: the outputs written as gzip (below); 0 = plain */
+    double max_average_error_rate; /* --max-aer (TooHighAverageErrorRate, predicates.py:74-95): a read of length > 0 is
+                                    removed when expected errors / length > this rate (FP64); 0 = off, else it must lie
+                                    in (0, 1).  Its count: cg_fastq_result.too_high_average_error_rate          */
+    int32_t zero_cap;            /* -z / --zero-cap (ZeroCapper, modifiers.py:806-822), the last modifier: quality
+                                    characters below trim.quality_base become trim.quality_base, for the filters and in
+                                    every output; info rows of reads with a match keep the original qualities.  0 / 1 */
+    int32_t reserved_pad;        /* 0 */
 } cg_fastq_params;
 typedef struct cg_fastq_result {
     int64_t n_records, n_written;
@@ -346,7 +353,7 @@ typedef struct cg_fastq_result {
     int64_t too_short, too_long, too_many_n, too_many_expected_errors, discarded, casava_filtered;
     int64_t reverse_complemented; /* --revcomp: reads replaced by their reverse complement             */
     int64_t out_bytes_plain;     /* size of the same outputs uncompressed (== out_bytes without gzip outputs) */
-    int64_t reserved[1];
+    int64_t too_high_average_error_rate; /* reads (pairs) removed by --max-aer                               */
 } cg_fastq_result;
 /* Formats (cg_fastq_params.format; both mates of a pair must have the same one, else CG_EINVAL):
  *   CG_FORMAT_FASTQ           FASTQ in, FASTQ out (zeroed parameters)
@@ -360,8 +367,9 @@ typedef struct cg_fastq_result {
  * record).  Rejected with CG_EINVAL, the message naming the line (1-based, within the chunk): any other line in front
  * of the first header (an empty one included), and a '#' line after the first header (the reference's test vectors
  * do not say what dnaio does with it).  A chunk must start at a header or at those comments.  FASTA has no qualities:
- * with CG_FORMAT_FASTA, quality_trim, nextseq_trim and max_expected_errors >= 0 are CG_EINVAL (the reference's CLI drops
- * --max-ee with a warning, cli.py:756-760; that is the caller's decision), the info-file rows have empty quality
+ * with CG_FORMAT_FASTA, quality_trim, nextseq_trim, max_expected_errors >= 0, max_average_error_rate != 0 and zero_cap are
+ * CG_EINVAL (the reference's CLI drops --max-ee and --max-aer with a warning, cli.py:756-776; that is the caller's
+ * decision), the info-file rows have empty quality
  * columns (adapters.py:408-415, steps.py:250).  FASTA output is ">name\nsequence\n", the sequence on one line.  It can
  * be LARGER than the input: a record without sequence line (">a" plus a line break) is written as ">a\n\n", so the
  * output of a FASTA chunk is at most 1.5 x its size plus 2 bytes; FASTQ -> FASTA output is never larger than the
@@ -622,8 +630,8 @@ int cg_fastq_collect_paired_interleaved(cg_ctx *ctx, int32_t slot1, int32_t slot
  *   [0] n_reads  [1] total_bp  [2] reads_with_adapters  [3] quality_trimmed_bp  [4] bp_removed_by_adapters
  *   [5] reverse_complemented  [6] n_written  [7] bp_written
  *   [8..14] filtered: too_short, too_long, too_many_n, too_many_expected_errors, casava_filtered, discard_trimmed,
- *           discard_untrimmed   [15] reserved
- *       ([5..14] are produced by steps outside the match records; this function leaves them alone)
+ *           discard_untrimmed   [15] too_high_average_error_rate
+ *       ([5..15] are produced by steps outside the match records; this function leaves them alone)
  *   [16 .. 16 + max_len]  read-length histogram after trimming (ReadLengthStatistics, statistics.py:5-48)
  *   then per adapter a and end e (0: matches removing what precedes them, 1: what follows them), i.e. the two
  *   EndStatistics of AdapterStatistics.end_statistics() (adapters.py:142-289):
@@ -657,7 +665,7 @@ int cg_process_batch_stats(cg_ctx *ctx, const cg_adapterset *set, const uint8_t 
  * Vector (int64): the cg_stats_* layout below at (n_adapters, max_len, kmax), with
  *   [0] n_records [1] bp_in [2] with_adapters [3] quality_trimmed_bp [4] bases removed by the adapter matches
  *   [5] reverse_complemented [6] n_written [7] bp_out [8..14] the filter counts of the result struct; discarded goes
- *   to [13] with discard_trimmed, else to [14]
+ *   to [13] with discard_trimmed, else to [14]; [15] too_high_average_error_rate
  *   read-length histogram: WRITTEN records by written length, all outputs of a demultiplexing call together (pairs
  *   dropped through dest_keep are not counted)
  *   per adapter and end: every match of every read that went through the cutter, filtered or not; adjacent bases

@@ -246,6 +246,10 @@ def main():
                     help="read and/or write interleaved paired-end reads (one input file, or no -p)")
     ap.add_argument("--max-n", type=float, default=None)
     ap.add_argument("--max-ee", type=float, default=None)
+    ap.add_argument("--max-average-error-rate", "--max-aer", dest="max_aer", type=float, default=None,
+                    help="remove reads whose expected errors per base exceed this rate (0 < rate < 1)")
+    ap.add_argument("-z", "--zero-cap", action="store_true",
+                    help="change negative quality values to zero (characters below --quality-base)")
     ap.add_argument("--length", "-l", type=int, default=None)
     ap.add_argument("--poly-a", action="store_true")
     ap.add_argument("--trim-n", action="store_true")
@@ -294,6 +298,13 @@ def main():
     if input_format == "fasta" and args.max_ee is not None:
         print("WARNING: Ignoring option --max-ee because input does not provide quality values", file=sys.stderr)
         args.max_ee = None
+    if input_format == "fasta" and args.max_aer is not None:
+        print("WARNING: Ignoring option --max-aer because input does not provide quality values", file=sys.stderr)
+        args.max_aer = None
+    if input_format == "fasta" and args.zero_cap:
+        ap.error("-z/--zero-cap needs quality values; the input is FASTA")
+    if args.max_aer is not None and not 0.0 < args.max_aer < 1.0:
+        ap.error(f"max_error_rate must be between 0.0 and 1.0, got {args.max_aer}.")
     host_reader = read_fasta_chunks if input_format == "fasta" else read_fastq_chunks
     # compressed bytes per submission of a device-inflated input: one thread inflates a member, so a submission must hold
     # many members; with --buffer-size 64 MiB, members of up to 1 MiB give 64 or more at once
@@ -317,7 +328,8 @@ def main():
                   minimum_length=min1, maximum_length=max1, max_n=args.max_n,
                   max_expected_errors=args.max_ee, discard_trimmed=args.discard_trimmed,
                   discard_untrimmed=args.discard_untrimmed, cut=args.cut, poly_a=args.poly_a, length=args.length,
-                  trim_n=args.trim_n, discard_casava=args.discard_casava, action=args.action)
+                  trim_n=args.trim_n, discard_casava=args.discard_casava, action=args.action,
+                  max_average_error_rate=args.max_aer, zero_cap=args.zero_cap)
     formats = dict(input_format=input_format, output_format=output_format, collect_statistics=args.json is not None)
     # filter outputs (the untrimmed output of a demultiplexer is its "unknown" output)
     redirect = [d for d, _ in FILTER_OUTPUTS if getattr(args, d + "_output") and "{name}" not in args.output]
