@@ -3586,6 +3586,89 @@ static int fastq_stage_pair_adapters(cg_ctx *c, FastqSlot &f1, FastqSlot &f2, co
     return fastq_stage_verdict(c, f2, fp2, 2, st, g2);
 }
 
+// PairedReverseComplementer (modifiers.py:311-400) for a chunk of pairs, at least one set given.  Each mate's own
+// modifiers in front of the cutters (-u, --nextseq-trim, -q) are folded into its records; then up to four trimming
+// passes: m11 = set1 on slot 1, m22 = set2 on slot 2, m12 = set1 on slot 2, m21 = set2 on slot 1 (a cross pass is laid
+// out for its set, so a slot's matches keep its own set's layout after the swap).  Each slot's chunk gets the other
+// slot's chunk appended, and fq_pair_swap_kernel moves the records of the swapped pairs across.  From there on the
+// pair is written, filtered, routed and counted like any other.
+static int fastq_stage_paired_revcomp(cg_ctx *c, FastqSlot &f1, FastqSlot &f2, const cg_adapterset *s1,
+                                      const cg_adapterset *s2, const cg_fastq_params *fp1, const cg_fastq_params *fp2,
+                                      cudaStream_t st, FqStage &g1, FqStage &g2)
+{
+    int rc;
+    if ((rc = fastq_stage_records(c, f1, fp1, s1 != nullptr, st, g1)) != CG_OK) return rc;
+    if ((rc = fastq_stage_records(c, f2, fp2, s2 != nullptr, st, g2)) != CG_OK) return rc;
+    if (g1.n != g2.n || g1.n == 0) return CG_OK;       // the caller reports the mismatch
+    const long long n = g1.n;
+    const int64_t b1 = f1.n_bytes, b2 = f2.n_bytes;
+    if (b1 + b2 > (int64_t)UINT32_MAX)
+        return fail(CG_EINVAL, "--revcomp on pairs: the two chunks of a pair must hold less than 4 GiB together");
+    g1.slots = s1 ? s1->host.slots : 1;
+    g2.slots = s2 ? s2->host.slots : 1;
+    const int per1 = g1.times * g1.slots, per2 = g2.times * g2.slots;
+    if ((rc = fastq_stage_fold_qtrim(c, f1, &fp1->trim, st, g1)) != CG_OK) return rc;
+    if ((rc = fastq_stage_fold_qtrim(c, f2, &fp2->trim, st, g2)) != CG_OK) return rc;
+    if ((rc = fastq_stage_pack(c, f1, st, g1, false)) != CG_OK) return rc;
+    if ((rc = fastq_stage_pack(c, f2, st, g2, false)) != CG_OK) return rc;
+    cg_params p1 = fp1->trim, p2 = fp2->trim;
+    p1.quality_trim = p1.nextseq_trim = p2.quality_trim = p2.nextseq_trim = 0;
+    // slot 1: d_matches = m11, d_matches_rc = m21; slot 2: d_matches = m22, d_matches_rc = m12
+    if (s1) {
+        if ((rc = f1.d_matches.ensure((size_t)n * per1)) != CG_OK) return rc;
+        if ((rc = f2.d_matches_rc.ensure((size_t)n * per1)) != CG_OK) return rc;
+        if ((rc = launch_trim(c, s1, f1.d_seq.p, nullptr, f1.d_offs.p, n, g1.max_len, &p1, f1.d_matches.p, nullptr, st,
+                              true)) != CG_OK)
+            return rc;
+        if ((rc = launch_trim(c, s1, f2.d_seq.p, nullptr, f2.d_offs.p, n, g2.max_len, &p1, f2.d_matches_rc.p, nullptr, st,
+                              true)) != CG_OK)
+            return rc;
+    }
+    if (s2) {
+        if ((rc = f2.d_matches.ensure((size_t)n * per2)) != CG_OK) return rc;
+        if ((rc = f1.d_matches_rc.ensure((size_t)n * per2)) != CG_OK) return rc;
+        if ((rc = launch_trim(c, s2, f2.d_seq.p, nullptr, f2.d_offs.p, n, g2.max_len, &p2, f2.d_matches.p, nullptr, st,
+                              true)) != CG_OK)
+            return rc;
+        if ((rc = launch_trim(c, s2, f1.d_seq.p, nullptr, f1.d_offs.p, n, g1.max_len, &p2, f1.d_matches_rc.p, nullptr, st,
+                              true)) != CG_OK)
+            return rc;
+    }
+    // slot 1's chunk becomes [chunk1 | chunk2], slot 2's [chunk2 | chunk1]: the writers, the rows and the statistics
+    // then find a record that moved to the other slot in that slot's own chunk
+    if ((rc = f1.d_norm.ensure((size_t)(b1 + b2) + 64)) != CG_OK) return rc;
+    if ((rc = f2.d_norm.ensure((size_t)(b1 + b2) + 64)) != CG_OK) return rc;
+    if (b1) {
+        CU(cudaMemcpyAsync(f1.d_norm.p, f1.d_in.p, (size_t)b1, cudaMemcpyDeviceToDevice, st));
+        CU(cudaMemcpyAsync(f2.d_norm.p + b2, f1.d_in.p, (size_t)b1, cudaMemcpyDeviceToDevice, st));
+    }
+    if (b2) {
+        CU(cudaMemcpyAsync(f2.d_norm.p, f2.d_in.p, (size_t)b2, cudaMemcpyDeviceToDevice, st));
+        CU(cudaMemcpyAsync(f1.d_norm.p + b1, f2.d_in.p, (size_t)b2, cudaMemcpyDeviceToDevice, st));
+    }
+    std::swap(f1.d_in, f1.d_norm);
+    std::swap(f2.d_in, f2.d_norm);
+    f1.n_bytes = f2.n_bytes = b1 + b2;               // what the packed reads of either slot can now need
+    if ((rc = f1.d_isrc.ensure((size_t)n)) != CG_OK) return rc;
+    if ((rc = f2.d_isrc.ensure((size_t)n)) != CG_OK) return rc;
+    CU(cg_launch_fastq_pair_swap(n, f1.d_rec.p, f1.d_len.p, f1.d_origin.p, s1 ? f1.d_matches.p : nullptr,
+                                 s2 ? f1.d_matches_rc.p : nullptr, per1, f2.d_rec.p, f2.d_len.p, f2.d_origin.p,
+                                 s2 ? f2.d_matches.p : nullptr, s1 ? f2.d_matches_rc.p : nullptr, per2, (uint32_t)b1,
+                                 (uint32_t)b2, f1.d_isrc.p, f2.d_isrc.p, f1.d_counters.p + 1, f2.d_counters.p + 1, st));
+    c->launches += 1;
+    for (FqStage *g : {&g1, &g2}) {
+        g->d_is_rc = (g == &g1 ? f1 : f2).d_isrc.p;
+        g->rc_suffix = fp1->revcomp == 1;
+        g->packed = false;                           // the statistics pack the swapped reads again
+    }
+    g1.d_matches = s1 ? f1.d_matches.p : nullptr;
+    g2.d_matches = s2 ? f2.d_matches.p : nullptr;
+    if ((rc = fastq_stage_stats(c, f1, g1, s1 ? s1->host.max_k : 0, st)) != CG_OK) return rc;
+    if ((rc = fastq_stage_stats(c, f2, g2, s2 ? s2->host.max_k : 0, st)) != CG_OK) return rc;
+    if ((rc = fastq_stage_verdict(c, f1, fp1, 1, st, g1)) != CG_OK) return rc;
+    return fastq_stage_verdict(c, f2, fp2, 2, st, g2);
+}
+
 static int fastq_collect_paired_run(cg_ctx *c, int32_t slot1, int32_t slot2, const cg_adapterset *s1,
                                     const cg_adapterset *s2, const FqPairAdapters *pa, const cg_fastq_params *fp1,
                                     const cg_fastq_params *fp2, int32_t pair_filter_mode, uint8_t *out1,
@@ -3597,8 +3680,10 @@ static int fastq_collect_paired_run(cg_ctx *c, int32_t slot1, int32_t slot2, con
         slot1 == slot2 || pair_filter_mode < 0 || pair_filter_mode > 2)
         return fail(CG_EINVAL, "cg_fastq_collect_paired: bad argument");
     if ((s1 && s1->ctx != c) || (s2 && s2->ctx != c)) return fail(CG_EINVAL, "adapter set belongs to another context");
-    if (fp1->revcomp || fp2->revcomp)
-        return fail(CG_EINVAL, "--revcomp on pairs (PairedReverseComplementer) is not available on the device path");
+    if (fp1->revcomp != fp2->revcomp)
+        return fail(CG_EINVAL, "cg_fastq_collect_paired: --revcomp is one option for the pair, params1.revcomp and "
+                               "params2.revcomp must be equal");
+    if (pa && fp1->revcomp) return fail(CG_EINVAL, "Cannot use --revcomp with --pair-adapters");   // cli.py:1086-1087
     FastqSlot &f1 = c->fq[slot1], &f2 = c->fq[slot2];
     if (!f1.busy || !f2.busy) return fail(CG_EINVAL, "cg_fastq_collect_paired: nothing was submitted to a slot");
     if ((f1.ilv || f2.ilv) && (f1.ilv != 1 || f2.ilv != 2 || f1.ilv_peer != slot2 || f2.ilv_peer != slot1))
@@ -3644,11 +3729,18 @@ static int fastq_collect_paired_run(cg_ctx *c, int32_t slot1, int32_t slot2, con
     if ((rc = fastq_rows_check(f1, n_entries1, "cg_fastq_collect_paired (mate 1)")) != CG_OK ||
         (rc = fastq_rows_check(f2, n_entries2, "cg_fastq_collect_paired (mate 2)")) != CG_OK)
         return rc;
+    // the reference builds the info row of a swapped pair from R1's own input read with the coordinates of the match
+    // on r2 (steps.py:233-247); that row is not produced here
+    if (fp1->revcomp && (f1.rows[CG_ROWS_INFO].requested || f2.rows[CG_ROWS_INFO].requested))
+        return fail(CG_EINVAL, "cg_fastq_collect_paired: info rows (--info-file) cannot be combined with --revcomp on "
+                               "pairs; rest and wildcard rows can");
     if ((rc = fqstats_lookup(c, fp1->stats, n_entries1, &g1.acc)) != CG_OK ||
         (rc = fqstats_lookup(c, fp2->stats, n_entries2, &g2.acc)) != CG_OK)
         return rc;
     if (pa) {
         if ((rc = fastq_stage_pair_adapters(c, f1, f2, *pa, fp1, fp2, st, g1, g2)) != CG_OK) return rc;
+    } else if (fp1->revcomp && (s1 || s2)) {        // without adapters --revcomp does nothing (cli.py:1103-1110)
+        if ((rc = fastq_stage_paired_revcomp(c, f1, f2, s1, s2, fp1, fp2, st, g1, g2)) != CG_OK) return rc;
     } else {
         if ((rc = fastq_stage_evaluate(c, f1, s1, fp1, 1, st, g1)) != CG_OK) return rc;
         if ((rc = fastq_stage_evaluate(c, f2, s2, fp2, 2, st, g2)) != CG_OK) return rc;

@@ -412,6 +412,51 @@ __global__ void __launch_bounds__(256) fq_revcomp_commit_kernel(uint8_t *buf, Cg
     if (lane == 0 && replaced) atomicAdd(&counters[11], (unsigned long long)replaced);
 }
 
+// PairedReverseComplementer.__call__ (modifiers.py:311-400), one thread per pair: fq_pair_swap_core decides; a swapped
+// pair exchanges its record-table entries, lengths and origins between the slots (R1's output then writes r2, R2's
+// writes r1), and each slot takes the matches its own cutter found on the read it now holds (m11 <- m12, m22 <- m21),
+// so that every later kernel works on the swapped pair without knowing about it.  Each slot's chunk holds the other
+// slot's chunk behind its own (base1 / base2: the size of slot 1's / slot 2's own chunk), so a record that moves is
+// rebased by the size of its new slot's own chunk.  is_rc of both slots; counters[11] of both += swapped pairs.
+__global__ void fq_pair_swap_kernel(long long n_pairs, CgFastqRecord *rec1, int32_t *len1, int32_t *origin1,
+                                    cg_match_rec *m11, const cg_match_rec *m21, int per1, CgFastqRecord *rec2,
+                                    int32_t *len2, int32_t *origin2, cg_match_rec *m22, const cg_match_rec *m12, int per2,
+                                    uint32_t base1, uint32_t base2, uint8_t *is_rc1, uint8_t *is_rc2,
+                                    unsigned long long *counters1, unsigned long long *counters2)
+{
+    const long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    bool swap = false;
+    if (p < n_pairs) {
+        swap = fq_pair_swap_core(m11 ? m11 + p * per1 : nullptr, m22 ? m22 + p * per2 : nullptr,
+                                 m12 ? m12 + p * per1 : nullptr, m21 ? m21 + p * per2 : nullptr, per1, per2);
+        is_rc1[p] = is_rc2[p] = swap;
+        if (swap) {
+            CgFastqRecord a = rec1[p], b = rec2[p];
+            b.hdr_start += base1; b.seq_start += base1; b.qual_start += base1;
+            a.hdr_start += base2; a.seq_start += base2; a.qual_start += base2;
+            rec1[p] = b;
+            rec2[p] = a;
+            const int32_t l = len1[p];
+            len1[p] = len2[p];
+            len2[p] = l;
+            for (int k = 0; k < 2; ++k) {
+                const int32_t o = origin1[2 * p + k];
+                origin1[2 * p + k] = origin2[2 * p + k];
+                origin2[2 * p + k] = o;
+            }
+            if (m11)
+                for (int k = 0; k < per1; ++k) m11[p * per1 + k] = m12[p * per1 + k];
+            if (m22)
+                for (int k = 0; k < per2; ++k) m22[p * per2 + k] = m21[p * per2 + k];
+        }
+    }
+    const unsigned w = __reduce_add_sync(0xFFFFFFFFu, swap ? 1u : 0u);
+    if ((threadIdx.x & 31) == 0 && w) {
+        atomicAdd(&counters1[11], (unsigned long long)w);
+        atomicAdd(&counters2[11], (unsigned long long)w);
+    }
+}
+
 // quality-driven trimming only (no adapter set): NextseqQualityTrimmer + QualityTrimmer straight on the chunk
 __global__ void fq_pretrim_kernel(const uint8_t *buf, const CgFastqRecord *rec, const int32_t *seq_len, long long n_records,
                                   int flags, int cutoff_front, int cutoff_back, int qbase, int32_t *qtrim)
@@ -1117,6 +1162,19 @@ cudaError_t cg_launch_fastq_revcomp_commit(uint8_t *d_buf, CgFastqRecord *d_rec,
     grid = cg_grid_cap(grid, 16);
     fq_revcomp_commit_kernel<<<(unsigned)grid, 256, 0, st>>>(d_buf, d_rec, d_seq_len, d_origin, n_records, d_matches,
                                                              d_matches_rc, per_read, d_is_rc, d_counters, has_qual);
+    return cudaGetLastError();
+}
+
+cudaError_t cg_launch_fastq_pair_swap(long long n_pairs, CgFastqRecord *d_rec1, int32_t *d_len1, int32_t *d_origin1,
+                                      cg_match_rec *d_m11, const cg_match_rec *d_m21, int per1, CgFastqRecord *d_rec2,
+                                      int32_t *d_len2, int32_t *d_origin2, cg_match_rec *d_m22, const cg_match_rec *d_m12,
+                                      int per2, uint32_t base1, uint32_t base2, uint8_t *d_is_rc1, uint8_t *d_is_rc2,
+                                      unsigned long long *d_counters1, unsigned long long *d_counters2, cudaStream_t st)
+{
+    if (n_pairs <= 0) return cudaSuccess;
+    fq_pair_swap_kernel<<<(unsigned)((n_pairs + 255) / 256), 256, 0, st>>>(
+        n_pairs, d_rec1, d_len1, d_origin1, d_m11, d_m21, per1, d_rec2, d_len2, d_origin2, d_m22, d_m12, per2, base1, base2,
+        d_is_rc1, d_is_rc2, d_counters1, d_counters2);
     return cudaGetLastError();
 }
 

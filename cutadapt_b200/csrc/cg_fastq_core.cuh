@@ -338,6 +338,24 @@ CG_HD int fq_finish_core(int m1, int m2, bool pair, int enabled1, int enabled2, 
     return -1;
 }
 
+// PairedReverseComplementer's decision (modifiers.py:311-400) for one pair: the score of a pairing is the sum of the
+// scores of every record with adapter >= 0 (all rounds, both parts of a linked match).  m11 / m22: cutter1 on r1 and
+// cutter2 on r2 (per1 / per2 records each); m12 / m21: cutter1 on r2 and cutter2 on r1.  A missing cutter passes
+// nullptr for its two arrays and scores 0.  The swapped pairing wins only if its score is strictly greater.
+CG_HD long long fq_match_score(const cg_match_rec *m, int per)
+{
+    long long s = 0;
+    if (m)
+        for (int k = 0; k < per; ++k)
+            if (m[k].adapter >= 0) s += m[k].score;
+    return s;
+}
+CG_HD bool fq_pair_swap_core(const cg_match_rec *m11, const cg_match_rec *m22, const cg_match_rec *m12,
+                             const cg_match_rec *m21, int per1, int per2)
+{
+    return fq_match_score(m12, per1) + fq_match_score(m21, per2) > fq_match_score(m11, per1) + fq_match_score(m22, per2);
+}
+
 // Do two headers (without '@' / '>') name the two mates of one pair?  The rule of dnaio's paired readers
 // (doc/reference.rst:925-950): compare the IDs, each header up to its first space or tab; a final '1', '2' or '3' of the
 // IDs is ignored, so "read1/1 some text" matches "read1/2 other text", but "my_read/1;1" does not match "my_read/2;1".

@@ -128,6 +128,13 @@ cudaError_t cg_launch_fastq_revcomp_commit(uint8_t *d_buf, CgFastqRecord *d_rec,
                                            long long n_records, cg_match_rec *d_matches, const cg_match_rec *d_matches_rc,
                                            int per_read, uint8_t *d_is_rc, unsigned long long *d_counters, cudaStream_t st,
                                            int has_qual = 1);
+// --revcomp on pairs: decide every pair, swap the records and matches of the swapped ones between the two slots
+// (counters[11] of both += swapped pairs)
+cudaError_t cg_launch_fastq_pair_swap(long long n_pairs, CgFastqRecord *d_rec1, int32_t *d_len1, int32_t *d_origin1,
+                                      cg_match_rec *d_m11, const cg_match_rec *d_m21, int per1, CgFastqRecord *d_rec2,
+                                      int32_t *d_len2, int32_t *d_origin2, cg_match_rec *d_m22, const cg_match_rec *d_m12,
+                                      int per2, uint32_t base1, uint32_t base2, uint8_t *d_is_rc1, uint8_t *d_is_rc2,
+                                      unsigned long long *d_counters1, unsigned long long *d_counters2, cudaStream_t st);
 cudaError_t cg_launch_fastq_pretrim(const uint8_t *d_buf, const CgFastqRecord *d_rec, const int32_t *d_seq_len,
                                     long long n_records, int flags, int cutoff_front, int cutoff_back, int qbase,
                                     int32_t *d_qtrim, cudaStream_t st);

@@ -521,8 +521,8 @@ class PairedRevcompBatch:
     ``--revcomp`` on pairs (PairedReverseComplementer, modifiers.py:311-400): four batched passes -- every mate against
     both adapter lists -- and ``paired_revcomp_select``.  ``process(seqs1, seqs2)`` returns (swapped[n], TrimResult of
     the new R1, TrimResult of the new R2); the caller writes old R2 as new R1 for a swapped pair and appends the
-    name suffix.  (The FASTQ kernels do the single-end form, ``FastqTrimmer(revcomp=True)``; this is the record-level
-    composition for pairs.)
+    name suffix.  (The FASTQ kernels do both forms, ``FastqTrimmer(revcomp=True)`` and
+    ``PairedFastqTrimmer(revcomp=True)``; this is the record-level composition for callers that work with records.)
     """
 
     def __init__(self, adapters1: Optional[Sequence], adapters2: Optional[Sequence], ctx: Optional[_lib.Context] = None):
@@ -1468,6 +1468,13 @@ class PairedFastqTrimmer:
     PairedInfoFileWriter, steps.py:256-269); ``gzip_rows`` / ``gzip_rows2`` the kinds compressed (default for R2: those
     of ``gzip_rows`` it has).  Every chunk method leaves ``last_rows`` = {kind: (bytes of R1, bytes of R2)}, b"" for a
     mate without that kind.  With ``pair_adapters`` the info rows name adapter i of each mate's own list.
+
+    ``revcomp`` / ``rc_suffix``: --revcomp for the pair (PairedReverseComplementer, modifiers.py:311-400), on the
+    device.  After each mate's own -u / --nextseq-trim / -q, the -a set also runs on R2 and the -A set on R1; a pair
+    whose swapped matches score strictly more is written swapped: R1's output gets R2's read trimmed by the -a set, R2's
+    output gets R1's read trimmed by the -A set, both names with " rc" unless rc_suffix is False.  Without adapters it
+    does nothing.  ``statistics[k]["reverse_complemented"]`` counts the swapped pairs; each adapter's
+    ``reverse_complemented`` its matches in swapped pairs.  Not with ``pair_adapters`` or info rows.
     """
 
     MODES = {"any": 0, "both": 1, "first": 2}
@@ -1479,17 +1486,27 @@ class PairedFastqTrimmer:
                  redirect: Sequence[str] = (), redirect_formats: Optional[dict] = None,
                  interleaved_outputs: Sequence[str] = (), gzip_outputs: Sequence[str] = (),
                  gzip_outputs2: Optional[Sequence[str]] = None, rows: Sequence[str] = (),
-                 rows2: Sequence[str] = (), gzip_rows: Sequence[str] = (), gzip_rows2: Optional[Sequence[str]] = None):
+                 rows2: Sequence[str] = (), gzip_rows: Sequence[str] = (), gzip_rows2: Optional[Sequence[str]] = None,
+                 revcomp: bool = False, rc_suffix: bool = True):
         if pair_filter not in self.MODES:
             raise ValueError("pair_filter must be 'any', 'both' or 'first'")
+        for options in (options1, options2):
+            for key in ("revcomp", "rc_suffix"):
+                if key in (options or {}):
+                    raise ValueError(f"--revcomp is one option for the pair: pass {key}= to PairedFastqTrimmer, "
+                                     "not in options1 / options2")
+        if revcomp and "info" in tuple(rows or ()) + tuple(rows2 or ()):
+            raise ValueError("info rows (--info-file) cannot be combined with --revcomp on pairs")
         self.rows, self.gzip_rows = _row_kinds(rows, gzip_rows)
         if gzip_rows2 is None:
             gzip_rows2 = [k for k in self.gzip_rows if k in (rows2 or ())]
         self.rows2, self.gzip_rows2 = _row_kinds(rows2, gzip_rows2, "rows2")
         self.last_rows = {}
-        formats = dict(input_format=input_format, output_format=output_format)
+        formats = dict(input_format=input_format, output_format=output_format, revcomp=revcomp, rc_suffix=rc_suffix)
         self.params1 = _fastq_params(**{**(options1 or {}), **formats})
         self.params2 = _fastq_params(**{**(options2 or {}), **formats})
+        if pair_adapters and revcomp:
+            raise ValueError("Cannot use --revcomp with --pair-adapters")            # cli.py:1087
         self.params1.gzip_outputs = _gzip_bits(gzip_outputs)
         self.params2.gzip_outputs = _gzip_bits(gzip_outputs if gzip_outputs2 is None else gzip_outputs2)
         self.redirect = tuple(dict.fromkeys(redirect or ()))
@@ -1517,8 +1534,6 @@ class PairedFastqTrimmer:
                                  f"Given: {len(adapters1)} for R1, {len(adapters2)} for R2")
             if not adapters1:
                 raise ValueError("No adapters given")
-            if self.params1.revcomp or self.params2.revcomp:
-                raise ValueError("Cannot use --revcomp with --pair-adapters")        # cli.py:1087
             self.adapters1, self.adapters2 = adapters1, adapters2
             self._pairs = [(_device_set([a1], self.ctx)[1], _device_set([a2], self.ctx)[1])
                            for a1, a2 in zip(adapters1, adapters2)]
@@ -1603,10 +1618,17 @@ class PairedFastqTrimmer:
         self.last_rows = {k: (r1.get(k, b""), r2.get(k, b"")) for k in ROW_KINDS if k in r1 or k in r2}
 
     def _out_buffers(self, tickets, n_dest: int = 4):
-        """Output buffers of a pair: out1 also holds R2 of the interleaved outputs."""
+        """Output buffers of a pair: out1 also holds R2 of the interleaved outputs.  With --revcomp either mate's output
+        can receive the other mate's records, each with " rc" (3 bytes on a FASTQ record of at least 6)."""
         (_, b1), (_, b2) = tickets
-        n1 = _output_capacity(b1.size, self.params1.format, self.params1.gzip_outputs != 0, n_dest)
-        n2 = _output_capacity(b2.size, self.params2.format, self.params2.gzip_outputs != 0, n_dest)
+        if self.params1.revcomp:
+            both = b1.size + b2.size
+            n_in = both + both // 2 if self.params1.format == _lib.CG_FORMAT_FASTQ else both
+            n1 = _output_capacity(n_in, self.params1.format, self.params1.gzip_outputs != 0, n_dest, True)
+            n2 = _output_capacity(n_in, self.params2.format, self.params2.gzip_outputs != 0, n_dest, True)
+        else:
+            n1 = _output_capacity(b1.size, self.params1.format, self.params1.gzip_outputs != 0, n_dest)
+            n2 = _output_capacity(b2.size, self.params2.format, self.params2.gzip_outputs != 0, n_dest)
         return np.empty(n1 + (n2 if self._interleave else 0), dtype=np.uint8), np.empty(n2, dtype=np.uint8)
 
     def _no_interleave(self, what: str):

@@ -329,10 +329,15 @@ typedef struct cg_fastq_params {
     int32_t trim_n;              /* --trim-n (NEndTrimmer, modifiers.py:902-918)                      */
     int32_t discard_casava;      /* --discard-casava (CasavaFiltered, predicates.py:125-139)          */
     int32_t action;              /* CG_ACTION_*: --action of the AdapterCutter (modifiers.py:236-249)   */
-    int32_t revcomp;             /* --revcomp (ReverseComplementer, modifiers.py:264-308; single-end collects): the
+    int32_t revcomp;             /* --revcomp.  Single-end collects (ReverseComplementer, modifiers.py:264-308): the
                                     adapters are searched on the read and on its reverse complement, the better
-                                    orientation is kept.  1 = append " rc" to the name of a replaced read, 2 = do not
-                                    (--rename given, cli.py:1082-1116)                                  */
+                                    orientation is kept.  Paired collects (PairedReverseComplementer, modifiers.py:
+                                    311-400; both mates' values must be equal, not with --pair-adapters): each mate's
+                                    set also runs on the other mate's read, and a pair whose swapped matches score
+                                    strictly more is written swapped (R1's output gets r2 trimmed by the -a set, R2's
+                                    gets r1 trimmed by the -A set); no info rows then.  1 = append " rc" to the name
+                                    of a replaced read (both mates of a swapped pair), 2 = do not (--rename given,
+                                    cli.py:1082-1116)                                                   */
     int32_t format;              /* CG_FORMAT_*: what the chunk is and what is written (below); 0 = FASTQ    */
     int32_t stats;               /* 0 = off, else a handle of cg_fastq_stats_create: the call ADDS this mate's
                                     statistics to that accumulator if it succeeds (cg_fastq_stats_read, below) */
@@ -351,7 +356,8 @@ typedef struct cg_fastq_result {
     int64_t out_bytes;           /* size of the formatted output                                      */
     int64_t with_adapters, quality_trimmed_bp;
     int64_t too_short, too_long, too_many_n, too_many_expected_errors, discarded, casava_filtered;
-    int64_t reverse_complemented; /* --revcomp: reads replaced by their reverse complement             */
+    int64_t reverse_complemented; /* --revcomp: reads replaced by their reverse complement; pairs: the swapped
+                                     pairs, in both mates' results                                      */
     int64_t out_bytes_plain;     /* size of the same outputs uncompressed (== out_bytes without gzip outputs) */
     int64_t too_high_average_error_rate; /* reads (pairs) removed by --max-aer                               */
 } cg_fastq_result;

@@ -38,6 +38,8 @@ tool's rule (prefixes of the reads compressed as one member of about 4 to 64 MiB
 three rounds alternating) and the smallest size from which the device wins at every larger size.  Last lines: the
 inflate kernels' device time per MiB of plain output from torch.profiler, in runs of their own, on the multi-member
 input and on the split stream.  The card's name and power limit are read in the run.
+--revcomp [n_reads] [chunk_megabytes]: the "paired" variant without and with --revcomp (the pair swap on the device), the
+two arms alternating over three rounds in one process; pairs per second of each and the card's name and power limit.
 --rows [n_reads] [chunk_megabytes] [--baseline-tree DIR]: the "paired" variant with the info rows of both mates
 (--info-file and --info-file-paired), four arms alternating over three rounds in one process: no rows, plain rows, rows
 compressed on the device (gzip_rows), and plain rows compressed by host zlib level 1 (one stream per mate, one thread).
@@ -403,7 +405,48 @@ def measure_rows(n, chunk_mb, baseline_tree=None):
                       "median": {k: sorted(v)[len(v) // 2] for k, v in runs.items()}}))
 
 
+def measure_paired_revcomp(n, chunk_mb):
+    """--revcomp: the "paired" variant without and with --revcomp (PairedReverseComplementer on the device), the two arms
+    alternating over three rounds in one process; host-to-host pairs per second of each."""
+    n -= n % 2
+    data, rec_len = build_fastq(n, pair_names=True)
+    per_chunk = max(2, max(1, (chunk_mb << 20) // rec_len) // 2 * 2)
+    mates = [np.ascontiguousarray(data.reshape(n // 2, 2, rec_len)[:, k]).reshape(-1) for k in (0, 1)]
+    mates = [torch.from_numpy(m).pin_memory().numpy() for m in mates]
+    half = per_chunk // 2
+    chunks = [tuple(m[i * rec_len:min(n // 2, i + half) * rec_len] for m in mates) for i in range(0, n // 2, half)]
+    adapters = [PA.BackAdapter("AGATCGGAAGAGC", max_errors=0.1, name="adapter")]
+    opts = dict(quality_cutoff=(0, 20), minimum_length=20)
+    arms = {"paired": PairedFastqTrimmer(adapters, adapters, opts, opts),
+            "paired_revcomp": PairedFastqTrimmer(adapters, adapters, opts, opts, revcomp=True)}
+
+    def run(name, cs):
+        return sum(len(a) + len(b) for parts in arms[name].process_chunks_split(cs) for a, b in parts.values())
+
+    for name in arms:
+        run(name, chunks[:3])                     # warm-up: buffers, module load
+    res = {name: {"wall_s": 0.0} for name in arms}
+    for _ in range(3):
+        for name in arms:
+            t0 = time.perf_counter()
+            res[name]["out_bytes"] = run(name, chunks)
+            res[name]["wall_s"] += time.perf_counter() - t0
+    for name, r in res.items():
+        r["pairs_per_s"] = 3 * (n // 2) / r["wall_s"]
+        r["reverse_complemented"] = int(arms[name].statistics[0].get("reverse_complemented", 0))
+    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader",
+                           "-i", str(torch.cuda.current_device())], capture_output=True, text=True).stdout.strip()
+    print(json.dumps({"what": "paired FASTQ (-a/-A AGATCGGAAGAGC -q 20 -m 20), host to host, without and with --revcomp",
+                      "pairs": n // 2, "chunk_mb": chunk_mb, "chunks": len(chunks), "gpu": torch.cuda.get_device_name(),
+                      "card_and_power_limit": card, "arms": res,
+                      "revcomp_over_plain_time": res["paired_revcomp"]["wall_s"] / res["paired"]["wall_s"]}))
+
+
 def main():
+    if "--revcomp" in sys.argv:
+        argv = [a for a in sys.argv if a != "--revcomp"]
+        return measure_paired_revcomp(int(argv[1]) if len(argv) > 1 else 4_000_000,
+                                      int(argv[2]) if len(argv) > 2 else 64)
     if "--rows" in sys.argv:
         argv = [a for a in sys.argv if a != "--rows"]
         base = None

@@ -12,6 +12,7 @@ command line (no reports): it shows the per-chunk worker of INTEGRATION.md secti
       -o out.fastq in.fastq                                                            (filter outputs)
   python tools/trim_fastq.py --interleaved -a ADAPT1 -A ADAPT2 -m 20:25 -o out.fastq in.interleaved.fastq
   python tools/trim_fastq.py -a AGATCGGAAGAGC -o out.fastq.gz in.fastq.gz                   (gzip)
+  python tools/trim_fastq.py --revcomp -g ^TTATTTGTCT -G ^TCCGCACTGG -o out.1.fastq -p out.2.fastq in.1.fastq in.2.fastq
   python tools/trim_fastq.py -a ADAPT1 -A ADAPT2 --info-file info1.txt.gz --info-file-paired info2.txt.gz \
       -o out.1.fastq -p out.2.fastq in.1.fastq in.2.fastq                               (per-read row files)
 
@@ -39,6 +40,11 @@ input of at least 16 MiB (DEVICE_GZIP_SPLIT_MIN; the single member that gzip and
 block-parallel (split_members=True).  Smaller ones are decompressed on the host with Python's gzip module.  The outputs are the same either way; the stderr line's "in_bytes_gzip" (the
 compressed bytes consumed) appears only when the device inflated the input.  The format is detected from the first
 decompressed byte.
+
+--revcomp / --rc: the adapters are also searched on the reverse complement of each read and the better orientation
+is written, " rc" appended to its name (ReverseComplementer).  On pairs the -a adapters also run on R2 and the -A
+adapters on R1, and a pair that matches better that way is written with R1 and R2 swapped, " rc" on both names
+(PairedReverseComplementer); --info-file is refused there.  --json counts them in "reverse_complemented".
 
 Row files: --info-file, -r/--rest-file and --wildcard-file get the rows of every read, filtered or not, formatted on the
 device next to every kind of output above.  On pairs they get R1's rows, as in the reference (PairedSingleEndStep,
@@ -257,6 +263,8 @@ def main():
     ap.add_argument("--discard-trimmed", action="store_true")
     ap.add_argument("--discard-untrimmed", action="store_true")
     ap.add_argument("--action", default="trim", choices=["trim", "none", "mask", "lowercase", "retain", "crop"])
+    ap.add_argument("--revcomp", "--rc", action="store_true",
+                    help="also search the adapters on the reverse complement (pairs: with R1 and R2 swapped)")
     ap.add_argument("--pair-filter", default="any", choices=["any", "both", "first"])
     ap.add_argument("--fasta", action="store_true", help="write FASTA even for FASTQ input")
     ap.add_argument("--buffer-size", type=int, default=64 << 20)
@@ -292,6 +300,9 @@ def main():
     min1, min2 = mate_lengths(ap, args.minimum_length, paired)
     max1, max2 = mate_lengths(ap, args.maximum_length, paired)
     check_filter_outputs(ap, args, paired, "{name}" in args.output, args.interleaved)
+    if paired and args.revcomp and (args.info_file or args.info_file2):
+        ap.error("--info-file cannot be combined with --revcomp on paired-end data: the info rows of swapped pairs are "
+                 "not produced")
     input_format = detect_format(args.inputs[0])
     fasta_out = file_format(args.output, input_format, args.fasta) == "fasta"
     output_format = "fasta" if fasta_out and input_format == "fastq" else None
@@ -331,6 +342,7 @@ def main():
                   trim_n=args.trim_n, discard_casava=args.discard_casava, action=args.action,
                   max_average_error_rate=args.max_aer, zero_cap=args.zero_cap)
     formats = dict(input_format=input_format, output_format=output_format, collect_statistics=args.json is not None)
+    revcomp1 = {} if paired else dict(revcomp=args.revcomp)
     # filter outputs (the untrimmed output of a demultiplexer is its "unknown" output)
     redirect = [d for d, _ in FILTER_OUTPUTS if getattr(args, d + "_output") and "{name}" not in args.output]
     split = dict(redirect=redirect,
@@ -372,7 +384,7 @@ def main():
         # an output is interleaved when its paired path is missing (cli.py:650-661, 913-921)
         interleaved = [d for d in ["output"] + redirect
                        if not (args.paired_output if d == "output" else getattr(args, d + "_paired_output"))]
-        t = PairedFastqTrimmer(ads1, ads2, common, options2, args.pair_filter, **formats, **split,
+        t = PairedFastqTrimmer(ads1, ads2, common, options2, args.pair_filter, **formats, **split, revcomp=args.revcomp,
                                interleaved_outputs=interleaved, gzip_outputs=gzip1, gzip_outputs2=gzip2, **rows,
                                rows2=tuple(row_paths2),
                                gzip_rows2=[k for k, p in row_paths2.items() if p.endswith(".gz")])
@@ -410,7 +422,7 @@ def main():
         # every demultiplexed output, "unknown" included, is compressed alike
         if args.untrimmed_output and args.untrimmed_output.endswith(".gz") != args.output.endswith(".gz"):
             ap.error("with demultiplexing, --untrimmed-output must be compressed (.gz) exactly when the -o template is")
-        t = FastqTrimmer(ads1, **common, **formats, gzip_outputs=gzip1, **rows)
+        t = FastqTrimmer(ads1, **common, **formats, **revcomp1, gzip_outputs=gzip1, **rows)
         files = {}
         f, chunks = single_input(t)
         with f:
@@ -429,7 +441,7 @@ def main():
             fh.close()
         stats = t.statistics
     elif redirect:
-        t = FastqTrimmer(ads1, **common, **formats, **split, gzip_outputs=gzip1, **rows)
+        t = FastqTrimmer(ads1, **common, **formats, **revcomp1, **split, gzip_outputs=gzip1, **rows)
         f, chunks = single_input(t)
         with f:
             files = {d: OutputFile(getattr(args, d + "_output")) for d in redirect}
@@ -442,7 +454,7 @@ def main():
                 fh.close()
         stats = t.statistics
     else:
-        t = FastqTrimmer(ads1, **common, **formats, gzip_outputs=gzip1, **rows)
+        t = FastqTrimmer(ads1, **common, **formats, **revcomp1, gzip_outputs=gzip1, **rows)
         o = OutputFile(args.output)
         f, chunks = single_input(t)
         with f:
