@@ -37,6 +37,7 @@ CG_GROUP_INDEXED = 2
 CG_FORMAT_FASTQ = 0              # cg_fastq_params.format: FASTQ in, FASTQ out
 CG_FORMAT_FASTA = 1              # FASTA in, FASTA out
 CG_FORMAT_FASTQ_TO_FASTA = 2     # FASTQ in, FASTA out
+CG_FORMAT_BAM = 3                # cg_fastq_submit_gzip only: unaligned BAM in, its records as FASTQ text in the slot
 CG_GZIN_SPLIT_MEMBERS = 1        # cg_gzin_create_ex: long members inflated block-parallel, consumed in part
 CG_GZIN_LONG_MEMBER = 64 * 1024  # compressed bytes above which a split stream takes a member block-parallel
 CG_GZIN_STRIDE = 64 * 1024       # compressed bytes between speculative chunk starts
@@ -231,6 +232,7 @@ def _declare(lib) -> None:
     lib.cg_gzin_create_ex.argtypes = [vp, i32, C.POINTER(i32)]
     lib.cg_fastq_slot_read.argtypes = [vp, i32, vp, i64, C.POINTER(i64)]
     lib.cg_gzin_destroy.argtypes = [vp, i32]
+    lib.cg_gzin_bam_tiles.argtypes = [vp, i32, C.POINTER(i64), C.POINTER(i64)]
     lib.cg_fastq_submit_gzip.argtypes = [vp, i32, vp, i64, i32, i32, C.POINTER(i32), C.POINTER(cg_gzin_result)]
     lib.cg_fastq_submit_gzip_paired.argtypes = [vp, i32, i32, vp, i64, vp, i64, i32, i32, C.POINTER(i32), C.POINTER(i32),
                                                 C.POINTER(cg_gzin_result), C.POINTER(cg_gzin_result)]

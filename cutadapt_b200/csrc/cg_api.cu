@@ -199,6 +199,20 @@ struct GzinStream {
     DevBuf<uint16_t> d_sym;
     DevBuf<int32_t> d_redo;
     DevBuf<uint32_t> d_part;
+    // the format of the stream's first committed submission: -1 none yet, 0 FASTQ / FASTA, 1 CG_FORMAT_BAM
+    int bam = -1;
+    // CG_FORMAT_BAM: whether the header was read and dropped; the offset of d_plain[0] in the decompressed stream and the
+    // records cut so far (for the messages); the tiles of the boundary walk and those walked again, over the stream's life
+    bool bam_hdr = false;
+    long long bam_base = 0, bam_records = 0, bam_tiles = 0, bam_rewalked = 0;
+    DevBuf<uint32_t> d_bm, d_start;
+    DevBuf<uint64_t> d_link;
+    DevBuf<long long> d_entry;
+    DevBuf<int32_t> d_wcnt, d_fsize;
+    DevBuf<int64_t> d_woff, d_foff;
+    DevBuf<BamSum> d_sum;
+    DevBuf<unsigned long long> d_berr;
+    DevBuf<uint8_t> d_rest;
     ~GzinStream() { if (done) cudaEventDestroy(done); }   // not copyable, as its buffers are not
 };
 
@@ -1771,10 +1785,9 @@ static int fastq_slot_upload(cg_ctx *c, FastqSlot &f, const uint8_t *fastq, int6
 // The argument checks of a submit: `ok` holds the caller's own, then up to two byte buffers and the format; `what` names
 // a buffer in the size message.
 static int submit_check(const char *who, bool ok, int32_t format, const char *what, const uint8_t *p1, int64_t n1,
-                        const uint8_t *p2 = nullptr, int64_t n2 = 0)
+                        const uint8_t *p2 = nullptr, int64_t n2 = 0, int32_t max_format = CG_FORMAT_FASTQ_TO_FASTA)
 {
-    if (!ok || n1 < 0 || n2 < 0 || (n1 && !p1) || (n2 && !p2) || format < CG_FORMAT_FASTQ ||
-        format > CG_FORMAT_FASTQ_TO_FASTA)
+    if (!ok || n1 < 0 || n2 < 0 || (n1 && !p1) || (n2 && !p2) || format < CG_FORMAT_FASTQ || format > max_format)
         return fail(CG_EINVAL, std::string(who) + ": bad argument");
     if (n1 >= (1LL << 31) || n2 >= (1LL << 31))
         return fail(CG_EINVAL, std::string(who) + ": a " + what + " must be smaller than 2 GiB");
@@ -2273,6 +2286,7 @@ static int gzin_commit(cg_ctx *c, GzinStream &g, FastqSlot *f, long long cut, lo
     g.consumed += g.pend_consumed;
     g.members += g.pend_members;
     g.pend_plain = g.pend_consumed = g.pend_members = 0;
+    if (g.bam < 0) g.bam = 0;
     if (g.split) {
         g.mem = g.pmem;
         if (g.mem.in) std::swap(g.d_win, g.d_pwin);
@@ -2290,13 +2304,180 @@ static GzinStream *gzin_lookup(cg_ctx *c, int32_t handle)
     return it == c->gzin.end() ? nullptr : &it->second;
 }
 
+// A stream keeps the format class (BAM or not) of its first committed submission
+static int gzin_format_check(const GzinStream &g, int32_t format, const char *who)
+{
+    const int bam = format == CG_FORMAT_BAM;
+    if (g.bam >= 0 && g.bam != bam)
+        return fail(CG_EINVAL, std::string(who) + ": the stream was " + (g.bam ? "BAM" : "FASTQ / FASTA") +
+                                   " input; a stream takes one format for its whole life");
+    return CG_OK;
+}
+
+// ------------------------------------------------------------------------------------------
+// BAM input (CG_FORMAT_BAM, cg_bam.cu): the inflated bytes behind the carry are the BAM stream.  The header is parsed on
+// the host from a readback of its bytes and dropped once whole; the record boundaries come from the tile walk, and the
+// records of the cut are written as FASTQ text into the slot.  The BAM bytes behind the cut become the carry.
+// ------------------------------------------------------------------------------------------
+static int bam_fail(int code, long long record, long long at, const std::string &what)
+{
+    return fail(code, "BAM input: record " + std::to_string(record) + " (at byte " + std::to_string(at) +
+                          " of the decompressed stream): " + what);
+}
+
+// The header of d_plain[0, total) on the host: *hdr its size once whole (0 while it is not and not final).
+static int bam_header_read(GzinStream &g, long long total, bool final, cudaStream_t st, long long *hdr)
+{
+    *hdr = 0;
+    std::vector<uint8_t> h;
+    for (long long want = 65536;; want *= 2) {
+        const long long m = std::min(want, total);
+        h.resize((size_t)m);
+        if (m) CU(cudaMemcpyAsync(h.data(), g.d_plain.p, (size_t)m, cudaMemcpyDeviceToHost, st));
+        CU(cudaStreamSynchronize(st));
+        int why = 0;
+        const int s = bam_header(h.data(), m, hdr, &why);
+        if (s == BAM_BAD)
+            return fail(CG_EINVAL, why == BAM_H_MAGIC ? "BAM input: not a BAM file (the decompressed stream does not "
+                                                        "start with BAM\\1)"
+                                                      : "BAM input: not a BAM file (a negative length in the header)");
+        if (s == BAM_OK) return CG_OK;
+        if (m == total) break;
+    }
+    *hdr = 0;
+    if (final) return fail(CG_EINVAL, "BAM input: the file ends inside the BAM header");
+    return CG_OK;
+}
+
+static const char *bam_what(int code)
+{
+    switch (code) {
+    case BAM_R_FLAG: return "flag is not 4 (an unmapped single read); only unaligned single-end BAM is read";
+    case BAM_R_NAME: return "a read name byte outside '!'..'~'";
+    case BAM_R_NOQUAL: return "the record has no quality values (first quality byte 0xFF)";
+    case BAM_R_QUAL: return "a quality value above 93";
+    default: return "block_size, l_read_name, n_cigar_op and l_seq do not fit together, or the name lacks its NUL";
+    }
+}
+
+// The BAM submission after gzin_inflate: cut, emit into slot f, commit.  *cut_bytes: the FASTQ bytes in the slot.
+static int gzin_bam(cg_ctx *c, GzinStream &g, FastqSlot &f, bool fin, cudaStream_t st, cg_gzin_result *res,
+                    long long *cut_bytes)
+{
+    int rc;
+    *cut_bytes = 0;
+    const long long total = g.carry + g.pend_plain;
+    long long s0 = 0;                          // header bytes in front of the records
+    if (!g.bam_hdr) {
+        if ((rc = bam_header_read(g, total, fin, st, &s0)) != CG_OK) return rc;
+        if (!s0) {                             // the header waits in the carry
+            g.carry = total;
+            g.consumed += g.pend_consumed;
+            g.members += g.pend_members;
+            g.pend_plain = g.pend_consumed = g.pend_members = 0;
+            g.bam = 1;
+            if (g.split) {
+                g.mem = g.pmem;
+                if (g.mem.in) std::swap(g.d_win, g.d_pwin);
+            }
+            CU(cudaEventRecord(g.done, st));
+            res->carry_bytes = g.carry;
+            return CG_OK;
+        }
+    }
+    const uint8_t *b = g.d_plain.p + s0;
+    const long long n = total - s0, T = cg_bam_tiles(n), W = cg_bam_words(n), R = cg_bam_max_records(n);
+    if ((rc = g.d_bm.ensure((size_t)W + 1)) != CG_OK || (rc = g.d_link.ensure((size_t)T + 1)) != CG_OK ||
+        (rc = g.d_entry.ensure((size_t)T + 1)) != CG_OK || (rc = g.d_wcnt.ensure((size_t)W + 1)) != CG_OK ||
+        (rc = g.d_woff.ensure((size_t)W + 1)) != CG_OK || (rc = g.d_start.ensure((size_t)R)) != CG_OK ||
+        (rc = g.d_fsize.ensure((size_t)R)) != CG_OK || (rc = g.d_foff.ensure((size_t)R + 1)) != CG_OK ||
+        (rc = g.d_sum.ensure(1)) != CG_OK || (rc = g.d_berr.ensure(1)) != CG_OK ||
+        (rc = g.d_scan.ensure((size_t)cg_scan_tiles(std::max(W, R)) + 1)) != CG_OK)
+        return rc;
+    CU(cg_launch_bam_bounds(b, n, g.d_bm.p, g.d_link.p, g.d_entry.p, g.d_sum.p, g.d_wcnt.p, st));
+    CU(cg_launch_scan_i32(g.d_wcnt.p, W, g.d_scan.p, g.d_woff.p, st));
+    CU(cg_launch_bam_starts(b, n, g.d_bm.p, g.d_entry.p, g.d_sum.p, g.d_woff.p, g.d_start.p, g.d_fsize.p, st));
+    CU(cg_launch_scan_i32(g.d_fsize.p, R, g.d_scan.p, g.d_foff.p, st));
+    CU(cg_launch_bam_cut(g.d_woff.p, n, g.d_start.p, g.d_foff.p, CG_GZIN_LIMIT - 1, g.d_sum.p, st));
+    c->launches += 12;
+    BamSum sum;
+    CU(cudaMemcpyAsync(&sum, g.d_sum.p, sizeof sum, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    // the refusals of every record of the chain, the text of the cut's
+    if ((rc = f.d_in.ensure((size_t)sum.fq_bytes + 64)) != CG_OK) return rc;
+    const unsigned long long none = ~0ULL;
+    CU(cudaMemcpyAsync(g.d_berr.p, &none, sizeof none, cudaMemcpyHostToDevice, st));
+    CU(cg_launch_bam_emit(b, g.d_start.p, g.d_foff.p, sum.n_rec, sum.n_cut, f.d_in.p, g.d_berr.p, st));
+    c->launches += 1;
+    unsigned long long err = none;
+    CU(cudaMemcpyAsync(&err, g.d_berr.p, sizeof err, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    const long long at0 = g.bam_base + s0;
+    if (err != none) {
+        const long long i = (long long)(err >> 3);
+        const int code = (int)(err & 7);
+        uint32_t p = 0;
+        CU(cudaMemcpy(&p, g.d_start.p + i, sizeof p, cudaMemcpyDeviceToHost));
+        return bam_fail(code == BAM_R_FLAG || code == BAM_R_NOQUAL ? CG_EUNSUPPORTED : CG_EINVAL, g.bam_records + i,
+                        at0 + p, bam_what(code));
+    }
+    if (sum.end_st == BAM_BAD)
+        return bam_fail(CG_EINVAL, g.bam_records + sum.n_rec, at0 + sum.end, bam_what(BAM_R_STRUCT));
+    if (sum.end_st == BAM_SHORT && fin)
+        return fail(CG_EINVAL, "BAM input: BAM file ends inside record " + std::to_string(g.bam_records + sum.n_rec) +
+                                   " (at byte " + std::to_string(at0 + sum.end) + " of the decompressed stream)");
+    if (sum.n_cut == 0 && sum.n_rec > 0)
+        return bam_fail(CG_EUNSUPPORTED, g.bam_records, at0,
+                        "its FASTQ text alone reaches the 2 GiB limit of a chunk");
+    // commit: the BAM bytes behind the cut become the carry
+    const long long drop = s0 + sum.bam_cut, rest = total - drop;
+    if (drop) {
+        if ((rc = g.d_rest.ensure((size_t)rest + 64)) != CG_OK) return rc;
+        if (rest) CU(cudaMemcpyAsync(g.d_rest.p, g.d_plain.p + drop, (size_t)rest, cudaMemcpyDeviceToDevice, st));
+        std::swap(g.d_rest, g.d_plain);
+    }
+    if (sum.n_cut && (rc = fastq_slot_count(c, f, sum.fq_bytes)) != CG_OK) return rc;
+    g.bam_hdr = true;
+    g.bam_base += drop;
+    g.bam_records += sum.n_cut;
+    g.bam_tiles += T;
+    g.bam_rewalked += sum.rewalked;
+    g.carry = rest;
+    g.consumed += g.pend_consumed;
+    g.members += g.pend_members;
+    g.pend_plain = g.pend_consumed = g.pend_members = 0;
+    g.bam = 1;
+    if (g.split) {
+        g.mem = g.pmem;
+        if (g.mem.in) std::swap(g.d_win, g.d_pwin);
+    }
+    CU(cudaEventRecord(g.done, st));
+    res->chunk_bytes = sum.n_cut ? sum.fq_bytes : 0;
+    res->carry_bytes = g.carry;
+    res->n_records = sum.n_cut;
+    *cut_bytes = res->chunk_bytes;
+    return CG_OK;
+}
+
+extern "C" int cg_gzin_bam_tiles(cg_ctx *c, int32_t handle, int64_t *tiles, int64_t *rewalked)
+{
+    if (!c || !tiles || !rewalked) return fail(CG_EINVAL, "cg_gzin_bam_tiles: bad argument");
+    GzinStream *g = gzin_lookup(c, handle);
+    if (!g) return fail(CG_EINVAL, "cg_gzin_bam_tiles: unknown handle");
+    *tiles = g->bam_tiles;
+    *rewalked = g->bam_rewalked;
+    return CG_OK;
+}
+
 extern "C" int cg_fastq_submit_gzip(cg_ctx *c, int32_t handle, const uint8_t *gz, int64_t n_bytes, int32_t format,
                                     int32_t final, int32_t *slot, cg_gzin_result *res)
 {
-    int rc = submit_check("cg_fastq_submit_gzip", c && slot && res, format, "submission", gz, n_bytes);
+    int rc = submit_check("cg_fastq_submit_gzip", c && slot && res, format, "submission", gz, n_bytes, nullptr, 0,
+                          CG_FORMAT_BAM);
     if (rc != CG_OK) return rc;
     GzinStream *g = gzin_lookup(c, handle);
     if (!g) return fail(CG_EINVAL, "cg_fastq_submit_gzip: unknown handle");
+    if ((rc = gzin_format_check(*g, format, "cg_fastq_submit_gzip")) != CG_OK) return rc;
     CU(cudaSetDevice(c->device));
     *slot = -1;
     memset(res, 0, sizeof *res);
@@ -2306,6 +2487,12 @@ extern "C" int cg_fastq_submit_gzip(cg_ctx *c, int32_t handle, const uint8_t *gz
     bool fin = false;
     if ((rc = fastq_slot_init(c, f)) != CG_OK) return rc;
     if ((rc = gzin_inflate(c, *g, gz, n_bytes, final != 0, f.stream, res, &fin)) != CG_OK) return rc;
+    if (format == CG_FORMAT_BAM) {
+        long long cut = 0;
+        if ((rc = gzin_bam(c, *g, f, fin, f.stream, res, &cut)) != CG_OK) return rc;
+        if (cut) fq_take(c, si, slot);
+        return CG_OK;
+    }
     GzinCount k;
     if ((rc = gzin_count(c, *g, format == CG_FORMAT_FASTA, f.stream, &k)) != CG_OK) return rc;
     long long cut, n_records;
@@ -2340,6 +2527,7 @@ extern "C" int cg_fastq_submit_gzip_interleaved(cg_ctx *c, int32_t handle, const
     if (rc != CG_OK) return rc;
     GzinStream *g = gzin_lookup(c, handle);
     if (!g) return fail(CG_EINVAL, "cg_fastq_submit_gzip_interleaved: unknown handle");
+    if ((rc = gzin_format_check(*g, format, "cg_fastq_submit_gzip_interleaved")) != CG_OK) return rc;
     CU(cudaSetDevice(c->device));
     *slot1 = *slot2 = -1;
     memset(res, 0, sizeof *res);
@@ -2374,6 +2562,9 @@ extern "C" int cg_fastq_submit_gzip_paired(cg_ctx *c, int32_t handle1, int32_t h
     if (rc != CG_OK) return rc;
     GzinStream *g1 = gzin_lookup(c, handle1), *g2 = gzin_lookup(c, handle2);
     if (!g1 || !g2) return fail(CG_EINVAL, "cg_fastq_submit_gzip_paired: unknown handle");
+    if ((rc = gzin_format_check(*g1, format, "cg_fastq_submit_gzip_paired")) != CG_OK ||
+        (rc = gzin_format_check(*g2, format, "cg_fastq_submit_gzip_paired")) != CG_OK)
+        return rc;
     CU(cudaSetDevice(c->device));
     *slot1 = *slot2 = -1;
     memset(res1, 0, sizeof *res1);

@@ -257,6 +257,25 @@ cudaError_t cg_launch_gunzip_flags(const uint8_t *d_buf, long long n, const uint
                                    int32_t *d_flag, cudaStream_t st);
 cudaError_t cg_launch_gunzip_select(const uint32_t *d_nl, long long n_nl, const int32_t *d_flag, const int64_t *d_offs,
                                     long long s, long long *d_cut, cudaStream_t st);
+// unaligned BAM input (cg_bam.cu, decisions in cg_bam_core.cuh) on the records behind the header, d_buf[0, n): the
+// bounds (bitmap d_bm of cg_bam_words(n) words, link words and entries per tile of cg_bam_tiles(n), the chain's end in
+// *d_sum, record starts per bitmap word in d_cnt); after an exclusive scan of d_cnt (d_woff) the starts in order and
+// their FASTQ sizes (cg_bam_max_records(n) entries, zero behind the last); after an exclusive scan of those (d_foff) the
+// cut under `limit` FASTQ bytes; then the refusals of the chain's n_rec records (*d_err: record << 3 | BAM_R_*, start
+// it at ~0) and the FASTQ text of the first n_cut of them into d_out.
+#include "cg_bam_core.cuh"
+long long cg_bam_words(long long n);
+long long cg_bam_tiles(long long n);
+long long cg_bam_max_records(long long n);
+cudaError_t cg_launch_bam_bounds(const uint8_t *d_buf, long long n, uint32_t *d_bm, uint64_t *d_link, long long *d_entry,
+                                 BamSum *d_sum, int32_t *d_cnt, cudaStream_t st);
+cudaError_t cg_launch_bam_starts(const uint8_t *d_buf, long long n, const uint32_t *d_bm, const long long *d_entry,
+                                 const BamSum *d_sum, const int64_t *d_woff, uint32_t *d_start, int32_t *d_fsize,
+                                 cudaStream_t st);
+cudaError_t cg_launch_bam_cut(const int64_t *d_woff, long long n, const uint32_t *d_start, const int64_t *d_foff,
+                              long long limit, BamSum *d_sum, cudaStream_t st);
+cudaError_t cg_launch_bam_emit(const uint8_t *d_buf, const uint32_t *d_start, const int64_t *d_foff, long long n_rec,
+                               long long n_cut, uint8_t *d_out, unsigned long long *d_err, cudaStream_t st);
 // --pair-adapters: fold the records of adapter pair `pair` into the best pair per read (modifiers.py:480-503)
 cudaError_t cg_launch_fastq_pair_select(long long n_records, int pair, const cg_match_rec *d_cur1, int slots1,
                                         const cg_match_rec *d_cur2, int slots2, cg_match_rec *d_best1, cg_match_rec *d_best2,

@@ -883,7 +883,9 @@ def read_gzip_device_chunks(f, trimmer, buffer_size: int = 4 * 1024 * 1024, spli
     Chunks of a gzip file (a binary file object of the compressed bytes) inflated on the device
     (``cg_fastq_submit_gzip``): every member is inflated on the GPU and the plain bytes never cross PCIe.  Yields
     ``DeviceChunk`` objects for ``trimmer`` (a FastqTrimmer; its context and format decide how the chunks are cut: the
-    records of read_fastq_chunks / read_fasta_chunks).  A chunk is submitted when the generator is advanced, so the
+    records of read_fastq_chunks / read_fasta_chunks).  A trimmer with ``input_format="bam"`` reads unaligned BAM
+    (``CG_FORMAT_BAM``): the records are decoded on the device into FASTQ chunks, and afterwards ``trimmer.bam_tiles``
+    holds (tiles of the record-boundary walk, tiles walked again).  A chunk is submitted when the generator is advanced, so the
     trimmer's one chunk in flight stays as it is.  ``trimmer.statistics["in_bytes_gzip"]`` counts the compressed bytes
     consumed.  Meant for files of many members (BGZF, concatenated .gz files, this project's gzip outputs); a member
     that does not fit one submission makes the buffer grow.  ``split_members=True`` (``CG_GZIN_SPLIT_MEMBERS``) inflates
@@ -891,16 +893,25 @@ def read_gzip_device_chunks(f, trimmer, buffer_size: int = 4 * 1024 * 1024, spli
     submissions as it takes.
     """
     g = _GzipInput(trimmer.ctx, f, buffer_size, split_members)
+    bam = getattr(trimmer, "input_format", None) == "bam"
+    fmt = _lib.CG_FORMAT_BAM if bam else trimmer.params.format
+    carry = 0
     try:
-        while not g.done:
+        # BAM: a last chunk that reaches the 2 GiB chunk limit leaves a carry behind, submitted again
+        while not g.done or carry:
             g.fill()
             slot, res = C.c_int32(-1), _lib.cg_gzin_result()
-            _lib.check(_lib.lib().cg_fastq_submit_gzip(trimmer.ctx.handle, g.handle, g.pointer(), g.end,
-                                                       trimmer.params.format, int(g.eof), C.byref(slot), C.byref(res)))
+            _lib.check(_lib.lib().cg_fastq_submit_gzip(trimmer.ctx.handle, g.handle, g.pointer(), g.end, fmt,
+                                                       int(g.eof), C.byref(slot), C.byref(res)))
             _add_gzip_bytes(trimmer.statistics, res.consumed)
             g.consume(res.consumed)
+            carry = res.carry_bytes if bam and g.done else 0
             if slot.value >= 0:
                 yield DeviceChunk(slot.value, res.chunk_bytes)
+        if bam:
+            tiles, rewalked = C.c_int64(), C.c_int64()
+            _lib.check(_lib.lib().cg_gzin_bam_tiles(trimmer.ctx.handle, g.handle, C.byref(tiles), C.byref(rewalked)))
+            trimmer.bam_tiles = (tiles.value, rewalked.value)
     finally:
         g.close()
 
@@ -951,14 +962,17 @@ def read_gzip_device_paired_chunks(f1, f2, trimmer, buffer_size: int = 4 * 1024 
 
 _FORMATS = {("fastq", None): _lib.CG_FORMAT_FASTQ, ("fastq", "fastq"): _lib.CG_FORMAT_FASTQ,
             ("fasta", None): _lib.CG_FORMAT_FASTA, ("fasta", "fasta"): _lib.CG_FORMAT_FASTA,
-            ("fastq", "fasta"): _lib.CG_FORMAT_FASTQ_TO_FASTA}
+            ("fastq", "fasta"): _lib.CG_FORMAT_FASTQ_TO_FASTA,
+            # BAM arrives as FASTQ chunks (read_gzip_device_chunks), so the collects see FASTQ
+            ("bam", None): _lib.CG_FORMAT_FASTQ, ("bam", "fastq"): _lib.CG_FORMAT_FASTQ,
+            ("bam", "fasta"): _lib.CG_FORMAT_FASTQ_TO_FASTA}
 
 
 def _format_code(input_format: str, output_format: Optional[str]) -> int:
     """cg_fastq_params.format of (input format, output format or None for the input's)."""
     if (input_format, output_format) not in _FORMATS:
         raise ValueError(f"unsupported formats: {input_format!r} in, {output_format!r} out "
-                         "(input 'fastq' or 'fasta'; output None, 'fasta', or 'fastq' for FASTQ input)")
+                         "(input 'fastq', 'fasta' or 'bam'; output None, 'fasta', or 'fastq' for FASTQ or BAM input)")
     return _FORMATS[(input_format, output_format)]
 
 
@@ -1180,8 +1194,11 @@ class FastqTrimmer:
     revcomp, rc_suffix  --revcomp: adapters are searched on the read and on its reverse complement and the better
                         orientation is written (" rc" appended to the name unless rc_suffix is False;
                         ReverseComplementer, modifiers.py:264-308), all on the device
-    input_format        "fastq" (default) or "fasta" (read_fasta_chunks; no quality options then)
-    output_format       None (the input's format) or "fasta" (FASTQ in, FASTA out: a .fasta / .fa output or --fasta)
+    input_format        "fastq" (default), "fasta" (read_fasta_chunks; no quality options then) or "bam" (unaligned
+                        BAM, single-end: chunks only from read_gzip_device_chunks, which decodes the records on the
+                        device; bytes are refused)
+    output_format       None (the input's format; FASTQ for BAM) or "fasta" (FASTQ or BAM in, FASTA out: a .fasta / .fa
+                        output or --fasta)
     collect_statistics  also collect what the report needs beyond the counters (cg_fastq_stats_*): per-adapter
                         statistics, the poly-A and written-length histograms; ``statistics_vector()``,
                         ``adapter_statistics()``, ``poly_a_trimmed_lengths``, ``written_lengths``
@@ -1221,6 +1238,7 @@ class FastqTrimmer:
                  gzip_outputs: Sequence[str] = (), rows: Sequence[str] = (), gzip_rows: Sequence[str] = (),
                  max_average_error_rate: Optional[float] = None, zero_cap: bool = False):
         self.rows, self.gzip_rows = _row_kinds(rows, gzip_rows)
+        self.input_format = input_format
         self.params = _fastq_params(times, quality_cutoff, quality_base, nextseq_cutoff, minimum_length, maximum_length,
                                     max_n, max_expected_errors, discard_trimmed, discard_untrimmed, cut, poly_a, length,
                                     trim_n, discard_casava, action, revcomp, rc_suffix, input_format, output_format,
@@ -1251,6 +1269,9 @@ class FastqTrimmer:
 
     def _submit(self, chunk, rows: Optional[tuple] = None) -> Tuple[int, int, object]:
         """Upload a chunk and request its rows (``rows``: kinds, default the trimmer's)."""
+        if self.input_format == "bam" and not isinstance(chunk, DeviceChunk):
+            raise ValueError("a BAM trimmer takes the chunks of read_gzip_device_chunks, not bytes: BAM records are "
+                             "decoded on the device")
         slot, buf = _submit_chunk(self.ctx, chunk)
         kinds = self.rows if rows is None else rows
         _request_rows(self.ctx, slot, kinds, self._texts(kinds), self.gzip_rows)
@@ -1490,6 +1511,8 @@ class PairedFastqTrimmer:
                  revcomp: bool = False, rc_suffix: bool = True):
         if pair_filter not in self.MODES:
             raise ValueError("pair_filter must be 'any', 'both' or 'first'")
+        if input_format == "bam":
+            raise ValueError("BAM input is read single-end only (as the reference reads it): use FastqTrimmer")
         for options in (options1, options2):
             for key in ("revcomp", "rc_suffix"):
                 if key in (options or {}):

@@ -437,6 +437,32 @@ int cg_gzin_create_ex(cg_ctx *ctx, int32_t flags, int32_t *handle);
 int cg_gzin_destroy(cg_ctx *ctx, int32_t handle);
 int cg_fastq_submit_gzip(cg_ctx *ctx, int32_t handle, const uint8_t *gz, int64_t n_bytes, int32_t format, int32_t final,
                          int32_t *slot, cg_gzin_result *res);
+/* Unaligned BAM input (what the reference reads single-end since v4.7 through dnaio): format CG_FORMAT_BAM, accepted only
+ * by cg_fastq_submit_gzip (default and split streams alike; CG_EINVAL in every other submit and as
+ * cg_fastq_params.format).  A BAM file is BGZF, so its members inflate like any gzip input; the plain stream is the BAM
+ * header ("BAM\1", l_text, text, n_ref, n_ref x (l_name, name, l_ref)), skipped, then records.  The slot holds the FASTQ
+ * text of the whole records cut so far -- per record "@" + name + "\n" + the sequence decoded with "=ACMGRSVTWYHKDBN" +
+ * "\n+\n" + every quality byte + 33 + "\n"; CIGAR and aux tags are skipped -- and is indistinguishable from
+ * cg_fastq_submit of that text: cg_fastq_slot_read returns it and every single-end collect takes it (params.format
+ * CG_FORMAT_FASTQ or CG_FORMAT_FASTQ_TO_FASTA).  Result: chunk_bytes is the FASTQ size of the slot, n_records its
+ * records, plain_bytes and carry_bytes count BAM bytes.  The cut keeps the FASTQ text under the 2 GiB chunk limit (FASTQ
+ * is at most 4/3 of its BAM bytes); at `final` a chunk that reaches it leaves carry_bytes > 0: submit again (final, no
+ * bytes) until the carry is empty.  A stream takes one format for its whole life: CG_FORMAT_BAM after another format,
+ * or another after CG_FORMAT_BAM, is CG_EINVAL.
+ * A record is structurally valid when l_read_name >= 1, its name ends in NUL, l_seq >= 0 and
+ * 32 + l_read_name + 4 n_cigar_op + (l_seq + 1) / 2 + l_seq <= block_size.  Where dnaio refuses a record or its answer
+ * is not known, the record is refused rather than guessed:
+ *   CG_EINVAL        not "BAM\1" or a negative length in the header ("not a BAM file"); a header or record still
+ *                    incomplete at `final` ("BAM file ends inside record N"); a structurally invalid record; a quality
+ *                    value above 93; a name byte outside 0x21..0x7E (the SAM specification's [!-?A-~]);
+ *   CG_EUNSUPPORTED  flag != 4 (dnaio reads unmapped single reads only); no qualities (l_seq > 0 and the first quality
+ *                    byte 0xFF); one record whose FASTQ text alone reaches 2 GiB.
+ * Messages name the record by its number in the file (0-based) and its offset in the decompressed stream.  As for gzip
+ * errors, no slot is taken, the stream is unchanged and the context stays usable. */
+#define CG_FORMAT_BAM 3
+/* The tiles of the BAM record-boundary walk a stream ran and those walked again because their speculative start was
+ * not on the true chain, over the stream's life. */
+int cg_gzin_bam_tiles(cg_ctx *ctx, int32_t handle, int64_t *tiles, int64_t *rewalked);
 /* The plain chunk of a submitted, not yet collected slot (not a mate of an interleaved chunk), copied to host memory:
  * what a caller keeps to submit a chunk from cg_fastq_submit_gzip again (a collect that needs a larger row buffer).
  * *n_bytes: its size; CG_EINVAL when capacity is smaller. */

@@ -46,6 +46,12 @@ compressed on the device (gzip_rows), and plain rows compressed by host zlib lev
 Per arm: host-to-host reads/s and the row bytes downloaded.  With --baseline-tree (a built checkout of another commit):
 its "paired" run and this tree's, both without rows, in alternating processes, three each.  The card's name and power
 limit are read in the run.
+--bam-input [n_reads] [submission_megabytes]: unaligned BAM input.  The same reads (-a AGATCGGAAGAGC -q 20 -m 20, plain
+output) in two forms, alternating over three rounds in one process, host to host: a BGZF uBAM read through the BAM path
+(FastqTrimmer(input_format="bam"), read_gzip_device_chunks: inflated, records decoded into FASTQ on the device) and the
+same reads as BGZF FASTQ through the member path.  Per arm: reads/s and the compressed bytes; for the BAM arm the tiles
+of the record-boundary walk and those walked again.  A second line: the BAM kernels' device time per MiB of BAM from
+torch.profiler, in a run of its own.  The card's name and power limit are read in the run.
 """
 import json
 import subprocess
@@ -343,6 +349,108 @@ def measure_gzip_input(n, submit_mb):
                           "ms_per_MiB_plain_total": sum(ms.values()) / mib, "launches": launches}))
 
 
+def _bgzf(plain, level=6):
+    """plain as BGZF members of 65 280 plain bytes (BC extra field), compressed on 16 threads, and the EOF block."""
+    import struct
+    from concurrent.futures import ThreadPoolExecutor
+
+    def member(piece):
+        c = zlib.compressobj(level, zlib.DEFLATED, -15)
+        data = c.compress(piece) + c.flush()
+        return (b"\x1f\x8b\x08\x04\0\0\0\0\0\xff\x06\x00BC\x02\x00" + struct.pack("<H", 25 + len(data)) + data
+                + struct.pack("<II", zlib.crc32(piece), len(piece)))
+    with ThreadPoolExecutor(16) as ex:
+        parts = list(ex.map(member, [plain[i:i + 65280] for i in range(0, len(plain), 65280)]))
+    return b"".join(parts) + bytes.fromhex("1f8b08040000000000ff0600424302001b0003000000000000000000")
+
+
+def _bam_of_fastq(data, rec_len):
+    """The unaligned BAM stream (header and records, flag 4) of fixed-size FASTQ records "@name\nSEQ\n+\nQUAL\n"."""
+    import struct
+
+    fq = np.frombuffer(data, dtype=np.uint8).reshape(-1, rec_len)
+    name_len = int(np.argmax(fq[0] == ord("\n"))) - 1
+    read_len = (rec_len - name_len - 5) // 2
+    n = fq.shape[0]
+    lrn, half = name_len + 1, (read_len + 1) // 2
+    body = 32 + lrn + half + read_len
+    rec = np.zeros((n, 4 + body), dtype=np.uint8)
+    rec[:, :36] = np.frombuffer(struct.pack("<iiiBBHHHiiii", body, -1, -1, lrn, 255, 4680, 0, 4, read_len, -1, -1, 0),
+                                dtype=np.uint8)
+    rec[:, 36:36 + name_len] = fq[:, 1:1 + name_len]
+    code = np.full(256, 15, dtype=np.uint8)
+    for i, ch in enumerate("=ACMGRSVTWYHKDBN"):
+        code[ord(ch)] = i
+    seq = code[fq[:, 2 + name_len:2 + name_len + read_len]]
+    if read_len & 1:
+        seq = np.concatenate([seq, np.zeros((n, 1), dtype=np.uint8)], axis=1)
+    rec[:, 36 + lrn:36 + lrn + half] = (seq[:, 0::2] << 4) | seq[:, 1::2]
+    q0 = 2 + name_len + read_len + 3
+    rec[:, 36 + lrn + half:] = fq[:, q0:q0 + read_len] - 33
+    text = b"@HD\tVN:1.6\tSO:unsorted\n"
+    return b"BAM\x01" + struct.pack("<i", len(text)) + text + struct.pack("<i", 0) + rec.tobytes()
+
+
+def measure_bam_input(n, submit_mb):
+    import io
+
+    from cutadapt_b200.pipeline import read_gzip_device_chunks
+
+    data, rec_len = build_fastq(n, pinned=False)
+    plain = data.tobytes()
+    forms = {"bam": _bgzf(_bam_of_fastq(plain, rec_len)), "bgzf_fastq": _bgzf(plain)}
+    adapters = [PA.BackAdapter("AGATCGGAAGAGC", max_errors=0.1)]
+    opts = dict(quality_cutoff=(0, 20), minimum_length=20)
+
+    def run(arm, gz):
+        t = FastqTrimmer(adapters, **opts, input_format="bam" if arm == "bam" else "fastq")
+        t0 = time.perf_counter()
+        out = sum(len(o) for o in t.process_chunks(read_gzip_device_chunks(io.BytesIO(gz), t, submit_mb << 20),
+                                                   copy=False))
+        return time.perf_counter() - t0, out, getattr(t, "bam_tiles", None)
+
+    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader",
+                           "-i", str(torch.cuda.current_device())], capture_output=True, text=True).stdout.strip()
+    warm = plain[:rec_len * 1000]
+    warm_forms = {"bam": _bgzf(_bam_of_fastq(warm, rec_len)), "bgzf_fastq": _bgzf(warm)}
+    for arm, gz in warm_forms.items():             # warm-up: buffers, module load
+        run(arm, gz)
+    res = {arm: {"wall_s": 0.0, "gz_bytes": len(gz)} for arm, gz in forms.items()}
+    outs = set()
+    for _ in range(3):
+        for arm, gz in forms.items():
+            w, out, tiles = run(arm, gz)
+            res[arm]["wall_s"] += w
+            outs.add(out)
+            if tiles:
+                res[arm]["tiles"], res[arm]["tiles_rewalked"] = tiles
+    for x in res.values():
+        x["M_reads_per_s"] = 3 * n / x["wall_s"] / 1e6
+    assert len(outs) == 1, "the arms wrote different amounts"
+    print(json.dumps({"what": "BGZF uBAM through the BAM path against the same reads as BGZF FASTQ (-a AGATCGGAAGAGC "
+                      "-q 20 -m 20), host to host", "reads": n, "submission_MiB": submit_mb,
+                      "gpu": torch.cuda.get_device_name(), "card_and_power_limit": card, "arms": res}))
+
+    from torch.profiler import ProfilerActivity, profile
+
+    kernels = ("bam_spec", "bam_resolve", "bam_count", "bam_starts", "bam_cut", "bam_emit")
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        run("bam", forms["bam"])
+        torch.cuda.synchronize()
+    ms, launches = {}, {}
+    for ev in prof.key_averages():
+        for k in kernels:
+            if "::" + k + "_kernel" in ev.key or ev.key.startswith(k + "_kernel"):
+                ms[k] = ms.get(k, 0.0) + ev.device_time_total / 1000.0
+                launches[k] = launches.get(k, 0) + ev.count
+    if not ms:
+        raise RuntimeError("the profiler saw no BAM kernel launch")
+    mib = len(_bam_of_fastq(plain, rec_len)) / 2**20
+    print(json.dumps({"what": "BAM kernels' device time (torch.profiler, CUDA activity)", "card_and_power_limit": card,
+                      "BAM_MiB": mib, "ms_total": ms, "ms_per_MiB_bam": {k: v / mib for k, v in ms.items()},
+                      "ms_per_MiB_bam_total": sum(ms.values()) / mib, "launches": launches}))
+
+
 def measure_rows(n, chunk_mb, baseline_tree=None):
     """--rows: the "paired" variant with info rows on both mates (--info-file + --info-file-paired), four arms
     alternating over three rounds in one process; then, with a baseline tree, its "paired" run without rows against
@@ -455,6 +563,9 @@ def main():
             base = argv[i + 1]
             del argv[i:i + 2]
         return measure_rows(int(argv[1]) if len(argv) > 1 else 4_000_000, int(argv[2]) if len(argv) > 2 else 64, base)
+    if "--bam-input" in sys.argv:
+        argv = [a for a in sys.argv if a != "--bam-input"]
+        return measure_bam_input(int(argv[1]) if len(argv) > 1 else 4_000_000, int(argv[2]) if len(argv) > 2 else 64)
     if "--gzip-input" in sys.argv:
         argv = [a for a in sys.argv if a != "--gzip-input"]
         return measure_gzip_input(int(argv[1]) if len(argv) > 1 else 4_000_000, int(argv[2]) if len(argv) > 2 else 64)

@@ -12,6 +12,7 @@ command line (no reports): it shows the per-chunk worker of INTEGRATION.md secti
       -o out.fastq in.fastq                                                            (filter outputs)
   python tools/trim_fastq.py --interleaved -a ADAPT1 -A ADAPT2 -m 20:25 -o out.fastq in.interleaved.fastq
   python tools/trim_fastq.py -a AGATCGGAAGAGC -o out.fastq.gz in.fastq.gz                   (gzip)
+  python tools/trim_fastq.py -a AGATCGGAAGAGC -q 20 -m 20 -o out.fastq reads.bam             (unaligned BAM)
   python tools/trim_fastq.py --revcomp -g ^TTATTTGTCT -G ^TCCGCACTGG -o out.1.fastq -p out.2.fastq in.1.fastq in.2.fastq
   python tools/trim_fastq.py -a ADAPT1 -A ADAPT2 --info-file info1.txt.gz --info-file-paired info2.txt.gz \
       -o out.1.fastq -p out.2.fastq in.1.fastq in.2.fastq                               (per-read row files)
@@ -40,6 +41,11 @@ input of at least 16 MiB (DEVICE_GZIP_SPLIT_MIN; the single member that gzip and
 block-parallel (split_members=True).  Smaller ones are decompressed on the host with Python's gzip module.  The outputs are the same either way; the stderr line's "in_bytes_gzip" (the
 compressed bytes consumed) appears only when the device inflated the input.  The format is detected from the first
 decompressed byte.
+
+Unaligned BAM input (uBAM, as basecallers and GATK-style workflows write it) is detected by content, whatever the file
+is called: a gzip file whose first member inflates to "BAM\\1".  It is read single-end only, as in the reference: its BGZF
+members are inflated and its records decoded into FASTQ on the device (read_gzip_device_chunks), and the output is
+FASTQ, or FASTA with --fasta or a .fasta / .fa name.  Two BAM inputs, or --interleaved with BAM, stop with an error.
 
 --revcomp / --rc: the adapters are also searched on the reverse complement of each read and the better orientation
 is written, " rc" appended to its name (ReverseComplementer).  On pairs the -a adapters also run on R2 and the -A
@@ -111,8 +117,23 @@ def gzip_route(path):
     return None
 
 
+def is_bam(path):
+    """Whether an input is BAM, by content as xopen plus detect_file_format see it: the file starts with 1f 8b and its
+    first gzip member inflates to "BAM\\1" (any name; .bam is the usual one)."""
+    with open(path, "rb") as f:
+        head = f.read(DEVICE_GZIP_FIRST_MEMBER)
+    if head[:2] != b"\x1f\x8b":
+        return False
+    try:
+        return zlib.decompressobj(31).decompress(head, 4) == b"BAM\x01"
+    except zlib.error:
+        return False
+
+
 def detect_format(path):
-    """"fasta" or "fastq" from the first (decompressed) byte (files.py:314-333)."""
+    """"bam", or "fasta" / "fastq" from the first (decompressed) byte (files.py:304-333)."""
+    if is_bam(path):
+        return "bam"
     with open_input(path) as f:
         return "fasta" if f.read(1) in (b">", b"#") else "fastq"
 
@@ -304,8 +325,11 @@ def main():
         ap.error("--info-file cannot be combined with --revcomp on paired-end data: the info rows of swapped pairs are "
                  "not produced")
     input_format = detect_format(args.inputs[0])
+    if input_format == "bam" or (len(args.inputs) == 2 and detect_format(args.inputs[1]) == "bam"):
+        if paired:
+            ap.error("BAM input is read single-end only: one BAM input file, without --interleaved")
     fasta_out = file_format(args.output, input_format, args.fasta) == "fasta"
-    output_format = "fasta" if fasta_out and input_format == "fastq" else None
+    output_format = "fasta" if fasta_out and input_format in ("fastq", "bam") else None
     if input_format == "fasta" and args.max_ee is not None:
         print("WARNING: Ignoring option --max-ee because input does not provide quality values", file=sys.stderr)
         args.max_ee = None
@@ -323,6 +347,9 @@ def main():
 
     def single_input(t):
         """(file, chunks) of the single input for trimmer t."""
+        if input_format == "bam":              # BGZF: every member inflated on the device, the records decoded there
+            f = open(args.inputs[0], "rb")
+            return f, read_gzip_device_chunks(f, t, gz_buffer)
         route = gzip_route(args.inputs[0])
         if route:
             f = open(args.inputs[0], "rb")
