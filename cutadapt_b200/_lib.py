@@ -144,7 +144,7 @@ class cg_fastq_params(C.Structure):
         ("gzip_outputs", C.c_int32),
         ("max_average_error_rate", C.c_double),
         ("zero_cap", C.c_int32),
-        ("reserved_pad", C.c_int32),
+        ("names", C.c_int32),
     ]
 
 
@@ -244,6 +244,9 @@ def _declare(lib) -> None:
     lib.cg_fastq_stats_create.argtypes = [vp, i32, C.POINTER(i32)]
     lib.cg_fastq_stats_read.argtypes = [vp, i32, C.POINTER(i32), C.POINTER(i32), vp, i64, C.POINTER(i64), C.c_int]
     lib.cg_fastq_stats_destroy.argtypes = [vp, i32]
+    lib.cg_names_create.argtypes = [vp, C.POINTER(cg_names_desc), C.POINTER(i32)]
+    lib.cg_names_set_mate.argtypes = [vp, i32, i32, C.c_char_p, vp, i32, vp, i32, i32]
+    lib.cg_names_destroy.argtypes = [vp, i32]
     lib.cg_adapterset_create.argtypes = [
         vp, C.POINTER(cg_adapter_desc), i32, C.POINTER(cg_group_desc), i32, C.POINTER(vp),
     ]
@@ -467,6 +470,54 @@ def make_params(quality_trim=False, cutoff_front=0, cutoff_back=0, quality_base=
 
 
 # ---- context ---------------------------------------------------------------------------------
+
+
+class cg_name_token(C.Structure):
+    _fields_ = [("kind", C.c_int32), ("mate", C.c_int32), ("text", C.c_char_p), ("len", C.c_int32)]
+
+
+class cg_names_desc(C.Structure):
+    _fields_ = [("length_tag", C.c_char_p), ("strip_suffix", C.POINTER(C.c_char_p)), ("n_strip_suffix", C.c_int32),
+                ("paired", C.c_int32), ("prefix", C.c_char_p), ("suffix", C.c_char_p),
+                ("rename", C.POINTER(cg_name_token)), ("n_rename", C.c_int32)]
+
+
+class Names:
+    """A names handle on a context (cg_names_*): the read-name modifiers of the collects whose parameters name
+    ``handle`` in ``names``.  tokens: the --rename template as (kind, mate, literal text) or None for no renamer."""
+
+    def __init__(self, ctx: "Context", length_tag=None, strip_suffix=(), prefix="", suffix="", tokens=None,
+                 paired=False):
+        enc = lambda x: x.encode("latin-1")
+        strips = (C.c_char_p * max(len(strip_suffix), 1))(*[enc(x) for x in strip_suffix])
+        toks = (cg_name_token * max(len(tokens or ()), 1))()
+        for i, (kind, mate, text) in enumerate(tokens or ()):
+            toks[i].kind, toks[i].mate, toks[i].text, toks[i].len = kind, mate, enc(text), len(enc(text))
+        d = cg_names_desc(enc(length_tag) if length_tag is not None else None, strips, len(strip_suffix), int(paired),
+                          enc(prefix or ""), enc(suffix or ""), toks, -1 if tokens is None else len(tokens))
+        h = C.c_int32(0)
+        check(lib().cg_names_create(ctx.handle, C.byref(d), C.byref(h)))
+        self.ctx, self.handle = ctx, h.value
+
+    def set_mate(self, mate: int, names, linked, last_cut_front: int = 0, last_cut_back: int = 0) -> None:
+        blobs = [n.encode("latin-1") for n in names]
+        offsets = np.zeros(len(blobs) + 1, dtype=np.int32)
+        offsets[1:] = np.cumsum([len(b) for b in blobs]) if blobs else []
+        flags = np.array(linked, dtype=np.uint8).reshape(-1)
+        check(lib().cg_names_set_mate(self.ctx.handle, self.handle, mate, b"".join(blobs), offsets.ctypes.data,
+                                      len(blobs), flags.ctypes.data if flags.size else None, int(last_cut_front),
+                                      int(last_cut_back)))
+
+    def close(self) -> None:
+        if self.handle:
+            check(lib().cg_names_destroy(self.ctx.handle, self.handle))
+            self.handle = 0
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
 
 
 class FastqStatistics:

@@ -7,6 +7,7 @@
 #include <cuda_runtime.h>
 #include <stdio.h>
 #include <stdlib.h>
+#include <ctype.h>
 #include <string.h>
 
 #include <algorithm>
@@ -157,6 +158,9 @@ struct FastqSlot {
     DevBuf<unsigned long long> d_fqstats;       // statistics on: the chunk's statistics vector (added on success)
     DevBuf<int32_t> d_polya;                    // statistics with --poly-a: bases PolyATrimmer removed, per record
     PinBuf<unsigned long long> h_fqstats;
+    DevBuf<int32_t> d_namelen;                  // read names: bytes of every new name (both steps, both mates' counts) ...
+    DevBuf<int64_t> d_nameoff;                  // ... their scans: step 1, then step 2
+    DevBuf<unsigned long long> d_namemis;       // ... the first pair whose new names no longer name mates
     DevBuf<int32_t> d_fold;                     // interleaved outputs: the sizes the partition runs on
     DevBuf<unsigned long long> d_ilverr;        // interleaved input: first problem of the split, record << 32 | code
     DevBuf<CgGzPiece> d_gzpieces;               // gzip outputs: the pieces of the destinations ...
@@ -223,6 +227,15 @@ struct FqStatsAcc {
     std::vector<int64_t> v;
 };
 
+// A names handle (cg_names_create): the parts of the program, and its blob (CgNameProg + pool) built from them once
+// the mates' adapter names are set, on the host and on the device
+struct NamesProg {
+    CgNameSpec spec;
+    std::vector<uint8_t> blob;
+    DevBuf<uint8_t> d_blob;
+    bool uploaded = false;
+};
+
 struct cg_ctx {
     int device = 0;
     cudaStream_t stream = nullptr;
@@ -271,6 +284,8 @@ struct cg_ctx {
     std::map<int32_t, FqStatsAcc> fq_stats;      // cg_fastq_stats_* by handle
     int32_t fq_stats_next = 1;
     std::map<int32_t, GzinStream> gzin;          // cg_gzin_* by handle
+    std::map<int32_t, NamesProg> names;          // cg_names_* by handle
+    int32_t names_next = 1;
     int32_t gzin_next = 1;
 };
 
@@ -2509,7 +2524,8 @@ extern "C" int cg_fastq_slot_read(cg_ctx *c, int32_t slot, uint8_t *dst, int64_t
     if (!c || !n_bytes || slot < 0 || slot >= CG_FQ_SLOTS || capacity < 0 || (capacity && !dst))
         return fail(CG_EINVAL, "cg_fastq_slot_read: bad argument");
     FastqSlot &f = c->fq[slot];
-    if (!f.busy || f.ilv) return fail(CG_EINVAL, "cg_fastq_slot_read: the slot holds no chunk of its own");
+    // the first slot of an interleaved chunk holds the whole chunk until the collect splits it; the second holds none
+    if (!f.busy || f.ilv == 2) return fail(CG_EINVAL, "cg_fastq_slot_read: the slot holds no chunk of its own");
     CU(cudaSetDevice(c->device));
     *n_bytes = f.n_bytes;
     if (capacity < f.n_bytes) return fail(CG_EINVAL, "cg_fastq_slot_read: buffer too small");
@@ -3591,6 +3607,229 @@ static int fastq_collect_finish(cg_ctx *c, const FqMate *m, int n_mates, FqDemux
     return CG_OK;
 }
 
+// ---- read names (cg_names_*; the name stage, cg_names_core.cuh) ----
+static void names_build(NamesProg &np)
+{
+    np.blob = cg_names_blob(np.spec);
+    np.uploaded = false;
+}
+
+extern "C" int cg_names_create(cg_ctx *c, const cg_names_desc *d, int32_t *handle)
+{
+    if (!c || !d || !handle || d->n_strip_suffix < 0 || (d->n_strip_suffix && !d->strip_suffix) ||
+        (d->n_rename > 0 && !d->rename))
+        return fail(CG_EINVAL, "cg_names_create: bad argument");
+    NamesProg np;
+    if (d->length_tag) {
+        np.spec.tag = d->length_tag;
+        if (np.spec.tag.empty()) return fail(CG_EINVAL, "cg_names_create: the length tag is empty");
+        for (char ch : np.spec.tag) {
+            const bool ok = isalnum((unsigned char)ch) || strchr("_=:,;/-@#%!~", ch) != nullptr;
+            if (!ok)
+                return fail(CG_EINVAL, std::string("cg_names_create: the length tag may hold letters, digits and "
+                                                   "_ = : , ; / - @ # % ! ~ only (the reference reads it as a regular "
+                                                   "expression), not '") + ch + "'");
+        }
+    }
+    for (int k = 0; k < d->n_strip_suffix; ++k) {
+        if (!d->strip_suffix[k]) return fail(CG_EINVAL, "cg_names_create: a strip suffix is NULL");
+        np.spec.strips.emplace_back(d->strip_suffix[k]);
+    }
+    np.spec.prefix = cg_names_affix(d->prefix);
+    np.spec.suffix = cg_names_affix(d->suffix);
+    np.spec.paired = d->paired != 0;
+    np.spec.has_rename = d->n_rename >= 0;
+    if (np.spec.has_rename && (!np.spec.prefix.empty() || !np.spec.suffix.empty()))
+        return fail(CG_EINVAL, "Option --rename cannot be combined with --prefix (-x) or --suffix (-y)");
+    for (int k = 0; k < d->n_rename; ++k) {
+        const cg_name_token &t = d->rename[k];
+        const bool mate_ok = t.mate == 0 || (np.spec.paired && (t.mate == 1 || t.mate == 2) && t.kind != CG_NT_ID &&
+                                             t.kind != CG_NT_RN && t.kind != CG_NT_LITERAL);
+        if (t.kind < 0 || t.kind >= CG_NT_KINDS || !mate_ok || (t.kind == CG_NT_RC && np.spec.paired) ||
+            (t.kind == CG_NT_RN && !np.spec.paired) || (t.kind == CG_NT_LITERAL && (t.len < 0 || (t.len && !t.text))))
+            return fail(CG_EINVAL, "cg_names_create: rename token " + std::to_string(k) + " is not a variable of " +
+                                       (np.spec.paired ? "PairedEndRenamer" : "Renamer"));
+        np.spec.rename.push_back({t.kind, t.mate, t.kind == CG_NT_LITERAL ? std::string(t.text, (size_t)t.len) : std::string()});
+    }
+    names_build(np);
+    const int32_t h = c->names_next++;
+    c->names.emplace(h, std::move(np));
+    *handle = h;
+    return CG_OK;
+}
+
+extern "C" int cg_names_set_mate(cg_ctx *c, int32_t handle, int32_t mate, const char *names, const int32_t *offsets,
+                                 int32_t n_names, const uint8_t *linked, int32_t last_cut_front, int32_t last_cut_back)
+{
+    if (!c || mate < 0 || mate > 1 || n_names < 0 || (n_names && (!offsets || !linked)) || last_cut_front < 0 ||
+        last_cut_back < 0)
+        return fail(CG_EINVAL, "cg_names_set_mate: bad argument");
+    auto it = c->names.find(handle);
+    if (it == c->names.end()) return fail(CG_EINVAL, "cg_names_set_mate: unknown names handle");
+    NamesProg &np = it->second;
+    if (n_names) {
+        if (offsets[0] != 0) return fail(CG_EINVAL, "cg_names_set_mate: offsets must start at 0");
+        for (int a = 0; a < n_names; ++a)
+            if (offsets[a + 1] < offsets[a]) return fail(CG_EINVAL, "cg_names_set_mate: offsets must not decrease");
+        if (offsets[n_names] && !names) return fail(CG_EINVAL, "cg_names_set_mate: names is NULL");
+    }
+    np.spec.names[mate].assign(names ? names : "", n_names ? (size_t)offsets[n_names] : 0);
+    np.spec.name_off[mate].assign(offsets ? offsets : nullptr, offsets ? offsets + n_names + 1 : nullptr);
+    if (!n_names) np.spec.name_off[mate].assign(1, 0);
+    np.spec.linked[mate].assign(linked ? linked : nullptr, linked ? linked + n_names : nullptr);
+    np.spec.cut_last[mate][0] = last_cut_front;
+    np.spec.cut_last[mate][1] = last_cut_back;
+    names_build(np);
+    return CG_OK;
+}
+
+extern "C" int cg_names_destroy(cg_ctx *c, int32_t handle)
+{
+    if (!c) return fail(CG_EINVAL, "cg_names_destroy: bad argument");
+    if (!c->names.erase(handle)) return fail(CG_EINVAL, "cg_names_destroy: unknown names handle");
+    return CG_OK;
+}
+
+// Slot f's chunk buffer with room for `need` bytes, its first `used` bytes kept (the spare d_norm takes them)
+static int names_room(FastqSlot &f, size_t used, size_t need, cudaStream_t st)
+{
+    if (need >= (1ull << 32))
+        return fail(CG_EINVAL, "cg_fastq: the chunk and its new read names exceed 4 GiB; use smaller chunks");
+    if (need <= f.d_in.cap) return CG_OK;
+    int rc = f.d_norm.ensure(need);
+    if (rc != CG_OK) return rc;
+    if (used) CU(cudaMemcpyAsync(f.d_norm.p, f.d_in.p, used, cudaMemcpyDeviceToDevice, st));
+    std::swap(f.d_in, f.d_norm);
+    return CG_OK;
+}
+
+static size_t align16(size_t x) { return (x + 15) & ~(size_t)15; }
+
+// The name stage of a collect (one mate, or both of a pair), once the matches and the written part of every read are
+// final and before the rows and the finish kernel: step 1 per mate (count, scan, write into an arena behind the
+// chunk), then with --rename step 2 over the step-1 names into a second arena.  The record tables point at the new
+// names and the writers' " rc" is off, so that every consumer reads the name as it is.
+static int fastq_stage_names(cg_ctx *c, FastqSlot *const *f, FqStage *const *g, const cg_fastq_params *const *fp,
+                             int n_mates, cudaStream_t st)
+{
+    if (fp[0]->names == 0 && (n_mates == 1 || fp[1]->names == 0)) return CG_OK;
+    if (n_mates == 2 && fp[0]->names != fp[1]->names)
+        return fail(CG_EINVAL, "cg_fastq_collect_paired: both mates' params must name the same names handle");
+    auto it = c->names.find(fp[0]->names);
+    if (it == c->names.end()) return fail(CG_EINVAL, "cg_fastq: unknown names handle");
+    NamesProg &np = it->second;
+    if (np.spec.paired != (n_mates == 2) && np.spec.has_rename)
+        return fail(CG_EINVAL, np.spec.paired ? "cg_fastq_collect: a paired --rename template needs a paired collect"
+                                         : "cg_fastq_collect_paired: a single-end --rename template on a pair");
+    int rc;
+    if (!np.uploaded) {
+        if ((rc = np.d_blob.ensure(np.blob.size())) != CG_OK) return rc;
+        CU(cudaMemcpyAsync(np.d_blob.p, np.blob.data(), np.blob.size(), cudaMemcpyHostToDevice, st));
+        CU(cudaStreamSynchronize(st));
+        np.uploaded = true;
+    }
+    const long long n = g[0]->n;
+    CgNameMate m[2];
+    memset(m, 0, sizeof m);
+    size_t arena1[2] = {0, 0}, arena2[2] = {0, 0};
+    long long total[2] = {0, 0};
+    auto mate_of = [&](int i) {
+        CgNameMate a;
+        a.buf = f[i]->d_in.p; a.rec = f[i]->d_rec.p; a.interval = f[i]->d_interval.p; a.mask = f[i]->d_mask.p;
+        a.origin = f[i]->d_origin.p; a.seq_len = f[i]->d_len.p; a.qtrim = g[i]->d_qtrim; a.matches = g[i]->d_matches;
+        a.times = g[i]->times; a.slots = g[i]->slots; a.mate = i; a.rc_suffix = g[i]->rc_suffix;
+        a.swapped = n_mates == 2 && g[i]->d_is_rc != nullptr;
+        a.cut_front = fp[i]->cut_front; a.cut_back = fp[i]->cut_back;
+        return a;
+    };
+    for (int i = 0; i < n_mates; ++i) {
+        FastqSlot &s = *f[i];
+        if ((rc = s.d_namelen.ensure((size_t)n * 2)) != CG_OK || (rc = s.d_nameoff.ensure((size_t)n * 2 + 2)) != CG_OK ||
+            (rc = s.d_scan.ensure((size_t)cg_scan_tiles(n) + 1)) != CG_OK)
+            return rc;
+        m[i] = mate_of(i);
+        const int casava = !np.spec.has_rename && fp[i]->discard_casava;
+        CU(cg_launch_fastq_names(0, 0, np.d_blob.p, m[i], m[i], n, s.d_namelen.p, nullptr, nullptr, nullptr, 0, 0, 0,
+                                 nullptr, st));
+        CU(cg_launch_scan_i32(s.d_namelen.p, n, s.d_scan.p, s.d_nameoff.p, st));
+        CU(cudaMemcpyAsync(&total[i], s.d_nameoff.p + n, sizeof total[i], cudaMemcpyDeviceToHost, st));
+        CU(cudaStreamSynchronize(st));
+        arena1[i] = align16((size_t)s.n_bytes);
+        if ((rc = names_room(s, (size_t)s.n_bytes, arena1[i] + (size_t)total[i] + 64, st)) != CG_OK) return rc;
+        m[i].buf = s.d_in.p;
+        CU(cg_launch_fastq_names(1, 0, np.d_blob.p, m[i], m[i], n, nullptr, nullptr, s.d_nameoff.p, nullptr,
+                                 (uint32_t)arena1[i], 0, casava, nullptr, st));
+        c->launches += 5;
+        g[i]->rc_suffix = 0;
+        m[i].rc_suffix = 0;
+    }
+    if (!np.spec.has_rename) return CG_OK;
+    const bool pair = n_mates == 2;
+    CgNameMate none;
+    memset(&none, 0, sizeof none);
+    CU(cg_launch_fastq_names(0, 1, np.d_blob.p, m[0], pair ? m[1] : none, n, f[0]->d_namelen.p + n,
+                             pair ? f[1]->d_namelen.p + n : nullptr, nullptr, nullptr, 0, 0, 0, nullptr, st));
+    c->launches += 1;
+    for (int i = 0; i < n_mates; ++i) {
+        FastqSlot &s = *f[i];
+        CU(cg_launch_scan_i32(s.d_namelen.p + n, n, s.d_scan.p, s.d_nameoff.p + n + 1, st));
+        long long t2 = 0;
+        CU(cudaMemcpyAsync(&t2, s.d_nameoff.p + 2 * n + 1, sizeof t2, cudaMemcpyDeviceToHost, st));
+        CU(cudaStreamSynchronize(st));
+        arena2[i] = align16(arena1[i] + (size_t)total[i]);
+        if ((rc = names_room(s, arena1[i] + (size_t)total[i], arena2[i] + (size_t)t2 + 64, st)) != CG_OK) return rc;
+        m[i].buf = s.d_in.p;
+        c->launches += 3;
+    }
+    if (pair) {
+        if ((rc = f[0]->d_namemis.ensure(1)) != CG_OK) return rc;
+        const unsigned long long unset = ~0ull;
+        CU(cudaMemcpyAsync(f[0]->d_namemis.p, &unset, sizeof unset, cudaMemcpyHostToDevice, st));
+    }
+    CU(cg_launch_fastq_names(1, 1, np.d_blob.p, m[0], pair ? m[1] : none, n, nullptr, nullptr, f[0]->d_nameoff.p + n + 1,
+                             pair ? f[1]->d_nameoff.p + n + 1 : nullptr, (uint32_t)arena2[0],
+                             pair ? (uint32_t)arena2[1] : 0, (fp[0]->discard_casava ? 1 : 0) |
+                             (pair && fp[1]->discard_casava ? 2 : 0), pair ? f[0]->d_namemis.p : nullptr, st));
+    c->launches += 1;
+    if (!pair) return CG_OK;
+    unsigned long long bad = 0;
+    CU(cudaMemcpyAsync(&bad, f[0]->d_namemis.p, sizeof bad, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    if (bad == ~0ull) return CG_OK;
+    // PairedEndRenamer's messages (modifiers.py:717-735), from R1's step-1 name and the new names of the pair
+    const long long p = (long long)(bad >> 1);
+    auto read_name = [&](const FastqSlot &s, CgFastqRecord r, std::string *out) {
+        out->resize((size_t)std::max(r.hdr_len, 0));
+        if (r.hdr_len > 0) CU(cudaMemcpy(&(*out)[0], s.d_in.p + r.hdr_start, (size_t)r.hdr_len, cudaMemcpyDeviceToHost));
+        return CG_OK;
+    };
+    auto split = [](const std::string &x, bool comment) {
+        CgSpan id, cm;
+        cg_name_split(cg_span((const uint8_t *)x.data(), (int)x.size()), &id, &cm);
+        const CgSpan &w = comment ? cm : id;
+        return std::string((const char *)w.p, (size_t)w.len);
+    };
+    std::string before, after[2];
+    {
+        int64_t o[2];
+        CU(cudaMemcpy(o, f[0]->d_nameoff.p + p, sizeof o, cudaMemcpyDeviceToHost));
+        CgFastqRecord r;
+        r.hdr_start = (uint32_t)(arena1[0] + (size_t)o[0]);
+        r.hdr_len = (int32_t)(o[1] - o[0]);
+        if ((rc = read_name(*f[0], r, &before)) != CG_OK) return rc;
+    }
+    if ((bad & 1) == 0)                         // the reference names R1's ID and R1's comment here
+        return fail(CG_EINVAL, "Input read IDs not identical: '" + split(before, false) + "' != '" + split(before, true) +
+                                   "'");
+    for (int k = 0; k < 2; ++k) {
+        CgFastqRecord r;
+        CU(cudaMemcpy(&r, f[k]->d_rec.p + p, sizeof r, cudaMemcpyDeviceToHost));
+        if ((rc = read_name(*f[k], r, &after[k])) != CG_OK) return rc;
+    }
+    return fail(CG_EINVAL, "After renaming R1 and R2, their IDs are no longer identical: '" + split(after[0], false) +
+                               "' != '" + split(after[1], false) + "'. Original read ID: '" + split(before, false) + "'. ");
+}
+
 static int fastq_collect_one(cg_ctx *c, FastqSlot &f, const cg_adapterset *s, const cg_fastq_params *fp, uint8_t *out,
                              int64_t out_capacity, cg_fastq_result *res, FqDemux *dm, int64_t *segments, FqSplit *sp)
 {
@@ -3604,6 +3843,9 @@ static int fastq_collect_one(cg_ctx *c, FastqSlot &f, const cg_adapterset *s, co
     if (rc != CG_OK) return rc;
     rc = fastq_stage_evaluate(c, f, s, fp, 1, f.stream, g);
     if (rc != CG_OK || g.n == 0) return rc;
+    FastqSlot *fs[1] = {&f};
+    FqStage *gs[1] = {&g};
+    if ((rc = fastq_stage_names(c, fs, gs, &fp, 1, f.stream)) != CG_OK) return rc;
     if ((rc = fastq_stage_rows(c, f, g, fp, f.stream)) != CG_OK) return rc;
     FqMate m;
     m.f = &f; m.g = &g; m.fp = fp; m.out = out; m.capacity = out_capacity; m.res = res; m.segments = segments;
@@ -3940,6 +4182,12 @@ static int fastq_collect_paired_run(cg_ctx *c, int32_t slot1, int32_t slot2, con
         return fail(CG_EINVAL, "paired FASTQ chunks differ in their number of records (" + std::to_string(g1.n) + " vs " +
                                    std::to_string(g2.n) + ")");
     if (g1.n == 0) return CG_OK;
+    {
+        FastqSlot *fs[2] = {&f1, &f2};
+        FqStage *gs[2] = {&g1, &g2};
+        const cg_fastq_params *fps[2] = {fp1, fp2};
+        if ((rc = fastq_stage_names(c, fs, gs, fps, 2, st)) != CG_OK) return rc;
+    }
     if ((rc = fastq_stage_rows(c, f1, g1, fp1, st)) != CG_OK || (rc = fastq_stage_rows(c, f2, g2, fp2, st)) != CG_OK)
         return rc;
     // --discard-untrimmed with adapters on one mate only tests "both" (cli.py:859-893)

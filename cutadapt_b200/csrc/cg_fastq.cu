@@ -1056,6 +1056,99 @@ __global__ void fq_ilv_offsets_kernel(long long n, const int32_t *route, int ilv
     off2[r] = ((ilv >> d) & 1) ? off1[r] + len1[r] : off2[r] + *total1;
 }
 
+// ---- read names (cg_names_core.cuh), one thread per record or pair ----
+// step 1 (cg_pre_name): the name LengthTagModifier, the SuffixRemovers and PrefixSuffixAdder leave
+template <bool WRITE>
+__global__ void fq_names_pre_kernel(const uint8_t *blob, CgNameMate a, long long n, int32_t *len, const int64_t *off,
+                                    uint32_t arena, int casava)
+{
+    const long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= n) return;
+    const CgNameProg &pr = *(const CgNameProg *)blob;
+    const CgFastqRecord m = a.rec[r];
+    const int mask = a.mask[r];
+    const CgSpan adapter = cg_adapter_name(blob, pr, a.mate, CG_FQ_MASK_ADAPTER(mask));
+    const bool rc = a.rc_suffix && (mask & CG_FQ_MASK_RC);
+    const int written = a.interval[2 * r + 1] - a.interval[2 * r];
+    if (!WRITE) {
+        CgNameCount c;
+        cg_pre_name(blob, pr, a.buf + m.hdr_start, m.hdr_len, rc, written, adapter, c);
+        len[r] = (int32_t)c.n;
+        return;
+    }
+    CgNameWrite w;
+    w.p = a.buf + arena + off[r];
+    cg_pre_name(blob, pr, a.buf + m.hdr_start, m.hdr_len, rc, written, adapter, w);
+    a.rec[r].hdr_start = arena + (uint32_t)off[r];
+    a.rec[r].hdr_len = (int32_t)w.n;
+    if (casava) a.mask[r] = (mask & ~16) | (fq_casava_filtered(w.p, (int)w.n) ? 16 : 0);
+}
+
+// What a template can name about record r of mate a (o: the other mate, for a turned pair's -u bases)
+__device__ CgNameVars fq_name_vars(const uint8_t *blob, const CgNameMate &a, const CgNameMate &o, long long r)
+{
+    const CgNameProg &pr = *(const CgNameProg *)blob;
+    CgNameVars v;
+    const CgFastqRecord m = a.rec[r];
+    v.header = cg_span(a.buf + m.hdr_start, m.hdr_len);
+    v.is_rc = (a.mask[r] & CG_FQ_MASK_RC) != 0;
+    // the read as it came: in this slot, reverse-complemented in place by single-end --revcomp; a turned pair's read
+    // is in the other slot as it came
+    const CgNameMate &src = (a.swapped && v.is_rc) ? o : a;
+    const uint8_t *read = src.buf + src.rec[r].seq_start - src.origin[2 * r];
+    cg_cut_spans(read, src.origin[2 * r + 1], v.is_rc && !a.swapped, a.cut_front, a.cut_back, pr.cut_last[a.mate][0],
+                 pr.cut_last[a.mate][1], &v.cut_prefix, &v.cut_suffix);
+    const int ws = a.qtrim ? a.qtrim[2 * r] : 0, we = a.qtrim ? a.qtrim[2 * r + 1] : a.seq_len[r];
+    cg_last_match(blob, pr, a.mate, a.buf + m.seq_start, ws, we,
+                  a.matches ? a.matches + (size_t)r * a.times * a.slots : nullptr, a.times, a.slots, &v);
+    return v;
+}
+
+// step 2 (cg_rename): the template; pairs (m2.buf) evaluate both mates before either record moves to its new name
+template <bool WRITE>
+__global__ void fq_names_rename_kernel(const uint8_t *blob, CgNameMate m1, CgNameMate m2, long long n, int32_t *len1,
+                                       int32_t *len2, const int64_t *off1, const int64_t *off2, uint32_t arena1,
+                                       uint32_t arena2, int casava, unsigned long long *mismatch)
+{
+    const long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= n) return;
+    const CgNameProg &pr = *(const CgNameProg *)blob;
+    const bool pair = m2.buf != nullptr;
+    CgNameVars v[2];
+    v[0] = fq_name_vars(blob, m1, m2, r);
+    v[1] = pair ? fq_name_vars(blob, m2, m1, r) : v[0];
+    if (!WRITE) {
+        CgNameCount c1;
+        cg_rename(blob, pr, v[0], v, 1, c1);
+        len1[r] = (int32_t)c1.n;
+        if (pair) {
+            CgNameCount c2;
+            cg_rename(blob, pr, v[1], v, 2, c2);
+            len2[r] = (int32_t)c2.n;
+        }
+        return;
+    }
+    CgNameWrite w1, w2;
+    w1.p = m1.buf + arena1 + off1[r];
+    cg_rename(blob, pr, v[0], v, 1, w1);
+    if (pair) {
+        w2.p = m2.buf + arena2 + off2[r];
+        cg_rename(blob, pr, v[1], v, 2, w2);
+        // PairedEndRenamer (modifiers.py:717-735): the step-1 names must name mates (code 1), and so must the new
+        // ones (code 2); the smallest pair is reported, as pair << 1 | (code - 1) keeps the input check of a pair first
+        if (!fq_mates_match(v[0].header.p, v[0].header.len, v[1].header.p, v[1].header.len))
+            atomicMin(mismatch, (unsigned long long)r << 1);
+        else if (!fq_mates_match(w1.p, (int)w1.n, w2.p, (int)w2.n))
+            atomicMin(mismatch, ((unsigned long long)r << 1) | 1ull);
+        m2.rec[r].hdr_start = arena2 + (uint32_t)off2[r];
+        m2.rec[r].hdr_len = (int32_t)w2.n;
+        if (casava & 2) m2.mask[r] = (m2.mask[r] & ~16) | (fq_casava_filtered(w2.p, (int)w2.n) ? 16 : 0);
+    }
+    m1.rec[r].hdr_start = arena1 + (uint32_t)off1[r];
+    m1.rec[r].hdr_len = (int32_t)w1.n;
+    if (casava & 1) m1.mask[r] = (m1.mask[r] & ~16) | (fq_casava_filtered(w1.p, (int)w1.n) ? 16 : 0);
+}
+
 }  // namespace
 
 // ------------------------------------------------------------------------------------------
@@ -1350,6 +1443,26 @@ cudaError_t cg_launch_fastq_info(int phase, const uint8_t *d_buf, const CgFastqR
         long long grid = (n_records + 7) / 8;
         grid = cg_grid_cap(grid, 16);
         fq_info_write_kernel<<<(unsigned)grid, 256, 0, st>>>(a, n_records, d_row_off, d_out);
+    }
+    return cudaGetLastError();
+}
+
+cudaError_t cg_launch_fastq_names(int phase, int rename, const uint8_t *d_blob, CgNameMate m1, CgNameMate m2,
+                                  long long n_records, int32_t *d_len1, int32_t *d_len2, const int64_t *d_off1,
+                                  const int64_t *d_off2, uint32_t arena1, uint32_t arena2, int casava,
+                                  unsigned long long *d_mismatch, cudaStream_t st)
+{
+    if (n_records <= 0) return cudaSuccess;
+    const unsigned grid = (unsigned)((n_records + 127) / 128);
+    if (!rename) {
+        if (phase == 0) fq_names_pre_kernel<false><<<grid, 128, 0, st>>>(d_blob, m1, n_records, d_len1, nullptr, 0, 0);
+        else fq_names_pre_kernel<true><<<grid, 128, 0, st>>>(d_blob, m1, n_records, nullptr, d_off1, arena1, casava);
+    } else if (phase == 0) {
+        fq_names_rename_kernel<false><<<grid, 128, 0, st>>>(d_blob, m1, m2, n_records, d_len1, d_len2, nullptr, nullptr, 0,
+                                                            0, 0, nullptr);
+    } else {
+        fq_names_rename_kernel<true><<<grid, 128, 0, st>>>(d_blob, m1, m2, n_records, nullptr, nullptr, d_off1, d_off2,
+                                                           arena1, arena2, casava, d_mismatch);
     }
     return cudaGetLastError();
 }

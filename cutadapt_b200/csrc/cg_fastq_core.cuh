@@ -155,6 +155,14 @@ CG_HD void fa_record_core(uint32_t hdr_start, int hdr_len, uint32_t seq_end, int
     *seq_len = len;
 }
 
+// CasavaFiltered (predicates.py:125-139) on a name: name.partition(" ")[2][1:4] == ":Y:"
+CG_HD bool fq_casava_filtered(const uint8_t *h, int hl)
+{
+    int sp = 0;
+    while (sp < hl && h[sp] != ' ') ++sp;
+    return sp + 4 < hl && h[sp + 2] == ':' && h[sp + 3] == 'Y' && h[sp + 4] == ':';
+}
+
 struct FqVerdict {
     int start, stop;         // what is written: read[start:stop] (relative to the record's sequence after -u)
     int k0, k1;              // the part the action leaves untouched ("remainder")
@@ -301,14 +309,7 @@ CG_HD FqVerdict fq_evaluate_core(const uint8_t *buf, const CgFastqRecord &rec, i
             if (f.max_aer > 0.0 && left > 0 && ee / (double)left > f.max_aer) mask |= 128;
         }
     }
-    if (f.discard_casava) {
-        // name.partition(" ")[2][1:4] == ":Y:"
-        const uint8_t *h = buf + rec.hdr_start;
-        const int hl = rec.hdr_len;
-        int sp = 0;
-        while (sp < hl && h[sp] != ' ') ++sp;
-        if (sp + 4 < hl && h[sp + 2] == ':' && h[sp + 3] == 'Y' && h[sp + 4] == ':') mask |= 16;
-    }
+    if (f.discard_casava && fq_casava_filtered(buf + rec.hdr_start, rec.hdr_len)) mask |= 16;
     if (matched) mask |= 32; else mask |= 64;          // masked by the enabled filters in the finish step
     v.start = start; v.stop = stop; v.k0 = k0; v.k1 = k1; v.mask = mask; v.last_adapter = last_adapter;
     v.matched = matched;

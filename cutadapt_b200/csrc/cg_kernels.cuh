@@ -183,6 +183,33 @@ cudaError_t cg_launch_fastq_dest(const int32_t *d_mask1, const int32_t *d_mask2,
 cudaError_t cg_launch_fastq_demux(int phase, const int32_t *d_out_len, const int32_t *d_dest, long long n_records,
                                   int n_dest, int32_t *d_bytes, const int64_t *d_base, int64_t *d_out_off, cudaStream_t st);
 // --info-file rows: phase 0 = bytes of every record's rows, phase 1 (after a scan) = the rows
+// ---- read names (cg_names_core.cuh): the name stage of a collect ----
+#include "cg_names_core.cuh"
+// One mate of the stage: its chunk (the names go into an arena behind the chunk's bytes, in the same buffer, and the
+// record table is repointed at them), its record table and verdict, its matches, and where -u took its bases.
+struct CgNameMate {
+    uint8_t *buf;
+    CgFastqRecord *rec;
+    const int32_t *interval;      // the read as written: LengthTagModifier's length
+    int32_t *mask;                // fail_mask: last adapter, RC bit; the CasavaFiltered bit is redone on the new name
+    const int32_t *origin;        // (bases in front of the record in the read as it came, length of that read)
+    const int32_t *seq_len, *qtrim;
+    const cg_match_rec *matches;
+    int times, slots;
+    int mate;                     // 0 = R1 / single-end, 1 = R2
+    int rc_suffix;                // the writers' " rc": the start name gets it instead
+    int swapped;                  // paired --revcomp: a turned pair's reads sit in the other mate's slot (no reversal)
+    int cut_front, cut_back;      // -u totals of this mate
+};
+// phase 0: bytes of every record's name (d_len1 / d_len2); phase 1: the names at arena + d_off, records repointed.
+// rename 0: step 1 (tag, suffixes, prefix / suffix) per record of m1; rename 1: the template over the step-1 names, one
+// thread per record of m1 or pair (m2.buf != nullptr); a pair whose step-1 names (code 0) or new names (code 1) do not
+// name mates sets *d_mismatch to min(pair << 1 | code).  casava: bit 0 / bit 1 = --discard-casava of m1 / m2 (step 1:
+// bit 0 for m1), its bit is redone on the final names.
+cudaError_t cg_launch_fastq_names(int phase, int rename, const uint8_t *d_blob, CgNameMate m1, CgNameMate m2,
+                                  long long n_records, int32_t *d_len1, int32_t *d_len2, const int64_t *d_off1,
+                                  const int64_t *d_off2, uint32_t arena1, uint32_t arena2, int casava,
+                                  unsigned long long *d_mismatch, cudaStream_t st);
 cudaError_t cg_launch_fastq_info(int phase, const uint8_t *d_buf, const CgFastqRecord *d_rec, const int32_t *d_origin,
                                  const int32_t *d_interval, const int32_t *d_mask, const cg_match_rec *d_matches, int times,
                                  int slots, const uint8_t *d_names, const int32_t *d_name_off, int revcomp, int rc_suffix,

@@ -20,12 +20,13 @@ chunk is one fused kernel launch:
 Reads shard across ranks by contiguous ranges (``shard_range``); no read ever needs another rank.
 """
 import ctypes as C
+import re
 from typing import List, Optional, Sequence, Tuple
 
 import numpy as np
 
 from . import _lib
-from .adapters import Matchable, MultipleAdapters
+from .adapters import LinkedAdapter, Matchable, MultipleAdapters
 
 
 # ---- statistics vector layout (include/cutadapt_b200.h: cg_stats_accumulate_device) ----------
@@ -1168,6 +1169,124 @@ def _read_rows(ctx, slot: int, kinds) -> dict:
     return rows
 
 
+# ---- read names (cg_names_*): --length-tag, --strip-suffix, -x / -y, --rename ----
+RENAME_VARIABLES = ("header", "id", "comment", "cut_prefix", "cut_suffix", "adapter_name", "rc", "match_sequence")
+_NAME_KINDS = {v: i + 1 for i, v in enumerate(RENAME_VARIABLES)}
+_NAME_KINDS["rn"] = 9
+LENGTH_TAG_CHARACTERS = "_=:,;/-@#%!~"
+
+
+def _tokenize_braces(text: str):
+    """tokenize_braces of the reference: (is a variable, value) in order; a stray brace is an error."""
+    for value in re.split(r"(\{[^}]*\})", text):
+        if value == "":
+            continue
+        brace = value.startswith("{") and value.endswith("}")
+        if brace:
+            value = value[1:-1]
+        for ch in "{}":
+            if ch in value:
+                raise ValueError(f"Unexpected '{ch}' encountered")
+        yield brace, value
+
+
+def rename_tokens(template: str, paired: bool = False) -> list:
+    """The --rename template as (kind, mate, literal text) tokens for cg_names_create, with the reference's errors as
+    ValueError (Renamer / PairedEndRenamer.__init__, modifiers.py:620-633, 706-711): the single-end template has "\\t"
+    replaced by a tab before it is tokenized, the paired one after."""
+    if not paired:
+        template = template.replace(r"\t", "\t")
+    try:
+        tokens = list(_tokenize_braces(template))
+    except ValueError as e:
+        raise ValueError(f"Error in template '{template}': {e}") from None
+    allowed = set(RENAME_VARIABLES)
+    if paired:
+        allowed = (allowed - {"rc"}) | {"rn"}
+        for v in set(RENAME_VARIABLES) - {"id", "rc"}:
+            allowed |= {"r1." + v, "r2." + v}
+    for brace, value in tokens:
+        if brace and value not in allowed:
+            raise ValueError(f"Error in template: Variable '{value}' not recognized")
+    out = []
+    for brace, value in tokens:
+        if not brace:
+            out.append((0, 0, value.replace(r"\t", "\t") if paired else value))
+        elif value[:3] in ("r1.", "r2."):
+            out.append((_NAME_KINDS[value[3:]], int(value[1]), ""))
+        else:
+            out.append((_NAME_KINDS[value], 0, ""))
+    return out
+
+
+def check_length_tag(tag: str) -> None:
+    """The length tags the device takes: literal text without regular-expression meaning."""
+    if tag == "":
+        raise ValueError("the length tag must not be empty")
+    for ch in tag:
+        if not (ch.isascii() and ch.isalnum()) and ch not in LENGTH_TAG_CHARACTERS:
+            raise ValueError(f"length tag {tag!r}: the character {ch!r} has a meaning in the reference's regular "
+                             f"expression; only letters, digits and {' '.join(LENGTH_TAG_CHARACTERS)} are accepted")
+
+
+def _names_wanted(rename, prefix, suffix, strip_suffix, length_tag) -> bool:
+    return rename is not None or bool(prefix) or bool(suffix) or bool(strip_suffix) or length_tag is not None
+
+
+def _make_names(ctx, rename, prefix, suffix, strip_suffix, length_tag, paired: bool):
+    """A names handle, or None when nothing changes a name.  An empty template is no --rename, and --rename '{header}'
+    installs no renamer (cli.py:982-990 test the template for truth and for "{header}")."""
+    rename = rename or None
+    if rename is not None and (prefix or suffix):
+        raise ValueError("Option --rename cannot be combined with --prefix (-x) or --suffix (-y)")
+    if rename is not None:
+        rename_tokens(rename, paired)           # the reference's template errors, "{header}" included
+    if rename == "{header}":
+        rename = None
+    if not _names_wanted(rename, prefix, suffix, strip_suffix, length_tag):
+        return None
+    if length_tag is not None:
+        check_length_tag(length_tag)
+    tokens = rename_tokens(rename, paired) if rename is not None else None
+    return _lib.Names(ctx, length_tag, tuple(strip_suffix or ()), prefix or "", suffix or "", tokens, paired)
+
+
+def _name_table(adapters, pair_list: bool = False):
+    """(adapter names by match-record index, linked flags): a linked adapter's parts carry its own name, as for
+    demultiplexing; with --pair-adapters, pair i of the list."""
+    if adapters is None:
+        return [], []
+    if pair_list:
+        return [str(a.name) for a in adapters], [0] * len(adapters)
+    singles, groups, owners = adapters._flatten()
+    names = [str(s.name) for s in singles]
+    linked = [0] * len(singles)
+    for (typ, a0, a1, _, _), owner in zip(groups, owners):
+        if typ == _lib.CG_GROUP_LINKED:
+            names[a0] = names[a1] = str(owner.name)
+            linked[a0] = linked[a1] = 1
+    return names, linked
+
+
+def _last_cuts(cut) -> Tuple[int, int]:
+    """The last -u value of each end: the bases {cut_prefix} / {cut_suffix} show."""
+    front = [int(c) for c in cut if c > 0]
+    back = [-int(c) for c in cut if c < 0]
+    return (front[-1] if front else 0), (back[-1] if back else 0)
+
+
+def _keep_chunk(ctx, chunk):
+    """The plain bytes of a chunk, read back from its slot when the device holds it: a collect with read names may
+    have to run the chunk again with a larger output buffer."""
+    if not isinstance(chunk, DeviceChunk):
+        return chunk
+    n = C.c_int64(0)
+    buf = np.empty(chunk.size, dtype=np.uint8)
+    _lib.check(_lib.lib().cg_fastq_slot_read(ctx.handle, chunk.slot, buf.ctypes.data if buf.size else None, buf.size,
+                                             C.byref(n)))
+    return buf[: n.value]
+
+
 class FastqTrimmer:
     """
     FASTQ chunks in, trimmed FASTQ chunks out -- the per-chunk worker of the reference
@@ -1217,6 +1336,12 @@ class FastqTrimmer:
                         ``last_rows`` = {kind: bytes} for the chunk it just returned or yielded
     gzip_rows           names out of ``rows`` whose rows are compressed on the device (gzip members as for
                         gzip_outputs)
+    length_tag, strip_suffix, prefix, suffix, rename
+                        --length-tag / --strip-suffix / -x / -y / --rename, last in the chain and on the device
+                        (cg_names_*): every output and row gets the new names.  A length tag may hold letters, digits and
+                        _ = : , ; / - @ # % ! ~ only; template and tag errors are ValueError, with the reference's
+                        messages; --rename '{header}' renames nothing.  Pass rc_suffix=False with rename, as the
+                        command line does
 
     ``process_chunk(bytes) -> bytes``; ``process_chunks(iterable)`` keeps one chunk in flight so that the
     upload of chunk i+1 overlaps the download of chunk i.  With ``redirect``: ``process_chunk_split(bytes) ->
@@ -1236,7 +1361,9 @@ class FastqTrimmer:
                  ctx: Optional[_lib.Context] = None, collect_statistics: bool = False,
                  redirect: Sequence[str] = (), redirect_formats: Optional[dict] = None,
                  gzip_outputs: Sequence[str] = (), rows: Sequence[str] = (), gzip_rows: Sequence[str] = (),
-                 max_average_error_rate: Optional[float] = None, zero_cap: bool = False):
+                 max_average_error_rate: Optional[float] = None, zero_cap: bool = False,
+                 rename: Optional[str] = None, prefix: str = "", suffix: str = "", strip_suffix: Sequence[str] = (),
+                 length_tag: Optional[str] = None):
         self.rows, self.gzip_rows = _row_kinds(rows, gzip_rows)
         self.input_format = input_format
         self.params = _fastq_params(times, quality_cutoff, quality_base, nextseq_cutoff, minimum_length, maximum_length,
@@ -1249,6 +1376,10 @@ class FastqTrimmer:
         self._redirect, self._fasta_outputs = _redirect_bits(self.redirect, redirect_formats, self.params)
         self.ctx = ctx or _lib.default_context()
         self.adapters, self._set = _device_set(adapters, self.ctx)
+        self._names = _make_names(self.ctx, rename, prefix, suffix, strip_suffix, length_tag, False)
+        if self._names is not None:
+            self._names.set_mate(0, *_name_table(self.adapters), *_last_cuts(cut))
+            self.params.names = self._names.handle
         self._stats = None
         if collect_statistics:
             n = len(self.adapters._flatten()[0]) if self.adapters is not None else 0
@@ -1308,18 +1439,36 @@ class FastqTrimmer:
             self._out_bufs[slot] = buf
         return buf
 
+    def _keep(self, chunk):
+        """A device chunk as bytes when read names may make a collect run it again (see _again)."""
+        return _keep_chunk(self.ctx, chunk) if self._names is not None else chunk
+
+    def _again(self, rc: int, res, out, chunk, slot):
+        """After a collect that failed because its output did not fit (" rc" suffixes in FASTA, longer read names;
+        the call says how much it needs): the ticket of the chunk submitted again, else None."""
+        grows = self._names is not None or self.params.format != _lib.CG_FORMAT_FASTQ
+        if rc == 0 or not grows or res.out_bytes <= out.size or isinstance(chunk, DeviceChunk):
+            return None
+        kinds = self._slot_rows.pop(slot, None)
+        if self.input_format == "bam":              # the slot held the decoded records as FASTQ text
+            slot, buf = _submit_chunk(self.ctx, chunk)
+            _request_rows(self.ctx, slot, kinds, self._texts(kinds), self.gzip_rows)
+            self._slot_rows[slot] = kinds
+            return slot, buf.size, buf
+        return self._submit(chunk, kinds)
+
     def _collect(self, ticket, copy: bool = True):
         slot, n_bytes, chunk = ticket
-        out = self._out_buffer(slot, self._capacity(n_bytes, chunk=chunk))
+        chunk = self._keep(chunk)
+        out = self._out_buffer(slot, self._capacity(n_bytes, chunk=ticket[2]))
         while True:
             res = _lib.cg_fastq_result()
             rc = _lib.lib().cg_fastq_collect(
                 self.ctx.handle, slot, self._set.handle if self._set is not None else None, C.byref(self.params),
                 out.ctypes.data, out.size, C.byref(res))
-            # FASTA output: " rc" suffixes can exceed the bound; the call says how much it needs, run the chunk again
-            if (rc != 0 and self.params.format != _lib.CG_FORMAT_FASTQ and res.out_bytes > out.size
-                    and not isinstance(chunk, DeviceChunk)):
-                slot, _, chunk = self._submit(chunk, self._slot_rows.pop(slot, None))
+            again = self._again(rc, res, out, chunk, slot)
+            if again is not None:
+                slot, _, chunk = again
                 out = self._out_buffer(slot, res.out_bytes)
                 continue
             _lib.check(rc)
@@ -1339,16 +1488,20 @@ class FastqTrimmer:
 
     def _collect_split(self, ticket, copy: bool = True) -> dict:
         slot, n_bytes, chunk = ticket
-        out = self._out_buffer(slot, self._capacity(n_bytes, chunk=chunk))
+        chunk = self._keep(chunk)
+        out = self._out_buffer(slot, self._capacity(n_bytes, chunk=ticket[2]))
         segments = np.zeros(5, dtype=np.int64)
         while True:
             res = _lib.cg_fastq_result()
             rc = _lib.lib().cg_fastq_collect_split(
                 self.ctx.handle, slot, self._set.handle if self._set is not None else None, C.byref(self.params),
                 self._redirect, self._fasta_outputs, out.ctypes.data, out.size, C.byref(res), segments.ctypes.data)
-            # " rc" suffixes can exceed the bound; the call says how much it needs, run the chunk again
-            if rc != 0 and res.out_bytes > out.size and not isinstance(chunk, DeviceChunk):
-                slot, _, chunk = self._submit(chunk, self._slot_rows.pop(slot, None))
+            # " rc" suffixes and read names can exceed the bound; the call says how much it needs, run the chunk again
+            again = self._again(rc, res, out, chunk, slot)
+            if again is None and rc != 0 and res.out_bytes > out.size and not isinstance(chunk, DeviceChunk):
+                again = self._submit(chunk, self._slot_rows.pop(slot, None))
+            if again is not None:
+                slot, _, chunk = again
                 out = self._out_buffer(slot, res.out_bytes)
                 continue
             _lib.check(rc)
@@ -1378,12 +1531,20 @@ class FastqTrimmer:
         self._no_redirect("demultiplexing")
         outputs, dest = self._demux_names()
         slot, n_bytes, _ = self._submit(chunk)
+        chunk = self._keep(chunk)
         out = self._out_buffer(slot, self._capacity(n_bytes, len(outputs) + 1))
-        res = _lib.cg_fastq_result()
         segments = np.zeros(len(outputs) + 2, dtype=np.int64)
-        _lib.check(_lib.lib().cg_fastq_collect_demux(
-            self.ctx.handle, slot, self._set.handle, C.byref(self.params), dest.ctypes.data, len(outputs),
-            out.ctypes.data, out.size, C.byref(res), segments.ctypes.data))
+        while True:
+            res = _lib.cg_fastq_result()
+            rc = _lib.lib().cg_fastq_collect_demux(
+                self.ctx.handle, slot, self._set.handle, C.byref(self.params), dest.ctypes.data, len(outputs),
+                out.ctypes.data, out.size, C.byref(res), segments.ctypes.data)
+            again = self._again(rc, res, out, chunk, slot)
+            if again is None:
+                _lib.check(rc)
+                break
+            slot, _, chunk = again
+            out = self._out_buffer(slot, res.out_bytes)
         self._account(res)
         self._take_rows(slot)
         return {name: out[segments[i]:segments[i + 1]].tobytes() for i, name in enumerate(outputs + [unknown])}
@@ -1496,6 +1657,10 @@ class PairedFastqTrimmer:
     output gets R1's read trimmed by the -A set, both names with " rc" unless rc_suffix is False.  Without adapters it
     does nothing.  ``statistics[k]["reverse_complemented"]`` counts the swapped pairs; each adapter's
     ``reverse_complemented`` its matches in swapped pairs.  Not with ``pair_adapters`` or info rows.
+
+    ``length_tag`` / ``strip_suffix`` / ``prefix`` / ``suffix`` / ``rename``: as for FastqTrimmer, on both mates; the
+    template is PairedEndRenamer's ({rn}, {r1.x} / {r2.x}), and a pair whose new IDs no longer name mates fails the call
+    with the reference's message.
     """
 
     MODES = {"any": 0, "both": 1, "first": 2}
@@ -1508,7 +1673,8 @@ class PairedFastqTrimmer:
                  interleaved_outputs: Sequence[str] = (), gzip_outputs: Sequence[str] = (),
                  gzip_outputs2: Optional[Sequence[str]] = None, rows: Sequence[str] = (),
                  rows2: Sequence[str] = (), gzip_rows: Sequence[str] = (), gzip_rows2: Optional[Sequence[str]] = None,
-                 revcomp: bool = False, rc_suffix: bool = True):
+                 revcomp: bool = False, rc_suffix: bool = True, rename: Optional[str] = None, prefix: str = "",
+                 suffix: str = "", strip_suffix: Sequence[str] = (), length_tag: Optional[str] = None):
         if pair_filter not in self.MODES:
             raise ValueError("pair_filter must be 'any', 'both' or 'first'")
         if input_format == "bam":
@@ -1576,6 +1742,15 @@ class PairedFastqTrimmer:
             self._stats = tuple(_lib.FastqStatistics(self.ctx, n) for n in counts)
             self.params1.stats, self.params2.stats = self._stats[0].handle, self._stats[1].handle
         pair_list = self._pairs is not None
+        self._names = _make_names(self.ctx, rename, prefix, suffix, strip_suffix, length_tag, True)
+        if self._names is not None and pair_list and rename and "match_sequence" in rename and any(
+                isinstance(a, LinkedAdapter) for a in self.adapters1 + self.adapters2):
+            # a linked adapter of a --pair-adapters list matches as one adapter here: its front,back form is not kept
+            raise ValueError("{match_sequence} cannot be combined with linked adapters under --pair-adapters")
+        if self._names is not None:
+            for mate, (adapters, options) in enumerate(((self.adapters1, options1), (self.adapters2, options2))):
+                self._names.set_mate(mate, *_name_table(adapters, pair_list), *_last_cuts((options or {}).get("cut", ())))
+            self.params1.names = self.params2.names = self._names.handle
         self._row_texts = ({k: _row_text(self.adapters1, k, pair_list) for k in self.rows},
                            {k: _row_text(self.adapters2, k, pair_list) for k in self.rows2})
 
@@ -1640,7 +1815,30 @@ class PairedFastqTrimmer:
         r1, r2 = _read_rows(self.ctx, s1, self.rows), _read_rows(self.ctx, s2, self.rows2)
         self.last_rows = {k: (r1.get(k, b""), r2.get(k, b"")) for k in ROW_KINDS if k in r1 or k in r2}
 
-    def _out_buffers(self, tickets, n_dest: int = 4):
+    def _run(self, tickets, call, n_dest: int = 4):
+        """(tickets, out1, out2, r1, r2) of call(tickets, out1, out2, r1, r2) -> rc.  With read names an output can
+        outgrow its bound: the call then says how much it needs and the pair is submitted and run again."""
+        kept = None
+        if self._names is not None:
+            (_, b1), (_, b2) = tickets
+            if b1 is b2:                                # one interleaved chunk (a device chunk: read from its first slot)
+                kept = (_keep_chunk(self.ctx, b1), None)
+            else:
+                kept = (_keep_chunk(self.ctx, b1), _keep_chunk(self.ctx, b2))
+        need = (0, 0)
+        while True:
+            out1, out2 = self._out_buffers(tickets, n_dest, need)
+            r1, r2 = _lib.cg_fastq_result(), _lib.cg_fastq_result()
+            rc = call(tickets, out1, out2, r1, r2)
+            cap1 = out1.size - (out2.size if self._interleave else 0)
+            if rc != 0 and kept is not None and (r1.out_bytes > cap1 or r2.out_bytes > out2.size):
+                need = (max(r1.out_bytes, cap1), max(r2.out_bytes, out2.size))
+                tickets = self._submit_pair(*kept)
+                continue
+            _lib.check(rc)
+            return tickets, out1, out2, r1, r2
+
+    def _out_buffers(self, tickets, n_dest: int = 4, need=(0, 0)):
         """Output buffers of a pair: out1 also holds R2 of the interleaved outputs.  With --revcomp either mate's output
         can receive the other mate's records, each with " rc" (3 bytes on a FASTQ record of at least 6)."""
         (_, b1), (_, b2) = tickets
@@ -1652,6 +1850,7 @@ class PairedFastqTrimmer:
         else:
             n1 = _output_capacity(b1.size, self.params1.format, self.params1.gzip_outputs != 0, n_dest)
             n2 = _output_capacity(b2.size, self.params2.format, self.params2.gzip_outputs != 0, n_dest)
+        n1, n2 = max(n1, need[0]), max(n2, need[1])
         return np.empty(n1 + (n2 if self._interleave else 0), dtype=np.uint8), np.empty(n2, dtype=np.uint8)
 
     def _no_interleave(self, what: str):
@@ -1669,22 +1868,23 @@ class PairedFastqTrimmer:
                              "use process_chunk_split / process_chunks_split")
 
     def _collect_split(self, tickets) -> dict:
-        (s1, b1), (s2, b2) = tickets
-        out1, out2 = self._out_buffers(tickets)
-        r1, r2 = _lib.cg_fastq_result(), _lib.cg_fastq_result()
         seg1, seg2 = np.zeros(5, dtype=np.int64), np.zeros(5, dtype=np.int64)
         sets = (self._set1.handle if self._set1 is not None else None,
                 self._set2.handle if self._set2 is not None else None)
-        if self._interleave:
-            _lib.check(_lib.lib().cg_fastq_collect_paired_interleaved(
-                self.ctx.handle, s1, s2, *sets, C.byref(self.params1), C.byref(self.params2), self.mode,
-                self._redirect, self._fasta_outputs, self._interleave, out1.ctypes.data, out1.size, out2.ctypes.data,
-                out2.size, C.byref(r1), C.byref(r2), seg1.ctypes.data, seg2.ctypes.data))
-        else:
-            _lib.check(_lib.lib().cg_fastq_collect_paired_split(
+
+        def call(tickets, out1, out2, r1, r2):
+            (s1, _), (s2, _) = tickets
+            if self._interleave:
+                return _lib.lib().cg_fastq_collect_paired_interleaved(
+                    self.ctx.handle, s1, s2, *sets, C.byref(self.params1), C.byref(self.params2), self.mode,
+                    self._redirect, self._fasta_outputs, self._interleave, out1.ctypes.data, out1.size,
+                    out2.ctypes.data, out2.size, C.byref(r1), C.byref(r2), seg1.ctypes.data, seg2.ctypes.data)
+            return _lib.lib().cg_fastq_collect_paired_split(
                 self.ctx.handle, s1, s2, *sets, C.byref(self.params1), C.byref(self.params2), self.mode,
                 self._redirect, self._fasta_outputs, out1.ctypes.data, out1.size, out2.ctypes.data, out2.size,
-                C.byref(r1), C.byref(r2), seg1.ctypes.data, seg2.ctypes.data))
+                C.byref(r1), C.byref(r2), seg1.ctypes.data, seg2.ctypes.data)
+
+        tickets, out1, out2, r1, r2 = self._run(tickets, call)
         self._account(r1, r2)
         self._take_rows(tickets)
         names = ("output",) + REDIRECT_OUTPUTS
@@ -1710,20 +1910,19 @@ class PairedFastqTrimmer:
         self._no_redirect("process_chunk")
         if self._interleave:
             return self._collect_split(self._submit_pair(chunk1, chunk2))["output"]
-        tickets = self._submit_pair(chunk1, chunk2)
-        (s1, b1), (s2, b2) = tickets
-        out1, out2 = self._out_buffers(tickets)
-        r1, r2 = _lib.cg_fastq_result(), _lib.cg_fastq_result()
-        if self._pairs is not None:
-            _lib.check(_lib.lib().cg_fastq_collect_pair_adapters(
-                self.ctx.handle, s1, s2, self._pair_handles[0], self._pair_handles[1], len(self._pairs),
-                C.byref(self.params1), C.byref(self.params2), self.mode, out1.ctypes.data, out1.size, out2.ctypes.data,
-                out2.size, C.byref(r1), C.byref(r2)))
-        else:
-            _lib.check(_lib.lib().cg_fastq_collect_paired(
+        def call(tickets, out1, out2, r1, r2):
+            (s1, _), (s2, _) = tickets
+            if self._pairs is not None:
+                return _lib.lib().cg_fastq_collect_pair_adapters(
+                    self.ctx.handle, s1, s2, self._pair_handles[0], self._pair_handles[1], len(self._pairs),
+                    C.byref(self.params1), C.byref(self.params2), self.mode, out1.ctypes.data, out1.size,
+                    out2.ctypes.data, out2.size, C.byref(r1), C.byref(r2))
+            return _lib.lib().cg_fastq_collect_paired(
                 self.ctx.handle, s1, s2, self._set1.handle if self._set1 is not None else None,
                 self._set2.handle if self._set2 is not None else None, C.byref(self.params1), C.byref(self.params2),
-                self.mode, out1.ctypes.data, out1.size, out2.ctypes.data, out2.size, C.byref(r1), C.byref(r2)))
+                self.mode, out1.ctypes.data, out1.size, out2.ctypes.data, out2.size, C.byref(r1), C.byref(r2))
+
+        tickets, out1, out2, r1, r2 = self._run(self._submit_pair(chunk1, chunk2), call)
         self._account(r1, r2)
         self._take_rows(tickets)
         return out1[: r1.out_bytes].tobytes(), out2[: r2.out_bytes].tobytes()
@@ -1754,17 +1953,18 @@ class PairedFastqTrimmer:
             dest2, n2 = None, 0
             keys = names1 + [unknown]
             keep = np.array([1] * n1 + [0 if discard_untrimmed else 1], dtype=np.uint8)
-        tickets = self._submit_pair(chunk1, chunk2)
-        (s1, b1), (s2, b2) = tickets
-        out1, out2 = self._out_buffers(tickets, len(keys))
-        r1, r2 = _lib.cg_fastq_result(), _lib.cg_fastq_result()
         seg1 = np.zeros(len(keys) + 1, dtype=np.int64)
         seg2 = np.zeros(len(keys) + 1, dtype=np.int64)
-        _lib.check(_lib.lib().cg_fastq_collect_paired_demux(
-            self.ctx.handle, s1, s2, self._set1.handle, self._set2.handle if self._set2 is not None else None,
-            C.byref(self.params1), C.byref(self.params2), self.mode, dest1.ctypes.data, n1,
-            dest2.ctypes.data if dest2 is not None else None, n2, keep.ctypes.data, out1.ctypes.data, out1.size,
-            out2.ctypes.data, out2.size, C.byref(r1), C.byref(r2), seg1.ctypes.data, seg2.ctypes.data))
+
+        def call(tickets, out1, out2, r1, r2):
+            (s1, _), (s2, _) = tickets
+            return _lib.lib().cg_fastq_collect_paired_demux(
+                self.ctx.handle, s1, s2, self._set1.handle, self._set2.handle if self._set2 is not None else None,
+                C.byref(self.params1), C.byref(self.params2), self.mode, dest1.ctypes.data, n1,
+                dest2.ctypes.data if dest2 is not None else None, n2, keep.ctypes.data, out1.ctypes.data, out1.size,
+                out2.ctypes.data, out2.size, C.byref(r1), C.byref(r2), seg1.ctypes.data, seg2.ctypes.data)
+
+        tickets, out1, out2, r1, r2 = self._run(self._submit_pair(chunk1, chunk2), call, len(keys))
         self._account(r1, r2)
         self._take_rows(tickets)
         return {key: (out1[seg1[i]:seg1[i + 1]].tobytes(), out2[seg2[i]:seg2[i + 1]].tobytes())

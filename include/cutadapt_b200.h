@@ -348,7 +348,10 @@ typedef struct cg_fastq_params {
     int32_t zero_cap;            /* -z / --zero-cap (ZeroCapper, modifiers.py:806-822), the last modifier: quality
                                     characters below trim.quality_base become trim.quality_base, for the filters and in
                                     every output; info rows of reads with a match keep the original qualities.  0 / 1 */
-    int32_t reserved_pad;        /* 0 */
+    int32_t names;               /* 0 = off, else a handle of cg_names_create (below): the read-name modifiers
+                                    (--length-tag, --strip-suffix, -x / -y, --rename) run on this mate's records.  Both
+                                    mates of a paired collect must give the same handle.  Without it a collect launches
+                                    exactly what it launches with 0 here. */
 } cg_fastq_params;
 typedef struct cg_fastq_result {
     int64_t n_records, n_written;
@@ -463,7 +466,8 @@ int cg_fastq_submit_gzip(cg_ctx *ctx, int32_t handle, const uint8_t *gz, int64_t
 /* The tiles of the BAM record-boundary walk a stream ran and those walked again because their speculative start was
  * not on the true chain, over the stream's life. */
 int cg_gzin_bam_tiles(cg_ctx *ctx, int32_t handle, int64_t *tiles, int64_t *rewalked);
-/* The plain chunk of a submitted, not yet collected slot (not a mate of an interleaved chunk), copied to host memory:
+/* The plain chunk of a submitted, not yet collected slot, copied to host memory (the first slot of an interleaved chunk
+ * returns the whole interleaved chunk; its second slot holds none):
  * what a caller keeps to submit a chunk from cg_fastq_submit_gzip again (a collect that needs a larger row buffer).
  * *n_bytes: its size; CG_EINVAL when capacity is smaller. */
 int cg_fastq_slot_read(cg_ctx *ctx, int32_t slot, uint8_t *dst, int64_t capacity, int64_t *n_bytes);
@@ -710,6 +714,68 @@ int cg_fastq_stats_create(cg_ctx *ctx, int32_t n_adapters, int32_t *handle);   /
 int cg_fastq_stats_read(cg_ctx *ctx, int32_t handle, int32_t *max_len, int32_t *kmax, int64_t *out, int64_t capacity,
                         int64_t *size, int reset);
 int cg_fastq_stats_destroy(cg_ctx *ctx, int32_t handle);
+
+/* ---- read names: --length-tag, --strip-suffix, -x / -y and --rename on the device ----
+ * The reference's name modifiers (LengthTagModifier, SuffixRemover, PrefixSuffixAdder, Renamer / PairedEndRenamer,
+ * modifiers.py:529-760) run last in its chain (cli.py:937-991, 1136-1146), after the adapters, --poly-a, --length and
+ * --trim-n; in pairs the first three run on each mate with that mate's own match.  A collect whose params name a names
+ * handle runs one name stage per mate once the matches and the written part of every read are final: after --revcomp,
+ * the pair swap, --pair-adapters and the filters' evaluation, before the rows and the sizing of the records.  Every
+ * output then carries the new name: main, filter, demultiplexed, interleaved and gzip outputs, FASTA output, and the
+ * info, rest and wildcard rows.  The name the chain starts from already carries the " rc" of --revcomp (revcomp = 1).
+ *   length_tag   TAG (NULL = off): when TAG occurs in the name, every non-overlapping match of \bTAG[0-9]*\b (Python
+ *                re, left to right; the longest digit run followed by a word boundary, possibly empty) becomes TAG
+ *                followed by the length of the sequence as written.  TAG is a literal here: only letters, digits and
+ *                _ = : , ; / - @ # % ! ~ are accepted (CG_EINVAL names any other character); "" is refused.
+ *   strip_suffix each value in order: removed once if the name ends with it ("" empties the name, as name[:-0] does)
+ *   prefix / suffix  (NULL = ""): prefix + name + suffix, "{name}" in either replaced by the adapter name of the read's
+ *                last match or "no_adapter"; no other brace is special.
+ *   rename / n_rename  the --rename template tokenized (tokenize_braces; the caller reports the reference's errors and
+ *                replaces a two-character \t by a tab in the literals); n_rename < 0: no renamer.  Variables:
+ *                header, id, comment (name.split(maxsplit=1) with Python's whitespace: one field or none gives the id
+ *                the whole name and an empty comment), cut_prefix / cut_suffix (the bases the last -u value of that end
+ *                removed; the 5' values are applied first), adapter_name, rc ("rc" / ""), match_sequence (the last
+ *                match's sequence[rstart:rstop] of the sequence its round searched, front + "," + back for a linked
+ *                match, "" without a match).  paired != 0 (PairedEndRenamer): rc is refused, rn (1 / 2) and the
+ *                mate forms (mate 1 = r1., 2 = r2.) of every variable but id and rc are allowed; each mate is
+ *                evaluated on its own record.  A pair whose step-1 names do not name mates (dnaio's rule) fails the
+ *                collect with "Input read IDs not identical: ..." (R1's ID and R1's comment, as the reference prints
+ *                them), a pair whose new IDs no longer do with "After renaming R1 and R2, ...", each naming the first
+ *                such pair.  Neither prefix nor suffix may be
+ *                given with a renamer.
+ * cg_names_set_mate: the adapter names of a mate's list, indexed as the match records index it (a linked adapter's
+ * parts both carry the linked adapter's name; with --pair-adapters, pair i of that mate's list), with linked[a] != 0
+ * for the parts of a linked adapter, and the last -u value of each end of that mate (>= 0).  A mate not set has no
+ * names ("no_adapter") and no -u cutter. */
+#define CG_NT_LITERAL 0
+#define CG_NT_HEADER 1
+#define CG_NT_ID 2
+#define CG_NT_COMMENT 3
+#define CG_NT_CUT_PREFIX 4
+#define CG_NT_CUT_SUFFIX 5
+#define CG_NT_ADAPTER_NAME 6
+#define CG_NT_RC 7
+#define CG_NT_MATCH_SEQUENCE 8
+#define CG_NT_RN 9
+typedef struct cg_name_token {
+    int32_t kind;                /* CG_NT_*                                                           */
+    int32_t mate;                /* 0 the record's own value, 1 {r1.x}, 2 {r2.x}                       */
+    const char *text;            /* CG_NT_LITERAL: the text (len bytes)                               */
+    int32_t len;
+} cg_name_token;
+typedef struct cg_names_desc {
+    const char *length_tag;
+    const char *const *strip_suffix;
+    int32_t n_strip_suffix;
+    int32_t paired;
+    const char *prefix, *suffix;
+    const cg_name_token *rename;
+    int32_t n_rename;
+} cg_names_desc;
+int cg_names_create(cg_ctx *ctx, const cg_names_desc *desc, int32_t *handle);   /* handle > 0 */
+int cg_names_set_mate(cg_ctx *ctx, int32_t handle, int32_t mate, const char *names, const int32_t *offsets,
+                      int32_t n_names, const uint8_t *linked, int32_t last_cut_front, int32_t last_cut_back);
+int cg_names_destroy(cg_ctx *ctx, int32_t handle);
 
 /* ---- host-side index helpers (adapters.py:1416-1442 use these to build AdapterIndex) ----
  * edit_environment (_align.pyx:785-882) / hamming_sphere-based environment

@@ -54,6 +54,7 @@ of the record-boundary walk and those walked again.  A second line: the BAM kern
 torch.profiler, in a run of its own.  The card's name and power limit are read in the run.
 """
 import json
+import os
 import subprocess
 import sys
 import time
@@ -550,7 +551,64 @@ def measure_paired_revcomp(n, chunk_mb):
                       "revcomp_over_plain_time": res["paired_revcomp"]["wall_s"] / res["paired"]["wall_s"]}))
 
 
+def measure_names(n, chunk_mb, baseline_tree=None):
+    """--names: the "fastq" variant without read names, with --rename '{id} {adapter_name} {comment}' and with
+    -y ' {name}' --length-tag length=, the three arms alternating over three rounds in one process; then, with a
+    baseline tree, its "fastq" run against this tree's (no names), alternating processes.  Both compile the run-time
+    specialised first stage at once (CUTADAPT_B200_JIT=1): by default it is compiled (~1 s of NVRTC) once a set has seen
+    4 Mi reads, which would fall inside one arm's timed round here and inside the single timed pass of a fresh process."""
+    os.environ["CUTADAPT_B200_JIT"] = "1"
+    data, rec_len = build_fastq(n)
+    per_chunk = max(1, (chunk_mb << 20) // rec_len)
+    chunks = [data[i * rec_len:min(n, i + per_chunk) * rec_len] for i in range(0, n, per_chunk)]
+    adapters = [PA.BackAdapter("AGATCGGAAGAGC", max_errors=0.1, name="adapter")]
+    opts = dict(quality_cutoff=(0, 20), minimum_length=20)
+    arms = {"no_names": FastqTrimmer(adapters, **opts),
+            "rename": FastqTrimmer(adapters, **opts, rename="{id} {adapter_name} {comment}"),
+            "suffix_length_tag": FastqTrimmer(adapters, **opts, suffix=" {name}", length_tag="length=")}
+
+    def run(name, cs):
+        return sum(len(o) for o in arms[name].process_chunks(cs, copy=False))
+
+    for name in arms:
+        run(name, chunks[:3])                     # warm-up: buffers, module load
+    res = {name: {"wall_s": 0.0, "round_s": []} for name in arms}
+    for _ in range(3):
+        for name in arms:
+            t0 = time.perf_counter()
+            res[name]["out_bytes"] = run(name, chunks)
+            res[name]["round_s"].append(time.perf_counter() - t0)
+            res[name]["wall_s"] += res[name]["round_s"][-1]
+    for r in res.values():
+        r["reads_per_s"] = 3 * n / r["wall_s"]
+    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader",
+                           "-i", str(torch.cuda.current_device())], capture_output=True, text=True).stdout.strip()
+    print(json.dumps({"what": "FASTQ (-a AGATCGGAAGAGC -q 20 -m 20), host to host: no read names, --rename "
+                              "'{id} {adapter_name} {comment}', -y ' {name}' --length-tag length=",
+                      "reads": n, "chunk_mb": chunk_mb, "chunks": len(chunks), "gpu": torch.cuda.get_device_name(),
+                      "card_and_power_limit": card, "arms": res}))
+    if baseline_tree is None:
+        return
+    runs = {"baseline": [], "this": []}
+    for _ in range(3):
+        for name, tree in (("baseline", baseline_tree), ("this", __file__.rsplit("/", 2)[0])):
+            out = subprocess.run([sys.executable, f"{tree}/tools/measure_fastq.py", str(n), str(chunk_mb), "fastq"],
+                                 capture_output=True, text=True, check=True).stdout
+            runs[name].append(json.loads(out.strip().split("\n")[-1])["reads_per_s"])
+    print(json.dumps({"what": "fastq variant without read names, this tree against the baseline tree, alternating "
+                              "processes", "card_and_power_limit": card, "reads_per_s": runs,
+                      "median": {k: sorted(v)[len(v) // 2] for k, v in runs.items()}}))
+
+
 def main():
+    if "--names" in sys.argv:
+        argv = [a for a in sys.argv if a != "--names"]
+        base = None
+        if "--baseline-tree" in argv:
+            i = argv.index("--baseline-tree")
+            base = argv[i + 1]
+            del argv[i:i + 2]
+        return measure_names(int(argv[1]) if len(argv) > 1 else 4_000_000, int(argv[2]) if len(argv) > 2 else 64, base)
     if "--revcomp" in sys.argv:
         argv = [a for a in sys.argv if a != "--revcomp"]
         return measure_paired_revcomp(int(argv[1]) if len(argv) > 1 else 4_000_000,

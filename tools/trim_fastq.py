@@ -52,6 +52,15 @@ is written, " rc" appended to its name (ReverseComplementer).  On pairs the -a a
 adapters on R1, and a pair that matches better that way is written with R1 and R2 swapped, " rc" on both names
 (PairedReverseComplementer); --info-file is refused there.  --json counts them in "reverse_complemented".
 
+Read names, as in the reference and in its order (after the adapters, --poly-a, --length and --trim-n; on pairs for
+each mate): --length-tag TAG replaces TAG followed by digits with TAG and the length of the read as written (TAG may
+hold letters, digits and _ = : , ; / - @ # % ! ~ only); --strip-suffix S (repeatable) removes S from the end of a name;
+-x / -y add a prefix / suffix in which {name} is the adapter of the last match (no_adapter without one); --rename
+TEMPLATE writes the name from the template's variables ({header}, {id}, {comment}, {cut_prefix}, {cut_suffix},
+{adapter_name}, {rc}, {match_sequence}; on pairs also {rn} and {r1.x} / {r2.x}) and turns the " rc" of --revcomp off.
+--rename cannot be combined with -x / -y.  Every output gets the new names, the row files included.  On pairs, -u
+cuts R1 and -U R2, as in the reference ({cut_prefix} / {cut_suffix} show what each cut).
+
 Row files: --info-file, -r/--rest-file and --wildcard-file get the rows of every read, filtered or not, formatted on the
 device next to every kind of output above.  On pairs they get R1's rows, as in the reference (PairedSingleEndStep,
 cli.py:675-696); --info-file-paired adds R2's info rows, and only together with --info-file; it also makes the run
@@ -267,6 +276,8 @@ def main():
     ap.add_argument("--quality-base", type=int, default=33)
     ap.add_argument("--nextseq-trim", type=int, default=None)
     ap.add_argument("-u", "--cut", type=int, action="append", default=[])
+    ap.add_argument("-U", dest="cut2", type=int, action="append", default=[],
+                    help="as -u, for R2 (-u then applies to R1 only)")
     ap.add_argument("-m", "--minimum-length", default=None, metavar="LEN[:LEN2]")
     ap.add_argument("-M", "--maximum-length", default=None, metavar="LEN[:LEN2]")
     ap.add_argument("--interleaved", action="store_true",
@@ -302,8 +313,17 @@ def main():
                     help="the info rows of the second mates (with --info-file)")
     ap.add_argument("-r", "--rest-file", metavar="FILE", help="write what follows (3') / precedes (5') the last match")
     ap.add_argument("--wildcard-file", metavar="FILE", help="write the read characters under the adapters' N positions")
+    ap.add_argument("--rename", metavar="TEMPLATE", default=None,
+                    help="rename reads with a template such as '{id} {adapter_name} {comment}'")
+    ap.add_argument("-x", "--prefix", default="", help="add this prefix to read names; {name}: the adapter name")
+    ap.add_argument("-y", "--suffix", default="", help="add this suffix to read names; {name}: the adapter name")
+    ap.add_argument("--strip-suffix", action="append", default=[], help="remove this suffix from read names")
+    ap.add_argument("--length-tag", metavar="TAG", default=None, help="replace TAG followed by a number with TAG and the "
+                                                                       "length of the trimmed read")
     ap.add_argument("inputs", nargs="+")
     args = ap.parse_args()
+    if args.rename and (args.prefix or args.suffix):
+        ap.error("Option --rename cannot be combined with --prefix (-x) or --suffix (-y)")     # cli.py:982-985
     if args.info_file2 and len(args.inputs) == 1 and not args.interleaved:
         # --info-file-paired enables paired-end mode (cli.py:525-538, 560-566)
         ap.error("You used an option that enables paired-end mode (such as -p, -A, -G, -B, -U), but only provided one "
@@ -369,7 +389,10 @@ def main():
                   trim_n=args.trim_n, discard_casava=args.discard_casava, action=args.action,
                   max_average_error_rate=args.max_aer, zero_cap=args.zero_cap)
     formats = dict(input_format=input_format, output_format=output_format, collect_statistics=args.json is not None)
-    revcomp1 = {} if paired else dict(revcomp=args.revcomp)
+    # --rename turns the " rc" suffix of --revcomp off (cli.py:964)
+    revcomp1 = {} if paired else dict(revcomp=args.revcomp, rc_suffix=not args.rename)
+    names = dict(rename=args.rename or None, prefix=args.prefix, suffix=args.suffix, strip_suffix=args.strip_suffix,
+                 length_tag=args.length_tag)
     # filter outputs (the untrimmed output of a demultiplexer is its "unknown" output)
     redirect = [d for d, _ in FILTER_OUTPUTS if getattr(args, d + "_output") and "{name}" not in args.output]
     split = dict(redirect=redirect,
@@ -407,12 +430,12 @@ def main():
             ap.error("paired-end input needs -p (or --interleaved for an interleaved output)")
         if len(args.inputs) == 2 and detect_format(args.inputs[1]) != input_format:
             ap.error("both inputs must have the same format")
-        options2 = dict(common, minimum_length=min2, maximum_length=max2)
+        options2 = dict(common, minimum_length=min2, maximum_length=max2, cut=args.cut2)   # -u is R1's, -U R2's
         # an output is interleaved when its paired path is missing (cli.py:650-661, 913-921)
         interleaved = [d for d in ["output"] + redirect
                        if not (args.paired_output if d == "output" else getattr(args, d + "_paired_output"))]
         t = PairedFastqTrimmer(ads1, ads2, common, options2, args.pair_filter, **formats, **split, revcomp=args.revcomp,
-                               interleaved_outputs=interleaved, gzip_outputs=gzip1, gzip_outputs2=gzip2, **rows,
+                               rc_suffix=not args.rename, **names, interleaved_outputs=interleaved, gzip_outputs=gzip1, gzip_outputs2=gzip2, **rows,
                                rows2=tuple(row_paths2),
                                gzip_rows2=[k for k, p in row_paths2.items() if p.endswith(".gz")])
         routes = [gzip_route(p) for p in args.inputs]
@@ -449,7 +472,7 @@ def main():
         # every demultiplexed output, "unknown" included, is compressed alike
         if args.untrimmed_output and args.untrimmed_output.endswith(".gz") != args.output.endswith(".gz"):
             ap.error("with demultiplexing, --untrimmed-output must be compressed (.gz) exactly when the -o template is")
-        t = FastqTrimmer(ads1, **common, **formats, **revcomp1, gzip_outputs=gzip1, **rows)
+        t = FastqTrimmer(ads1, **common, **formats, **revcomp1, **names, gzip_outputs=gzip1, **rows)
         files = {}
         f, chunks = single_input(t)
         with f:
@@ -468,7 +491,7 @@ def main():
             fh.close()
         stats = t.statistics
     elif redirect:
-        t = FastqTrimmer(ads1, **common, **formats, **revcomp1, **split, gzip_outputs=gzip1, **rows)
+        t = FastqTrimmer(ads1, **common, **formats, **revcomp1, **names, **split, gzip_outputs=gzip1, **rows)
         f, chunks = single_input(t)
         with f:
             files = {d: OutputFile(getattr(args, d + "_output")) for d in redirect}
@@ -481,7 +504,7 @@ def main():
                 fh.close()
         stats = t.statistics
     else:
-        t = FastqTrimmer(ads1, **common, **formats, **revcomp1, gzip_outputs=gzip1, **rows)
+        t = FastqTrimmer(ads1, **common, **formats, **revcomp1, **names, gzip_outputs=gzip1, **rows)
         o = OutputFile(args.output)
         f, chunks = single_input(t)
         with f:
